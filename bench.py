@@ -1,12 +1,14 @@
 #!/usr/bin/env python3
-"""bench.py -- UIS-RNN predict() throughput on B200 (BASELINE.json metric).
+"""bench.py -- UIS-RNN predict() throughput on H100 (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path
+  python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a path
   python bench.py --impl reference --gpus N --steps K ...  # reference CPU arm (host cores)
 
 A "step" is one predict() pass over one batch of synthetic utterances (BASELINE config 2:
 500-frame 256-d utterances, hidden 512, beam_size 10, look_ahead 1, test_iteration 2).
 Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for the definitions.
+--dump-outputs DIR writes the labels of the last timed step as DIR/labels.npy (float64; one file per rank,
+labels_rank<r>.npy, when N > 1); the inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -29,9 +31,7 @@ WORKLOAD = ('configs[1]: predict() synthetic 256-d d-vectors, 500-frame utteranc
             'beam_size=10, look_ahead=1, test_iteration=2')
 MODEL_FIXTURE = os.path.join(ROOT, 'tests', 'golden', 'model_toy100.npz')
 FIRST_SEED = 100000          # utterance i of the workload = synth_utt(FIRST_SEED + i)
-STRONG_UTTS = 888            # fixed list of the strong-scaling side measurement (utterances 0..887 of the job)
-MMA_FLOOR_CYCLES = 86.4      # measured: cycles per 128 x N x 16 kind::f16 MMA fed from shared memory, N <= 128
-                             # (tools/tc/tc_chain_probe.cu, profiles/r2_tc_chain_probe_uniform_issue.txt)
+STRONG_UTTS = 792            # fixed list of the strong-scaling side measurement (utterances 0..791 of the job)
 
 
 def synth_batch(first_seed, n_utt, pinned=False):
@@ -108,22 +108,8 @@ def load_peaks():
     return {'hbm_gbs': float(d['hbm_gbs']), 'tensor_tflops': float(d['bf16_tflops']),
             'tensor_tflops_sustained': float(d.get('bf16_tflops_sustained', d['bf16_tflops'])),
             'sm_max_mhz': float(d.get('sm_max_mhz', 1965.0)), 'source': 'measured (MEASURED_PEAKS.json)'}
-  return {'hbm_gbs': 6650.0, 'tensor_tflops': 1590.0, 'tensor_tflops_sustained': 1400.0, 'sm_max_mhz': 1965.0,
-          'source': 'fallback (B200_PROFILING.md)'}
-
-
-def measured_traffic(utts, engine):
-  """DRAM bytes per launch of the beam kernel from the committed ncu capture of THIS build's kernel on THIS
-  workload size (profiles/r3_traffic.json); None when the capture does not match what was just run."""
-  path = os.path.join(ROOT, 'profiles', 'r3_traffic.json')
-  try:
-    with open(path) as f:
-      d = json.load(f)
-    if d['utterances'] == utts and d['frames_per_utterance'] == N_FRAMES and d['engine'] == engine:
-      return d['dram_bytes_read'] + d['dram_bytes_write'], d.get('l2_to_sm_bytes')
-  except Exception:  # pylint: disable=broad-except
-    pass
-  return None, None
+  return {'hbm_gbs': 3350.0, 'tensor_tflops': 989.0, 'tensor_tflops_sustained': 989.0, 'sm_max_mhz': 1980.0,
+          'source': 'H100 SXM data sheet (700 W; dense fp16)'}
 
 
 def host_info():
@@ -204,9 +190,9 @@ def secondary_metrics(model, torch):
     tr.close()
   except Exception as err:  # pylint: disable=broad-except
     out['config4_fit_batch32'] = {'error': str(err)[:200]}
-  try:  # config 3: beam_size=30, look_ahead=2 (wide-beam stress), device-resident, 148 x 100 frames
+  try:  # config 3: beam_size=30, look_ahead=2 (wide-beam stress), device-resident, 132 x 100 frames
     from uisrnn_b200.synth import synth_utt
-    U3, N3 = 148, 100
+    U3, N3 = 132, 100
     x3 = torch.from_numpy(np.concatenate([synth_utt(1000 + u, n_frames=N3, dim=DIM)[0] for u in range(U3)]).astype(np.float32)).cuda()
     lab3 = torch.empty(U3 * N3, dtype=torch.int32, device='cuda')
     off3 = np.arange(U3 + 1, dtype=np.int64) * N3
@@ -219,7 +205,7 @@ def secondary_metrics(model, torch):
     out['config3_beam30_lookahead2'] = {'error': str(err)[:200]}
   try:  # SURVEY 8(d): latency mode (U=1), small batches and the FFMA engine on the bench batch, device-resident
     from uisrnn_b200.synth import synth_utt
-    for U1, engine in ((1, 0), (64, 0), (296, 1)):
+    for U1, engine in ((1, 0), (64, 0), (264, 1)):
       xs = torch.from_numpy(np.concatenate([synth_utt(1000 + u, n_frames=N_FRAMES, dim=DIM)[0] for u in range(U1)]).astype(np.float32)).cuda()
       lab = torch.empty(U1 * N_FRAMES, dtype=torch.int32, device='cuda')
       offs = np.arange(U1 + 1, dtype=np.int64) * N_FRAMES
@@ -324,7 +310,7 @@ def partition_secondary(api_model, iargs, rank, world, torch, dist, barrier):
 
 def _ref_worker(job):
   """One process of the CPU legs: decodes the first `n_frames` frames of workload utterance `seed` with the
-  unmodified reference (kind 'reference': baseline/_ref through its public predict()), the reference on a CUDA
+  unmodified reference (kind 'reference': oracle/_ref through its public predict()), the reference on a CUDA
   device ('reference_cuda') or the oracle port; returns (seconds, labels)."""
   kind, weights_path, seed, n_frames, threads = job
   import torch
@@ -333,9 +319,9 @@ def _ref_worker(job):
   from uisrnn_b200.synth import synth_utt
   x = synth_utt(seed, n_frames=N_FRAMES, dim=DIM)[0][:n_frames]
   if kind in ('reference', 'reference_cuda'):
-    sys.path[:0] = [os.path.join(ROOT, 'oracle', 'shims'), os.path.join(ROOT, 'baseline', '_ref')]
+    sys.path[:0] = [os.path.join(ROOT, 'oracle', 'shims'), os.path.join(ROOT, 'oracle', '_ref')]
     import uisrnn as ref
-    assert 'baseline' in ref.__file__
+    assert os.path.join('oracle', '_ref') in ref.__file__
     argv, sys.argv = sys.argv, [sys.argv[0]]
     try:
       margs, _, iargs = ref.parse_arguments()
@@ -372,7 +358,7 @@ def _ref_worker(job):
 
 
 def have_reference():
-  return os.path.exists(os.path.join(ROOT, 'baseline', '_ref', 'uisrnn', 'uisrnn.py'))
+  return os.path.exists(os.path.join(ROOT, 'oracle', '_ref', 'uisrnn', 'uisrnn.py'))
 
 
 def run_in_fresh_process(jobs, procs=1):
@@ -384,7 +370,7 @@ def run_in_fresh_process(jobs, procs=1):
 
 def cpu_baseline_and_parity(gpu_labels_of):
   """(a) cpu_baseline: SURVEY 8(d)(i), the unmodified reference in ONE process with the default torch threads on a
-  bounded sample (2 slices x 40 frames of workload utterances; the oracle port if baseline/_ref is absent);
+  bounded sample (2 slices x 40 frames of workload utterances; the oracle port if oracle/_ref is absent);
   (b) parity: full 500-frame utterances of the timed batch decoded by the oracle port -- the checker -- and compared
   with the labels the GPU produced for the same utterances."""
   import torch
@@ -402,7 +388,7 @@ def cpu_baseline_and_parity(gpu_labels_of):
          'sample': '%d slice x %d frames of a workload utterance (seed %d), one process, %d torch threads (default %d, '
                    'usable cores %d), %s; %.1f s in predict(), %.1f s with start-up' % (
                        n_slices, slice_frames, FIRST_SEED, threads, torch.get_num_threads(), host_info()['usable_cores'],
-                       'unmodified reference predict() from baseline/_ref' if kind == 'reference' else 'oracle/uis_oracle.py port',
+                       'unmodified reference predict() from oracle/_ref' if kind == 'reference' else 'oracle/uis_oracle.py port',
                        busy, wall)}
   # parity: utterances of the batch at their whole length (the reference-decoded ones are checked separately)
   which = sorted(gpu_labels_of.keys())
@@ -448,7 +434,7 @@ def run_reference(args):
   value = frames * len(times) / total
   sample = ('%d processes x 1 utterance slice of %d frames per step (the workload generator and seeds of the GPU arm), '
             '%s, 1 torch thread per process; calibration step with 16-frame slices: %.1f s' % (
-                procs, n_frames, 'unmodified reference predict() from baseline/_ref' if kind == 'reference'
+                procs, n_frames, 'unmodified reference predict() from oracle/_ref' if kind == 'reference'
                 else 'oracle/uis_oracle.py port', t16))
   secondary = {}
   try:  # SURVEY 8(d)(i): one process, default torch threads
@@ -508,7 +494,7 @@ def run_b200(args):
   rank = int(os.environ.get('RANK', '0'))
   local = int(os.environ.get('LOCAL_RANK', '0'))
   if not torch.cuda.is_available():
-    raise SystemExit('bench.py: no CUDA device; the sm_100a path cannot run (no CPU fallback by design)')
+    raise SystemExit('bench.py: no CUDA device; the sm_90a path cannot run (no CPU fallback by design)')
   torch.cuda.set_device(local)
   if world > 1:
     dist.init_process_group('nccl', device_id=torch.device('cuda', local))
@@ -598,6 +584,10 @@ def run_b200(args):
   assert np.array_equal(np.concatenate([np.asarray(o, dtype=np.int32) for o in got_mine]), labels_first), \
       'e2e and device-resident legs disagree'
   e2e_stats = api_model._native_model().stats()  # pylint: disable=protected-access
+  if args.dump_outputs:
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    name = 'labels.npy' if world == 1 else 'labels_rank%d.npy' % rank
+    np.save(os.path.join(args.dump_outputs, name), labels_first.astype(np.float64))
 
   t = torch.tensor([dev_ms, e2e_s * 1e3], dtype=torch.float64, device='cuda')
   if world > 1:
@@ -638,7 +628,7 @@ def run_b200(args):
   steps_per_launch = TEST_ITER * N_FRAMES
   # SURVEY 8(d): per beam-step "launch" over U utterances: the 6.3 MB weight set once + U * (4*D*L + 8*L) bytes
   hbm_alg = steps_per_launch * (4 * (3 * H * D + 3 * H * H + 6 * H + H * H + H + D * H + D) + U * (4 * D + 8))
-  traffic, l2_to_sm = measured_traffic(U, engine)
+  traffic = None  # no DRAM capture of this kernel is stored with the project
   wbytes_pass = 4 * (3 * H * H + H * H + H * D)             # W_hh, W1, W2 (fp32, or fp16 hi + lo planes): streamed once per pass
   roof = {
       'kernel': 'uis_beam_kernel<512,256,tensor-core %d columns>' % st['tc_columns'] if engine == 2 else 'uis_beam_kernel<512,256> (FFMA)',
@@ -647,8 +637,7 @@ def run_b200(args):
       'hbm': {'algorithmic_bytes': hbm_alg, 'achieved_gbs': hbm_alg / beam_s / 1e9, 'peak_gbs': peaks['hbm_gbs'],
               'frac': hbm_alg / beam_s / 1e9 / peaks['hbm_gbs'], 'traffic': traffic,
               'note': 'SURVEY 8(d): weights once per beam step + per-frame I/O; the weights stay L2-resident, so this is not '
-                      'the binding resource (traffic = ncu dram bytes of the committed capture of this kernel and batch size, '
-                      'profiles/r3_traffic.json; null if none matches)'},
+                      'the binding resource'},
       'l2_to_sm_bytes': st['weight_passes'] * wbytes_pass,
       'fp32_fma_equivalent': {'achieved_tflops': flops / beam_s / 1e12, 'peak_tflops': fp32_peak,
                               'frac': flops / beam_s / 1e12 / fp32_peak, 'sm_mhz_used': sm_mhz,
@@ -656,24 +645,17 @@ def run_b200(args):
                                       'yardstick; the tensor-core engine can exceed 1'},
   }
   if engine == 2:
-    mma_per_pass = (3 * H + H + D) // 128 * (H // 64) * 2 * 4      # tiles x k atoms x planes x k steps
+    mma_per_pass = (3 * H + H + D) // 128 * (H // 64) * 2 * 4      # 128-row tiles x k atoms x planes x k steps
     np_cols = 2 * st['tc_columns']
     issued = st['weight_passes'] * mma_per_pass * 2.0 * 128 * np_cols * 16
-    kernel_cycles = beam_s * sm_mhz * 1e6
     roof.update({
         'bound': 'tensor', 'unit': 'TFLOP/s', 'achieved': flops / beam_s / 1e12, 'peak': peaks['tensor_tflops'],
         'frac': flops / beam_s / 1e12 / peaks['tensor_tflops'], 'traffic': traffic,
         'issued_tflops': issued / beam_s / 1e12,
-        'mma_slot': {'mma_per_pass': mma_per_pass, 'floor_cycles_per_mma': MMA_FLOOR_CYCLES,
-                     'frac': st['weight_passes'] * mma_per_pass * MMA_FLOOR_CYCLES / (kernel_cycles * st['ctas']),
-                     'issuer_us_per_pass': {k: v / (sm_mhz) / max(1, st['weight_passes']) for k, v in zip(
-                         ('stall_tma', 'stall_epilogue', 'stall_operand', 'issue'), st['tc_cycles'])},
-                     'note': 'share of the kernel the tensor pipe is busy at its measured per-instruction floor: a 128 x N x 16 '
-                             'MMA fed from shared memory costs 86.4 cycles for ANY N <= 128 (tools/tc/tc_chain_probe.cu), '
-                             'so with <= 48 live columns per pass the pipe is instruction-bound, not flop-bound: `frac` of '
-                             'the dense fp16 peak stays small by construction'},
+        'pass_us_per_pass': {k: v / (sm_mhz) / max(1, st['weight_passes']) for k, v in zip(
+            ('wait_tma', 'wait_mma', 'stage_b_operand', 'pass'), st['tc_cycles'])},
         'note': 'achieved = useful fp32-grade flops (each runs as 4 fp16 products: hi/lo split of both operands, see '
-                'issued_tflops for what the pipe executes, padding included); peak = measured dense bf16/fp16 (burst)'})
+                'issued_tflops for what the pipe executes, padding included); peak = dense fp16 (peak_source)'})
   else:
     roof.update({'bound': 'fp32_fma', 'unit': 'TFLOP/s', 'achieved': flops / beam_s / 1e12, 'peak': fp32_peak,
                  'frac': flops / beam_s / 1e12 / fp32_peak, 'traffic': traffic})
@@ -683,7 +665,7 @@ def run_b200(args):
       'dtype': 'f32', 'data': 'synthetic',
       'config': {'workload': WORKLOAD, 'utterances_per_gpu_per_step': U, 'frames_per_gpu_per_step': frames,
                  'model': 'D=256 H=512 depth=1, weights = reference fit() 100 it on toy data (tests/golden/model_toy100.npz)',
-                 'engine': {1: 'fp32 FFMA kernels', 2: 'tcgen05 tensor-core pass (fp16 hi/lo split operands, fp32-grade)'}[engine],
+                 'engine': {1: 'fp32 FFMA kernels', 2: 'wgmma tensor-core pass (fp16 hi/lo split operands, fp32-grade)'}[engine],
                  'lanes_per_cta': st['lanes'],
                  'parallelism': 'utterance list of %d x %d sharded by frame count over %d rank(s) (shard_by_frames), '
                                 'no data-path collective' % (world, U, world),
@@ -737,11 +719,12 @@ def main():
   ap.add_argument('--steps', type=int, default=5)
   ap.add_argument('--warmup', type=int, default=3)
   ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
-  ap.add_argument('--utts', type=int, default=888, help='utterances per GPU per step (6 lanes x 148 CTAs)')
+  ap.add_argument('--utts', type=int, default=792, help='utterances per GPU per step (6 lanes x 132 CTAs)')
   ap.add_argument('--engine', type=int, default=0, help='0 auto (tensor cores), 1 FFMA kernels, 2 tensor cores')
   ap.add_argument('--no-cpu-baseline', action='store_true')
   ap.add_argument('--pageable', action='store_true', help='e2e leg from ordinary (pageable) numpy arrays instead of pinned ones')
   ap.add_argument('--no-secondary', action='store_true', help='skip the config-3 / config-4 side measurements')
+  ap.add_argument('--dump-outputs', metavar='DIR', help='write the labels of the last timed step to DIR/labels.npy')
   args = ap.parse_args()
   if args.impl == 'reference':
     run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * uisrnn_b200.h -- C ABI of libuisrnn_b200.so: the B200 (sm_100a) implementation of UIS-RNN's
+ * uisrnn_b200.h -- C ABI of libuisrnn_b200.so: the H100 (sm_90a) implementation of UIS-RNN's
  * predict() hot path (beam search over GRU hypotheses).
  *
  * The reference (google/uis-rnn) has NO native / FFI layer (SURVEY.md 2.2): its only boundary
@@ -32,7 +32,7 @@ extern "C" {
 typedef enum uis_status {
   UIS_OK = 0,
   UIS_ERR_INVALID = -1,     /* bad argument (shape, NULL, beam_size < 1, ...)                  */
-  UIS_ERR_UNSUPPORTED = -2, /* shape / option the sm_100a kernels are not instantiated for     */
+  UIS_ERR_UNSUPPORTED = -2, /* shape / option the sm_90a kernels are not instantiated for      */
   UIS_ERR_CUDA = -3,        /* a CUDA runtime call failed; uis_last_error() has the string     */
   UIS_ERR_OVERFLOW = -4,    /* a hypothesis opened more than `kcap` clusters; retry with more  */
   UIS_ERR_NOMEM = -5,
@@ -60,7 +60,7 @@ typedef struct uis_predict_opts {
                              shared memory of 32 CTAs, products split by rows, cooperative launch)         */
   int32_t engine;         /* matrix engine of the look_ahead-1 beam kernel: 0 = auto (tensor cores
                              when some CTA gets more than one utterance), 1 = fp32 FFMA kernels,
-                             2 = tcgen05 tensor-core pass (fp16 hi/lo split operands, fp32-grade;
+                             2 = wgmma tensor-core pass (fp16 hi/lo split operands, fp32-grade;
                              depth 1, hidden/dim multiples of 128; kcap defaults to 16)          */
 } uis_predict_opts;
 
@@ -101,9 +101,9 @@ typedef struct uis_stats {
   int64_t phase_cycles[10]; /* SM cycles summed over CTAs: [0] re-pack (P4), [1] gather, [2] GRU pass,
                                [3] W1 pass, [4] W2 pass, [5] advance/back-track, [6] frame landing
                                (P0), [7] scoring (P1), [8] ranking (P2), [9] column/slot assignment (P3) */
-  int64_t tc_cycles[4];     /* tensor-core pass, SM cycles of the MMA-issuing thread summed over CTAs: stalled on [0] a
-                               weight box not yet landed (TMA), [1] an accumulator slot not yet drained (epilogue),
-                               [2] the B operand of the next product; [3] inside passes (first operand ready -> last issue) */
+  int64_t tc_cycles[4];     /* tensor-core pass, SM cycles of consumer thread 0 summed over CTAs: waiting for [0] a
+                               weight box not yet landed (TMA), [1] MMAs to complete; [2] staging the B operands;
+                               [3] inside passes */
   /* host-buffer entry point (uis_predict) only, ABI 4: */
   float h2d_ms;             /* span of the chunked host->device copies on the copy stream                              */
   float pipeline_ms;        /* compute stream: first cast kernel -> start of the beam kernel (casts + input projections,

@@ -77,7 +77,7 @@ def test_synth500_in_cluster_mode(toy_model):
 
 
 def test_stationary_weights_mode_reproduces_reference_labels(toy_model):
-  """cluster=32: all 25 toy utterances through groups of 32 CTAs (4 groups on a 148-SM device take them in turn)."""
+  """cluster=32: all 25 toy utterances through groups of 32 CTAs (4 groups on a 132-SM device take them in turn)."""
   xs, labs = toy_utterances()
   got = toy_model.predict(xs, cluster=32)
   st = toy_model.stats()

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a path, called through the C ABI (ctypes -> libuisrnn_b200.so),
+"""GPU parity tests: the sm_90a path, called through the C ABI (ctypes -> libuisrnn_b200.so),
 against (a) golden vectors produced by the unmodified reference and (b) the CPU oracle on fresh
 seeded inputs.  Labels must be identical; scores within 1e-5 relative; GRU hidden states and
 running means within 1e-5 absolute (BASELINE.md section 3.4)."""

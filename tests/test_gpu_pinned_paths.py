@@ -8,7 +8,7 @@ Variants are forced through the C ABI's `lanes` / `cluster` options (`include/ui
   lanes=1 cluster=-1   the same kernel, one utterance per CTA
   lanes=0 cluster=0    automatic choice (few utterances -> thread-block-cluster kernel)
   lanes=0 cluster=32   stationary-weights mode (groups of 32 CTAs, weights resident in shared memory)
-  engine=2             the tensor-core pass (tcgen05): tests/test_gpu_tensorcore.py
+  engine=2             the tensor-core pass (wgmma): tests/test_gpu_tensorcore.py
 """
 import numpy as np
 import pytest

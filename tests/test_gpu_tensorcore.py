@@ -1,5 +1,5 @@
-"""The tensor-core engine of the look_ahead-1 beam kernel (`engine=2`: tcgen05 MMAs over fp16 hi/lo split operands,
-TMEM accumulators, tensor-map TMA -- uisrnn_b200/csrc/uis_beam_tc.cuh) against the same pins as the FFMA kernels:
+"""The tensor-core engine of the look_ahead-1 beam kernel (`engine=2`: wgmma MMAs over fp16 hi/lo split operands,
+register accumulators, tensor-map TMA -- uisrnn_b200/csrc/uis_beam_tc.cuh) against the same pins as the FFMA kernels:
 labels produced by the unmodified reference (toy test set, 500-frame utterances of bench.py's workload), per-step
 winners / scores / final hidden states of the reference's own trace (scores 1e-5 relative, states 1e-5 absolute,
 BASELINE.md section 3.4), and the CPU oracle on the other tileable shape (256, 128)."""

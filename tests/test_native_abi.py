@@ -1,4 +1,4 @@
-"""The C-ABI shared library: builds for sm_100a without a GPU, loads, and exports every symbol
+"""The C-ABI shared library: builds for sm_90a without a GPU, loads, and exports every symbol
 include/uisrnn_b200.h declares.  No compute calls here (CPU only)."""
 import ctypes
 import os
@@ -55,8 +55,8 @@ def test_invalid_arguments_are_rejected_without_a_gpu(lib):
   assert cdll.uis_model_destroy(None) == 0
 
 
-def test_sass_uses_tma_and_packed_fma():
-  """The hot kernel must contain TMA bulk copies (UBLKCP), mbarrier ops (SYNCS) and FFMA2."""
+def test_sass_uses_tma_and_register_rebalancing():
+  """The hot kernel must contain TMA bulk copies (UBLKCP) and mbarrier ops (SYNCS)."""
   import shutil
   import subprocess
   tool = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
@@ -64,16 +64,15 @@ def test_sass_uses_tma_and_packed_fma():
     pytest.skip('cuobjdump not available')
   from uisrnn_b200 import native
   sass = subprocess.run([tool, '-sass', native.LIB_PATH], capture_output=True, text=True).stdout
-  assert 'UBLKCP' in sass and 'SYNCS' in sass and 'FFMA2' in sass
+  assert 'UBLKCP' in sass and 'SYNCS' in sass
   # register re-balancing of the warp-specialised CTA, and the cluster (latency) mode: cluster barrier at start-up,
   # remote mbarrier arrives (the .RED form) for the distributed-shared-memory exchange
   assert 'USETMAXREG' in sass and 'UCGABAR_ARV' in sass and 'SYNCS.ARRIVE.TRANS64.RED' in sass
 
 
-def test_sass_uses_tcgen05_tmem_and_tensor_map_tma():
-  """The tensor-core engine must be the real thing: tcgen05.mma (UTCHMMA), TMEM loads (LDTM) and tensor-map TMA
-  (UTMALDG) inside the uis_beam_kernel<.., columns> instantiations -- B200_PROFILING.md, "What proves a
-  Blackwell-native kernel"."""
+def test_sass_uses_wgmma_and_tensor_map_tma():
+  """The tensor-core engine must be the real thing: warpgroup MMAs (HGMMA, with the WARPGROUP fences and waits around
+  them) and tensor-map TMA (UTMALDG) inside the uis_beam_kernel<.., columns> instantiations."""
   import shutil
   import subprocess
   tool = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
@@ -85,5 +84,5 @@ def test_sass_uses_tcgen05_tmem_and_tensor_map_tma():
   assert start >= 0, 'tensor-core instantiation missing'
   end = sass.find('Function :', start + 10)
   body = sass[start:end if end > 0 else len(sass)]
-  for mnemonic in ('UTCHMMA', 'LDTM', 'UTMALDG', 'UTCBAR'):
+  for mnemonic in ('HGMMA.64x96x16.F32', 'WARPGROUP', 'UTMALDG', 'SYNCS'):
     assert mnemonic in body, mnemonic

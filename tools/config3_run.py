@@ -3,7 +3,7 @@ import sys, os, numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from uisrnn_b200 import native
 from uisrnn_b200.synth import synth_utt
-U = int(sys.argv[1]) if len(sys.argv) > 1 else 148
+U = int(sys.argv[1]) if len(sys.argv) > 1 else 132
 N = int(sys.argv[2]) if len(sys.argv) > 2 else 100
 beam = int(sys.argv[3]) if len(sys.argv) > 3 else 30
 la = int(sys.argv[4]) if len(sys.argv) > 4 else 2

@@ -47,8 +47,8 @@ def predict(U, **kw):
   lab = torch.empty(U * 500, dtype=torch.int32, device='cuda')
   model.predict_device(x.data_ptr(), np.arange(U + 1, dtype=np.int64) * 500, lab.data_ptr(), **kw)
   return model.stats()
-predict(296, engine=1); fit_loop('after FFMA beam kernel (U=296)')
+predict(264, engine=1); fit_loop('after FFMA beam kernel (U=264)')
 predict(1); fit_loop('after cluster beam kernel (U=1)')
 predict(300, engine=2); fit_loop('after tensor-core beam kernel (U=300)')
-predict(148, beam_size=30, look_ahead=2); fit_loop('after look-ahead tree kernel')
+predict(132, beam_size=30, look_ahead=2); fit_loop('after look-ahead tree kernel')
 fit_loop('100 iterations', iters=100)

@@ -12,7 +12,7 @@ for U in (1, 2, 4, 8, 32, 64):
   off = np.arange(U + 1, dtype=np.int64) * N
   ref = None
   for cluster in (-1, 0, 2, 4, 8, 32):
-    if cluster > 0 and cluster < 32 and U * cluster > 148:
+    if cluster > 0 and cluster < 32 and U * cluster > 132:
       continue
     if cluster == 32 and U > 8:
       continue

@@ -1,5 +1,5 @@
 """A/B of the beam-kernel engines on bench.py's workload (device-resident): frames/s, kernel ms, phase shares.
-  python tools/tc_bench.py [U ...]      e.g.  python tools/tc_bench.py 296 888
+  python tools/tc_bench.py [U ...]      e.g.  python tools/tc_bench.py 264 792
 Environment: UISRNN_B200_TC_N=32|48 selects the columns per tensor-core pass."""
 import json
 import os
@@ -19,7 +19,7 @@ def main():
   from uisrnn_b200.synth import synth_utt
   native.load_library()
   model = native.NativeModel(dict(np.load(os.path.join(ROOT, 'tests', 'golden', 'model_toy100.npz'))))
-  sizes = [int(a) for a in sys.argv[1:]] or [296, 888]
+  sizes = [int(a) for a in sys.argv[1:]] or [264, 792]
   n_frames = int(os.environ.get('TC_BENCH_FRAMES', '500'))
   umax = max(sizes)
   xs = np.concatenate([synth_utt(100000 + u, n_frames=n_frames)[0] for u in range(umax)]).astype(np.float32)
@@ -50,10 +50,10 @@ def main():
             'passes': st['weight_passes'], 'labels_equal_ffma': bool(np.array_equal(got, ref.get(U, got))),
             'mismatching_frames': int((got != ref.get(U, got)).sum()),
             'phase_share': {n: round(c / tot, 3) for n, c in zip(PHASES, st['phase_cycles'])},
-            'phase_us_per_cta_step': {n: round(c / 1965.0 / max(1, st['beam_steps'] / max(1, st['lanes'])), 2)
+            'phase_us_per_cta_step': {n: round(c / 1980.0 / max(1, st['beam_steps'] / max(1, st['lanes'])), 2)
                                       for n, c in zip(PHASES, st['phase_cycles'])},
-            'mma_issuer_us_per_pass': {n: round(c / 1965.0 / max(1, st['weight_passes']), 2) for n, c in
-                                       zip(['stall_tma', 'stall_epilogue', 'stall_operand', 'pass_issue'], st['tc_cycles'])}}),
+            'tc_pass_us_per_pass': {n: round(c / 1980.0 / max(1, st['weight_passes']), 2) for n, c in
+                                    zip(['wait_tma', 'wait_mma', 'stage_b_operand', 'pass'], st['tc_cycles'])}}),
               flush=True)
 
 

@@ -1,5 +1,5 @@
 """Drop-in alias: `import uisrnn` gives the public surface of google/uis-rnn
-(`/root/reference/uisrnn/__init__.py:21-30`) backed by the B200-native package `uisrnn_b200`.
+(its `uisrnn/__init__.py:21-30`) backed by the H100-native package `uisrnn_b200`.
 Sub-modules (`uisrnn.uisrnn`, `uisrnn.utils`, `uisrnn.evals`, `uisrnn.loss_func`,
 `uisrnn.arguments`, `uisrnn.contrib.*`) resolve to the same module objects."""
 import sys as _sys

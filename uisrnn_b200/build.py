@@ -1,4 +1,4 @@
-"""Builds libuisrnn_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libuisrnn_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
 Staleness is decided by a content hash of the sources (a sidecar file next to the library), not
 by mtimes -- the tree is copied to the GPU box, which does not preserve a meaningful mtime order --
@@ -19,7 +19,7 @@ SOURCES = ['uis_api.cu', 'uis_train.cu', 'uis_kernels_beam_large.cu', 'uis_kerne
            'uis_kernels_tree_large.cu', 'uis_kernels_tree_small.cu']
 DEPS = SOURCES + ['uis_beam.cuh', 'uis_beam_tc.cuh', 'uis_beam_stat.cuh', 'uis_beam_tree.cuh', 'uis_prepass.cuh', 'uis_common.cuh', 'uis_launch.cuh',
         os.path.join('..', '..', 'include', 'uisrnn_b200.h')]
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-shared', '-Xcompiler', '-fPIC', '--threads', '0']
 
 

@@ -208,7 +208,7 @@ int dispatch_tree(int H, int D, const uis::BeamParams& p, int ctas, cudaStream_t
                 p.B, p.Kcap, smem);
   cudaError_t e = cudaSuccess;
   if (!uis::launch_tree_large(H, D, p, ctas, smem, st, &e) && !uis::launch_tree_small(H, D, p, ctas, smem, st, &e))
-    return fail(UIS_ERR_UNSUPPORTED, "no sm_100a kernel instantiated for hidden=%d dim=%d", H, D);
+    return fail(UIS_ERR_UNSUPPORTED, "no sm_90a kernel instantiated for hidden=%d dim=%d", H, D);
   if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "look-ahead kernel launch failed: %s", cudaGetErrorString(e));
   return 0;
 }
@@ -238,7 +238,7 @@ int dispatch_beam(int H, int D, const uis::BeamParams& p, int ctas, int* cluster
                 p.B, p.Kcap, p.G, smem);
   cudaError_t e = cudaSuccess;
   if (!uis::launch_beam_large(H, D, p, ctas, smem, st, &e) && !uis::launch_beam_small(H, D, p, ctas, smem, st, &e))
-    return fail(UIS_ERR_UNSUPPORTED, "no sm_100a kernel instantiated for hidden=%d dim=%d", H, D);
+    return fail(UIS_ERR_UNSUPPORTED, "no sm_90a kernel instantiated for hidden=%d dim=%d", H, D);
   if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "beam kernel launch failed: %s", cudaGetErrorString(e));
   return 0;
 }
@@ -278,7 +278,7 @@ float tc_pow2_scale(double bound) {
   return std::ldexp(1.0f, e);
 }
 
-// Splits w * scale into fp16 hi + lo (22 significant bits) -- the A operand planes of the tcgen05 pass.
+// Splits w * scale into fp16 hi + lo (22 significant bits) -- the A operand planes of the wgmma pass.
 void tc_split(const std::vector<float>& w, float scale, __half* hi, __half* lo) {
   for (size_t i = 0; i < w.size(); ++i) {
     const float v = w[i] * scale;
@@ -771,7 +771,7 @@ int uis_model_create(uis_model** out, int device, int D, int H, int depth, const
   if (!w_ih || !w_hh || !b_ih || !b_hh || !w1 || !b1 || !w2 || !b2 || !h0 || !sigma2)
     return fail(UIS_ERR_INVALID, "NULL weight pointer");
   if (depth < 1 || depth > uis::kMaxDepth)
-    return fail(UIS_ERR_UNSUPPORTED, "rnn_depth=%d: the sm_100a kernels support 1..%d stacked GRU layers", depth, uis::kMaxDepth);
+    return fail(UIS_ERR_UNSUPPORTED, "rnn_depth=%d: the sm_90a kernels support 1..%d stacked GRU layers", depth, uis::kMaxDepth);
   if (D < 1 || H < 1) return fail(UIS_ERR_INVALID, "observation_dim and rnn_hidden_size must be >= 1");
   if ((H > 512 || D > 256) && depth > 1)
     return fail(UIS_ERR_UNSUPPORTED, "hidden=%d dim=%d with rnn_depth=%d: models above hidden=512 / dim=256 run with one GRU layer", H, D, depth);
@@ -783,7 +783,7 @@ int uis_model_create(uis_model** out, int device, int D, int H, int depth, const
   for (auto& sh : shapes)
     if (!Hp && H <= sh[0] && D <= sh[1]) { Hp = sh[0]; Dp = sh[1]; }
   if (!Hp)
-    return fail(UIS_ERR_UNSUPPORTED, "hidden=%d dim=%d: the sm_100a kernels hold models up to hidden=1024 dim=512", H, D);
+    return fail(UIS_ERR_UNSUPPORTED, "hidden=%d dim=%d: the sm_90a kernels hold models up to hidden=1024 dim=512", H, D);
   uis::DeviceGuard device_guard_(device);
   CU(device_guard_.status);
   std::vector<float> v, p_wih((size_t)3 * Hp * Dp + (size_t)(depth - 1) * 3 * Hp * Hp, 0.f), p_whh((size_t)depth * 3 * Hp * Hp, 0.f),
@@ -1099,7 +1099,7 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
       if (!e) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     if (staged && !m->copy_pool) {
       const unsigned hw = std::max(1u, std::thread::hardware_concurrency());
-      int nthreads = (int)std::min(16u, std::max(2u, hw / 2));  // measured on the B200 box: 4 -> 40 ms, 8 -> 29 ms, 16 -> 23 ms for 909 MB
+      int nthreads = (int)std::min(16u, std::max(2u, hw / 2));  // more threads fill the staging ring faster
       if (const char* env = std::getenv("UISRNN_B200_COPY_THREADS")) nthreads = std::max(1, std::min(64, std::atoi(env)));
       m->copy_pool = new CopyPool(nthreads);
     }

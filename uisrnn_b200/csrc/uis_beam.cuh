@@ -1,4 +1,4 @@
-// Persistent beam-search kernel for UIS-RNN predict() on sm_100a  (look_ahead = 1, depth = 1).
+// Persistent beam-search kernel for UIS-RNN predict() on sm_90a  (look_ahead = 1, depth = 1).
 //
 // What it replaces (all under /root/reference/uisrnn/): the whole loop body of
 // UISRNN.predict_single (uisrnn.py:529-561) -- _calculate_score (:455-477), the np.sort/argsort
@@ -18,7 +18,7 @@
 //     R rows x 16 columns (R = 6 for the GRU gates, 4 for the MLP layers with the K dimension
 //     split over thread groups) so that each value fetched from shared memory feeds >= 3 FMAs:
 //     the shared-memory return path (one 32-bit register per lane per cycle per SM) -- not
-//     the FMA pipe -- is what bounds a skinny matvec batch otherwise (profiles/r1_v1_*).
+//     the FMA pipe -- is what bounds a skinny matvec batch otherwise.
 //   * hypothesis state is a slot pool in global memory (L2): slot = (mean[D], hidden[H]) written
 //     once and never modified; a hypothesis is a table of (slot, block count, visit count) per
 //     cluster held in shared memory.  A child differs from its parent in ONE table entry, so the
@@ -165,7 +165,7 @@ enum { LS_U = 0, LS_N, LS_TN, LS_T, LS_NB, LS_GEN, LS_ACTIVE, LS_FAILED, LS_TRAC
        LS_NWIN, LS_ERR, LS_M, LS_COLBASE, LS_NE, LS_ROW0_LO, LS_ROW0_HI, LS_DBGROWS_LO, LS_DBGROWS_HI,
        LS_FRESH, LS_COUNT = 24 };
 // CTA scalars
-enum { MI_PUBLISHED = 0, MI_DONE, MI_MTOT, MI_QNEXT, MI_NLIST, MI_MAXK, MI_TCEXIT };
+enum { MI_PUBLISHED = 0, MI_DONE, MI_MTOT, MI_QNEXT, MI_NLIST, MI_MAXK };
 
 template <int H, int D, int kCP = kCPBeam, bool XCL = false, int TCN = 0, bool STAT = false>
 __host__ __device__ inline SmemLayout make_layout(int B, int Kcap, int G) {
@@ -202,11 +202,11 @@ __host__ __device__ inline SmemLayout make_layout(int B, int Kcap, int G) {
   L.lanes = o;     o += L.lane_stride * G;
   L.cols = o;      o += align_up(6u * G * B * 4, 16);  // collane, colsrc, colnew, colvis, colrow (8 B each)
   L.bars = o;
-  if constexpr (TCN > 0) o += (2 * TcCfg<H, D, TCN>::STAGES + 2 * kTcSlots + 2) * 8;  // full, empty, tfull, tempty, bready, TMEM base
+  if constexpr (TCN > 0) o += 2 * TcCfg<H, D, TCN>::STAGES * 8;  // full, empty
   else o += 2 * kStages * 8;
   L.misc = o;      o += 64;
   L.slist = o;     o += 4u * 64u * G;  // (lane, slot) work list of the per-slot scoring
-  L.phase = o;     o += 128 + 32;  // thread 0's statistics: 10 phase cycle counters, phase mark, 5 counters; MMA issuer: 4 stall counters
+  L.phase = o;     o += 128 + 32;  // thread 0's statistics: 10 phase cycle counters, phase mark, 5 counters, 4 tensor-core pass counters
   L.xch = o; L.xbar = o;
   if (XCL) {  // cluster K-split: two exchange buffers of kXchVals floats per consumer thread + 2 mbarriers
     o = align_up(o, 16);
@@ -305,7 +305,7 @@ __device__ __forceinline__ void lin_pass(const float* __restrict__ ring, uint64_
   auto tile_x = [&](int tile) -> const float4* {
     return reinterpret_cast<const float4*>(X + (size_t)(tile * KT + kg * KPG) * C::CP);
   };
-  // volatile ld.shared: keeps the loads of k-step s+1 AHEAD of the FFMA2s of k-step s in the
+  // volatile ld.shared: keeps the loads of k-step s+1 AHEAD of the FFMAs of k-step s in the
   // instruction stream (the compiler otherwise sinks them next to their first use, which
   // exposes the ~30-cycle shared-memory latency with only 2 warps per scheduler)
   auto load = [&](Operands<R, NC>& o, const float* wt, const float4* xp, int kq) {
@@ -323,17 +323,12 @@ __device__ __forceinline__ void lin_pass(const float* __restrict__ ring, uint64_
   auto mac = [&](const Operands<R, NC>& o) {
 #pragma unroll
     for (int c = 0; c < NC; ++c) {
-      const float2 xlo = make_float2(o.x[c].x, o.x[c].y), xhi = make_float2(o.x[c].z, o.x[c].w);
 #pragma unroll
-      for (int i = 0; i < R; ++i) {
-        // packed fp32 FMA (sm_100 FFMA2): two IEEE-RN fmas per instruction, w broadcast
-        const float2 w2 = make_float2(o.w[i], o.w[i]);
-        float2 a0 = make_float2(acc[i][4 * c + 0], acc[i][4 * c + 1]);
-        float2 a1 = make_float2(acc[i][4 * c + 2], acc[i][4 * c + 3]);
-        a0 = __ffma2_rn(xlo, w2, a0);
-        a1 = __ffma2_rn(xhi, w2, a1);
-        acc[i][4 * c + 0] = a0.x; acc[i][4 * c + 1] = a0.y;
-        acc[i][4 * c + 2] = a1.x; acc[i][4 * c + 3] = a1.y;
+      for (int i = 0; i < R; ++i) {  // IEEE-RN fmas, w broadcast over the 4 columns
+        acc[i][4 * c + 0] = __fmaf_rn(o.x[c].x, o.w[i], acc[i][4 * c + 0]);
+        acc[i][4 * c + 1] = __fmaf_rn(o.x[c].y, o.w[i], acc[i][4 * c + 1]);
+        acc[i][4 * c + 2] = __fmaf_rn(o.x[c].z, o.w[i], acc[i][4 * c + 2]);
+        acc[i][4 * c + 3] = __fmaf_rn(o.x[c].w, o.w[i], acc[i][4 * c + 3]);
       }
     }
   };
@@ -747,152 +742,138 @@ __device__ __forceinline__ void stat_pass(const BeamParams& p, const float* sW, 
   stat_group_sync<NT>(bar, epoch, tid);  // the next step scores against the new means / gathers the new hidden states
 }
 
-// ---- tensor-core weight pass (consumer warps' side; uis_beam_tc.cuh has the TMA producer and the MMA issuer) ----
-// Columns [m0, m0 + Mp), Mp <= N.  Thread <-> weight row: warp w reads TMEM lanes 32 * (w & 3) .. + 31 (the hardware
-// ties a warp to the lane quarter warp_id % 4) and takes the 8-column chunks of parity w >> 2.
+// ---- tensor-core weight pass (consumer warps' side; uis_beam_tc.cuh has the TMA producer and the MMA tiles) -----
+// Columns [m0, m0 + Mp), Mp <= N.  Warpgroup wg = warp / 4 multiplies rows 64 wg .. 64 wg + 63 of every 128-row tile;
+// its accumulator layout gives a thread rows r0 and r0 + 8 and the columns 8 i + 2 (lane % 4) + {0, 1}.
+// tstat: thread 0's pass counters ([0] box waits, [1] MMA waits, [2] B operand staging, [3] cycles inside passes).
 template <int H, int D, int N, class Idle>
-__device__ __forceinline__ void tc_run_pass(const BeamParams& p, unsigned char* bop, uint32_t tmem_base, const TcBars& tb,
-                                            unsigned& tcnt, const ColCtx cc, int m0, int Mp, float* pool_mean_cta,
-                                            float* pool_hidden_cta, float* scratch_cta, int tid, int lane, int warp,
-                                            long long* ph, long long& tmark, Idle idle_work) {
+__device__ __forceinline__ void tc_run_pass(const BeamParams& p, const unsigned char* ring, unsigned char* bop,
+                                            const TcBars& tb, unsigned& tbox, const ColCtx cc, int m0, int Mp,
+                                            float* pool_mean_cta, float* pool_hidden_cta, float* scratch_cta, int tid,
+                                            int lane, int warp, long long* ph, long long& tmark, long long* tstat,
+                                            Idle idle_work) {
   using TC = TcCfg<H, D, N>;
-  constexpr int NT = 256;
+  constexpr int NT = 256, NI = N / 8;
   const size_t lane_pool_h = (size_t)p.P * H, lane_pool_m = (size_t)p.P * D;
-  const int qd = warp & 3, hsel = warp >> 2;
-  const int r = qd * 32 + lane;
-  const uint32_t tlane = ((uint32_t)(qd * 32)) << 16;
-  auto tile_wait = [&](unsigned t) -> uint32_t {  // accumulator of tile t is complete -> its TMEM address for this warp
-    const unsigned slot = t % kTcSlots;
-    if (p.dbg_mode & 4) tc_mbar_wait(&tb.tfull[slot], (t / kTcSlots) & 1);   // experiment: spinning wait
-    else tc_mbar_wait_parked(&tb.tfull[slot], (t / kTcSlots) & 1);
-    return tmem_base + tlane + slot * TC::NP;
+  const int wg = warp >> 2;
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  long long* ts = (tid == 0) ? tstat : nullptr;
+  const long long t_in = clock64();
+  float acc[TC::NACC];
+  auto stage_b = [&](auto src, float scale) {
+    const long long w0 = clock64();
+    tc_gather_b<H, N, NT>(bop, src, Mp, scale, tid);
+    tc_publish_b<NT>();
+    if (ts) ts[2] += clock64() - w0;
   };
   // ---------------- B = h_src (fp16 hi / lo), then the GRU gates per 128-unit tile
-  tc_gather_b<H, N, NT>(bop, [&](int m) -> const float* {
-    return pool_hidden_cta + (size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.src[m0 + m] * H; }, Mp, p.tc_sh, tid);
-  tc_signal_b(tb.bready, lane);
+  stage_b([&](int m) -> const float* {
+    return pool_hidden_cta + (size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.src[m0 + m] * H; }, p.tc_sh);
   if (tid == 0) { const long long now_ = clock64(); ph[1] += now_ - tmark; tmark = now_; }
-  idle_work();  // the first accumulator tiles are ~10 us away: the consumer warps use the gap (next step's Gaussian terms)
+  idle_work();  // the next step's Gaussian terms (their frame has landed by now)
+  // (charged to the scoring phase: the TMA ring is already filled meanwhile, the MMAs wait for it)
+  if (tid == 0) { const long long now_ = clock64(); ph[7] += now_ - tmark; tmark = now_; }
+  // The r and z sums of a unit tile wait in this CTA's scratch (free until the W1 epilogue) while the n tile is
+  // multiplied: held in registers next to its accumulator they would not fit the 168 registers of a thread.
+  static_assert(H >= NT, "gate parking: 2 * (N / 2) * NT floats within the [N][H] scratch");
+  float* park = scratch_cta + tid;
   for (int ut = 0; ut < TC::UT; ++ut) {
-    const int j = ut * 128 + r;
-    const float bhr = __ldg(p.bhh + j), bhz = __ldg(p.bhh + H + j), bhn = __ldg(p.bhh + 2 * H + j);
-    uint32_t ta[3];
+    {
+      float v[TC::NV];
+      tc_tile<TC>(acc, ring, bop, tb, tbox, wg, lane, ts);
+      tc_fold<TC>(acc, v, p.tc_inv_hh);
 #pragma unroll
-    for (int g = 0; g < 3; ++g) ta[g] = tile_wait(tcnt + g);
-    tc_fence_after();
-    for (int c0 = hsel * 8; c0 < ((p.dbg_mode & 2) ? 0 : Mp); c0 += 16) {
-      float gr[8], gz[8], gn[8], ho[8];
+      for (int q = 0; q < TC::NV; ++q) park[q * NT] = v[q];
+      tc_tile<TC>(acc, ring, bop, tb, tbox, wg, lane, ts);
+      tc_fold<TC>(acc, v, p.tc_inv_hh);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {  // per-column operands from L2 / L1, issued before the TMEM loads
-        const int m = c0 + i;
-        gr[i] = gz[i] = gn[i] = ho[i] = 0.f;
-        if (m < Mp) {
-          const float* gi = p.gi + (size_t)cc.girow[m0 + m] * 3 * H;
-          gr[i] = gi[j]; gz[i] = gi[H + j]; gn[i] = gi[2 * H + j];
-          ho[i] = pool_hidden_cta[(size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.src[m0 + m] * H + j];
-        }
-      }
-      uint32_t a[6][8];
-#pragma unroll
-      for (int g = 0; g < 3; ++g) {
-        tc_tmem_ld8(ta[g] + (uint32_t)c0, a[2 * g]);
-        tc_tmem_ld8(ta[g] + (uint32_t)(N + c0), a[2 * g + 1]);
-      }
-      tc_tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int m = c0 + i;
-        if (m < Mp) {
-          const float ar = __fmul_rn(__fadd_rn(__uint_as_float(a[0][i]), __uint_as_float(a[1][i])), p.tc_inv_hh);
-          const float az = __fmul_rn(__fadd_rn(__uint_as_float(a[2][i]), __uint_as_float(a[3][i])), p.tc_inv_hh);
-          const float an = __fmul_rn(__fadd_rn(__uint_as_float(a[4][i]), __uint_as_float(a[5][i])), p.tc_inv_hh);
-          // GRU cell, PyTorch gate order r,z,n (uisrnn.py:39-47):  h' = (h - n) * z + n
-          const float rg = sigmoid_f32(__fadd_rn(gr[i], __fadd_rn(ar, bhr)));
-          const float zg = sigmoid_f32(__fadd_rn(gz[i], __fadd_rn(az, bhz)));
-          const float ng = tanhf(__fadd_rn(gn[i], __fmul_rn(rg, __fadd_rn(an, bhn))));
-          const float hn = __fadd_rn(__fmul_rn(__fsub_rn(ho[i], ng), zg), ng);
-          pool_hidden_cta[(size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.dst[m0 + m] * H + j] = hn;
-        }
-      }
+      for (int q = 0; q < TC::NV; ++q) park[(TC::NV + q) * NT] = v[q];
     }
+    tc_tile<TC>(acc, ring, bop, tb, tbox, wg, lane, ts);
+    float an[TC::NV];
+    tc_fold<TC>(acc, an, p.tc_inv_hh);
 #pragma unroll
-    for (int g = 0; g < 3; ++g) tc_release_slot(&tb.tempty[(tcnt + g) % kTcSlots], lane);
-    tcnt += 3;
+    for (int h = 0; h < 2; ++h) {
+      const int j = ut * 128 + r0 + 8 * h;
+      const float bhr = __ldg(p.bhh + j), bhz = __ldg(p.bhh + H + j), bhn = __ldg(p.bhh + 2 * H + j);
+#pragma unroll
+      for (int i = 0; i < NI; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int m = 8 * i + cq + e, v = 4 * i + 2 * h + e;
+          if (m < Mp) {
+            const float* gi = p.gi + (size_t)cc.girow[m0 + m] * 3 * H;
+            const float ho = pool_hidden_cta[(size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.src[m0 + m] * H + j];
+            // GRU cell, PyTorch gate order r,z,n:  h' = (h - n) * z + n
+            const float rg = sigmoid_f32(__fadd_rn(gi[j], __fadd_rn(park[v * NT], bhr)));
+            const float zg = sigmoid_f32(__fadd_rn(gi[H + j], __fadd_rn(park[(TC::NV + v) * NT], bhz)));
+            const float ng = tanhf(__fadd_rn(gi[2 * H + j], __fmul_rn(rg, __fadd_rn(an[v], bhn))));
+            pool_hidden_cta[(size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.dst[m0 + m] * H + j] =
+                __fadd_rn(__fmul_rn(__fsub_rn(ho, ng), zg), ng);
+          }
+        }
+    }
   }
   named_bar_sync(1, NT);  // h' of every column is in the slot pool (global memory, CTA-scope ordering)
   if (tid == 0) { const long long now_ = clock64(); ph[2] += now_ - tmark; tmark = now_; }
   // ---------------- B = h', a = relu(W1 h' + b1) -> scratch
-  tc_gather_b<H, N, NT>(bop, [&](int m) -> const float* {
-    return pool_hidden_cta + (size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.dst[m0 + m] * H; }, Mp, p.tc_sh, tid);
-  tc_signal_b(tb.bready, lane);
+  stage_b([&](int m) -> const float* {
+    return pool_hidden_cta + (size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.dst[m0 + m] * H; }, p.tc_sh);
   for (int mt = 0; mt < TC::T2; ++mt) {
-    const int j = mt * 128 + r;
-    const float b1j = __ldg(p.b1 + j);
-    const uint32_t ta = tile_wait(tcnt);
-    tc_fence_after();
-    for (int c0 = hsel * 8; c0 < Mp; c0 += 16) {
-      uint32_t a[2][8];
-      tc_tmem_ld8(ta + (uint32_t)c0, a[0]);
-      tc_tmem_ld8(ta + (uint32_t)(N + c0), a[1]);
-      tc_tmem_ld_wait();
+    float v1[TC::NV];
+    tc_tile<TC>(acc, ring, bop, tb, tbox, wg, lane, ts);
+    tc_fold<TC>(acc, v1, p.tc_inv_1);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int m = c0 + i;
-        if (m < Mp) {
-          const float v = __fmul_rn(__fadd_rn(__uint_as_float(a[0][i]), __uint_as_float(a[1][i])), p.tc_inv_1);
-          scratch_cta[(size_t)m * H + j] = fmaxf(__fadd_rn(v, b1j), 0.f);
+    for (int h = 0; h < 2; ++h) {
+      const int j = mt * 128 + r0 + 8 * h;
+      const float b1j = __ldg(p.b1 + j);
+#pragma unroll
+      for (int i = 0; i < NI; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int m = 8 * i + cq + e;
+          if (m < Mp) scratch_cta[(size_t)m * H + j] = fmaxf(__fadd_rn(v1[4 * i + 2 * h + e], b1j), 0.f);
         }
-      }
     }
-    tc_release_slot(&tb.tempty[tcnt % kTcSlots], lane);
-    tcnt += 1;
   }
   named_bar_sync(1, NT);
   if (tid == 0) { const long long now_ = clock64(); ph[3] += now_ - tmark; tmark = now_; }
   // ---------------- B = a, mean = W2 a + b2, then the running-mean update of the cluster
-  tc_gather_b<H, N, NT>(bop, [&](int m) -> const float* { return scratch_cta + (size_t)m * H; }, Mp, p.tc_sa, tid);
-  tc_signal_b(tb.bready, lane);
+  stage_b([&](int m) -> const float* { return scratch_cta + (size_t)m * H; }, p.tc_sa);
   for (int mt = 0; mt < TC::T3; ++mt) {
-    const int d = mt * 128 + r;
-    const float b2d = __ldg(p.b2 + d);
-    const uint32_t ta = tile_wait(tcnt);
-    tc_fence_after();
-    for (int c0 = hsel * 8; c0 < Mp; c0 += 16) {
-      float mu_old[8];
+    float v2[TC::NV];
+    tc_tile<TC>(acc, ring, bop, tb, tbox, wg, lane, ts);
+    tc_fold<TC>(acc, v2, p.tc_inv_2);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int m = c0 + i;
-        mu_old[i] = (m < Mp) ? pool_mean_cta[(size_t)cc.lane[m0 + m] * lane_pool_m + (size_t)cc.src[m0 + m] * D + d] : 0.f;
-      }
-      uint32_t a[2][8];
-      tc_tmem_ld8(ta + (uint32_t)c0, a[0]);
-      tc_tmem_ld8(ta + (uint32_t)(N + c0), a[1]);
-      tc_tmem_ld_wait();
+    for (int h = 0; h < 2; ++h) {
+      const int d = mt * 128 + r0 + 8 * h;
+      const float b2d = __ldg(p.b2 + d);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int m = c0 + i;
-        if (m < Mp) {
-          const float v = __fmul_rn(__fadd_rn(__uint_as_float(a[0][i]), __uint_as_float(a[1][i])), p.tc_inv_2);
-          const float mval = __fadd_rn(v, b2d);
-          const int n = cc.vis[m0 + m];  // visits BEFORE this one (uisrnn.py:425-429)
-          // mean_set[c] = (mean_set[c] * (n - 1) + mean) / n   -- fp32, true division
-          const float mu = (n == 0) ? mval
-                                    : __fdiv_rn(__fadd_rn(__fmul_rn(mu_old[i], (float)(n - 1)), mval), (float)n);
-          pool_mean_cta[(size_t)cc.lane[m0 + m] * lane_pool_m + (size_t)cc.dst[m0 + m] * D + d] = mu;
+      for (int i = 0; i < NI; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int m = 8 * i + cq + e;
+          if (m < Mp) {
+            const float mu_old = pool_mean_cta[(size_t)cc.lane[m0 + m] * lane_pool_m + (size_t)cc.src[m0 + m] * D + d];
+            const float mval = __fadd_rn(v2[4 * i + 2 * h + e], b2d);
+            const int n = cc.vis[m0 + m];  // visits BEFORE this one
+            // mean_set[c] = (mean_set[c] * (n - 1) + mean) / n   -- fp32, true division
+            const float mu = (n == 0) ? mval : __fdiv_rn(__fadd_rn(__fmul_rn(mu_old, (float)(n - 1)), mval), (float)n);
+            pool_mean_cta[(size_t)cc.lane[m0 + m] * lane_pool_m + (size_t)cc.dst[m0 + m] * D + d] = mu;
+          }
         }
-      }
     }
-    tc_release_slot(&tb.tempty[tcnt % kTcSlots], lane);
-    tcnt += 1;
   }
+  if (ts) ts[3] += clock64() - t_in;
 }
 
 // ------------------------------------------------------------------ the kernel
 // XCL = cluster (latency) mode: the kernel is launched with thread-block clusters of 2/4/8 CTAs; the CTAs of a
 // cluster run the SAME utterances in lock step (all selection phases replicated, bit-identical), and split every
 // weight matrix by k-tiles, exchanging partial sums through distributed shared memory (xch_allreduce).
-// TCN > 0 = tensor-core pass (uis_beam_tc.cuh): the three matrix products of the step run as tcgen05 MMAs over
-// TCN columns per pass; warp NW drives the tensor-map TMA, warp NW + 1 issues the MMAs and owns the TMEM allocation.
+// TCN > 0 = tensor-core pass (uis_beam_tc.cuh): the three matrix products of the step run as wgmma MMAs over
+// TCN columns per pass, issued by the two consumer warpgroups; warp NW drives the tensor-map TMA.
 // XM = 2: stationary-weights mode (uis_beam_stat.cuh): groups of 32 CTAs, one utterance stream per group, weights
 // resident in shared memory, products split by rows, group barriers in global memory (cooperative launch).
 template <int H, int D, bool DEEP, int XM = 0, int TCN = 0>
@@ -919,8 +900,7 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + L.bars);
   uint64_t* empty = full + (TC ? TCC::STAGES : kStages);
   volatile int* misc = reinterpret_cast<volatile int*>(smem + L.misc);
-  TcBars tb{full, empty, empty + TCC::STAGES, empty + TCC::STAGES + kTcSlots, empty + TCC::STAGES + 2 * kTcSlots};
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tb.bready + 1);
+  TcBars tb{full, empty};
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
@@ -928,13 +908,8 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
     if constexpr (TC) {
       for (int s = 0; s < TCC::STAGES; ++s) {
         mbar_init(&tb.full[s], 1);
-        mbar_init(&tb.empty[s], 1);
+        mbar_init(&tb.empty[s], NW);
       }
-      for (int s = 0; s < kTcSlots; ++s) {
-        mbar_init(&tb.tfull[s], kTcIssuers);
-        mbar_init(&tb.tempty[s], NW);
-      }
-      mbar_init(tb.bready, NW);
     } else {
       for (int s = 0; s < kStages; ++s) {
         mbar_init(&full[s], 1);
@@ -953,44 +928,15 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
     if constexpr (STAT) misc[MI_QNEXT] = sgroup;  // ... and to the groups of the stationary-weights mode
     fence_mbar_init();
   }
-  if constexpr (TC) {
-    if (warp == NW + 1) {  // the MMA warp owns the TMEM allocation (whole TMEM: one CTA per SM)
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                   "r"((uint32_t)TCC::TMEM_COLS));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    tc_fence_before();
-  }
   __syncthreads();
   if constexpr (XCL) cluster_sync_all();  // every peer's exchange barriers exist before anyone arrives on them
-  uint32_t tmem_base = 0;
-  if constexpr (TC) {
-    tc_fence_after();
-    tmem_base = *tmem_slot;
-  }
-  // end of the tensor-core kernel: every warp meets here; the allocating warp returns the TMEM columns
-  auto tc_teardown = [&]() {
-    tc_fence_before();
-    __syncthreads();
-    if (warp == NW + 1) {
-      tc_fence_after();
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TCC::TMEM_COLS));
-    }
-  };
 
   if (warp >= NW) {  // ---------------- producer warp (+ idle warps of its warpgroup)
     if constexpr (STAT) return;  // nothing streams: the weights are resident
-    if constexpr (TC) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");  // the unrolled MMA issue loop must not spill
+    if constexpr (TC) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     else if constexpr (C::REBALANCE) asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
     if constexpr (TC) {
-      if (warp == NW)
-        tc_producer_loop<TCC, H>(&p.tc_wmap, reinterpret_cast<unsigned char*>(ring), tb, &misc[MI_DONE]);
-      else if (warp == NW + 1 || (kTcIssuers == 2 && warp == NW + 2))  // whole warps run the issue loop (uniform operands); one elected lane issues
-        tc_mma_loop<TCC>(reinterpret_cast<const unsigned char*>(ring), reinterpret_cast<const unsigned char*>(XA), tmem_base,
-                         tb, &misc[MI_DONE], reinterpret_cast<long long*>(smem + L.phase) + 16, lane, warp - (NW + 1),
-                         &misc[MI_TCEXIT]);
-      __syncwarp();
-      tc_teardown();
+      if (warp == NW) tc_producer_loop<TCC, H>(&p.tc_wmap, reinterpret_cast<unsigned char*>(ring), tb, &misc[MI_DONE]);
     } else {
       if (warp == NW && lane == 0) producer_loop<C, XCL>(p, ring, full, empty, misc);
     }
@@ -1018,7 +964,7 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
 #pragma unroll
   for (int u = 0; u < UPT; ++u) b1r[u] = TC ? 0.f : p.b1[tid + NT * u];
   const float b2r = (tid < D && !TC) ? p.b2[tid] : 0.f;
-  unsigned tc_tiles = 0;  // tensor-core pass: accumulator tiles consumed so far (identical in every consumer thread)
+  unsigned tc_boxes = 0;  // tensor-core pass: ring boxes consumed so far (identical in every consumer thread)
   float* tc_scratch_cta = TC ? p.tc_scratch + (size_t)blockIdx.x * (TC ? TCN : 1) * H : nullptr;
   if (tid < D) wv[tid] = p.wvec[tid];
   unsigned stat_epoch = 0;
@@ -1045,7 +991,7 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
     for (int i = 0; i < 16; ++i) ph[i] = 0;
     ph[10] = clock64();
   }
-  // (ph[16..19], the MMA issuer's stall counters, are zeroed by thread 0 before the first __syncthreads)
+  // (ph[16..19], the tensor-core pass counters, are zeroed by thread 0 before the first __syncthreads)
   long long& tmark = ph[10];
   long long& st_cols = ph[11]; long long& st_pass = ph[12]; long long& st_cand = ph[13]; long long& st_steps = ph[14];
   long long& st_maxk = ph[15];
@@ -1582,13 +1528,13 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
           reinterpret_cast<unsigned*>(lane_base(f / (int)PW) + L.l_scored)[f % (int)PW] = 0;
       for (int m0 = 0; m0 < Mtot; m0 += TCN) {
         if (m0 == 0)
-          tc_run_pass<H, D, TC ? TCN : 16>(p, reinterpret_cast<unsigned char*>(XA), tmem_base, tb, tc_tiles, cc, m0,
-                                           min(TCN, Mtot - m0), pool_mean_cta, pool_hidden_cta, tc_scratch_cta, tid, lane,
-                                           warp, ph, tmark, prescore);
+          tc_run_pass<H, D, TC ? TCN : 16>(p, reinterpret_cast<const unsigned char*>(ring), reinterpret_cast<unsigned char*>(XA),
+                                           tb, tc_boxes, cc, m0, min(TCN, Mtot - m0), pool_mean_cta, pool_hidden_cta,
+                                           tc_scratch_cta, tid, lane, warp, ph, tmark, ph + 16, prescore);
         else
-          tc_run_pass<H, D, TC ? TCN : 16>(p, reinterpret_cast<unsigned char*>(XA), tmem_base, tb, tc_tiles, cc, m0,
-                                           min(TCN, Mtot - m0), pool_mean_cta, pool_hidden_cta, tc_scratch_cta, tid, lane,
-                                           warp, ph, tmark, nothing);
+          tc_run_pass<H, D, TC ? TCN : 16>(p, reinterpret_cast<const unsigned char*>(ring), reinterpret_cast<unsigned char*>(XA),
+                                           tb, tc_boxes, cc, m0, min(TCN, Mtot - m0), pool_mean_cta, pool_hidden_cta,
+                                           tc_scratch_cta, tid, lane, warp, ph, tmark, ph + 16, nothing);
         named_bar_sync(1, NT);
         UIS_PHASE(4);
       }
@@ -1708,10 +1654,7 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
     atomicAdd(&p.stats[3], (unsigned long long)st_steps);
     atomicMax(&p.stats[4], (unsigned long long)max(st_maxk, (long long)misc[MI_MAXK]));
     for (int i = 0; i < 10; ++i) atomicAdd(&p.stats[8 + i], (unsigned long long)ph[i]);
-  }
-  if constexpr (TC) {
-    tc_teardown();  // (a __syncthreads: the issuer's counters are final)
-    if (tid == 0)
+    if constexpr (TC)
       for (int i = 0; i < 4; ++i) atomicAdd(&p.stats[18 + i], (unsigned long long)ph[16 + i]);
   }
 }

@@ -3,8 +3,7 @@
 //
 // Why: with one utterance in flight a beam step is a chain of three small matrix products (uisrnn.py:45-52) whose cost
 // in the streaming kernels is the time to pull 4.7 MB of weights through a TMA ring every step -- bound by the latency
-// of the L2 -> shared-memory round trip (96 KB in flight per CTA), 33 us per step in the 4-CTA cluster mode
-// (profiles/r3_beam_cluster_kernel_ncu_details.txt).  4.7 MB do not fit one thread-block cluster (16 x 227 KB), but they
+// of the L2 -> shared-memory round trip (96 KB in flight per CTA), also in the cluster mode.  4.7 MB do not fit one thread-block cluster (16 x 227 KB), but they
 // fit 32 CTAs: CTA q owns the rows of 16 hidden units of W_hh (48 rows), 16 rows of W1 and 8 rows of W2 (72 x 512 fp32
 // = 147 KB) and never loads them again.  Row split, so no partial sums travel: every CTA computes its rows of the
 // product for all columns, writes them where the next product reads them -- the new slots of the (group-shared) slot

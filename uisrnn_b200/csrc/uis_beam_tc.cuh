@@ -1,26 +1,24 @@
-// Tensor-core weight pass of the beam kernel (tcgen05 / TMEM / tensor-map TMA, sm_100a).
+// Tensor-core weight pass of the beam kernel (warpgroup MMA / tensor-map TMA, sm_90a).
 //
-// Same arithmetic as run_pass() in uis_beam.cuh -- h' = GRU(x_t, h_src), a = relu(W1 h' + b1), m = W2 a + b2 of
-// /root/reference/uisrnn/uisrnn.py:45-52 for the step's distinct source states -- but the three matrix products run
-// on the 5th-generation tensor cores at fp32-grade accuracy:
+// Same arithmetic as run_pass() in uis_beam.cuh -- h' = GRU(x_t, h_src), a = relu(W1 h' + b1), m = W2 a + b2 of the
+// reference's CoreRNN.forward for the step's distinct source states -- but the three matrix products run on the
+// tensor cores (wgmma) at fp32-grade accuracy:
 //
 //   * every weight w is split once, at uis_model_create, into two fp16 planes  w * 2^s = hi + lo  (22 significant
-//     bits; s = a per-matrix power of two) stored K-major [2 * ROWS][H]; the planes are the A operand (M = 128 weight
-//     rows per instruction), streamed through a shared-memory ring by tensor-map TMA (cp.async.bulk.tensor.2d,
-//     128-byte swizzle, boxes of 128 rows x 64 k = 16 KB);
+//     bits; s = a per-matrix power of two) stored K-major [2 * ROWS][H]; the planes are the A operand, streamed through
+//     a shared-memory ring by tensor-map TMA (cp.async.bulk.tensor.2d, 128-byte swizzle, boxes of 128 rows x 64 k =
+//     16 KB); each of the two consumer warpgroups multiplies the 64 rows of a box that are its own (m64 instructions);
 //   * the hidden columns of the pass are split the same way by the consumer warps and stay in shared memory as the
 //     B operand: per 64-wide k atom, rows [0, N) hold the hi halves and rows [N, 2N) the lo halves of the N columns,
 //     so ONE instruction with N' = 2N multiplies a weight box with both:  D[:, 0:N] += A * Bhi,  D[:, N:2N] += A * Blo;
 //   * per 128-row tile the lo boxes go first, then the hi boxes: the tensor core adds into its fp32 accumulator
-//     with truncation, and the small products cost nothing while the accumulator is still small (measured / simulated:
-//     max |error| 2.7e-6 against fp64 for 512-term sums of magnitude ~3, the fp32 FMA chain of the FFMA kernel: 2.3e-6);
-//   * accumulators live in TMEM (5 slots of 2N fp32 columns); the consumer warps read them back with tcgen05.ld
-//     (thread <-> weight row, so gate math and the slot-pool writes stay coalesced exactly as in the FFMA kernel)
-//     while the issuing thread already works on the next tiles.
+//     with truncation, and the small products cost nothing while the accumulator is still small (max |error| 2.7e-6
+//     against fp64 for 512-term sums of magnitude ~3; the fp32 FMA chain of the FFMA kernel: 2.3e-6);
+//   * accumulators live in registers (m64 x 2N fp32 = N registers per thread); a warpgroup keeps one box of MMAs in
+//     flight behind the one it issues and returns a ring box to the TMA producer as soon as its MMAs have completed.
 //
-// Cost model (tools/tc/tc_gemm_probe.cu on B200): a 128 x N' x 16 MMA fed from shared memory takes ~90-105 cycles
-// for any N' <= 128, so the pass costs the same for 1 or 48 columns -- the kernel therefore runs up to 6 utterances
-// (lanes) per CTA and gives all their columns to one pass.
+// The cost of an m64 x N' x 16 MMA hardly depends on N' <= 96, so the kernel runs up to 6 utterances (lanes) per CTA and
+// gives all their columns to one pass.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -29,12 +27,6 @@
 namespace uis {
 
 constexpr int kTcBoxBytes = 16384;  // 128 rows x 64 k, fp16
-constexpr int kTcSlots = 5;         // TMEM accumulator slots
-#ifndef UIS_TC_COMMIT_PER_BOX
-constexpr unsigned kTcPairMask = 1u;  // one commit per pair of ring boxes (8 MMAs)
-#else
-constexpr unsigned kTcPairMask = 0u;  // one commit per ring box (4 MMAs): the earlier scheme, kept for A/B builds
-#endif
 
 template <int H, int D, int N>
 struct TcCfg {
@@ -44,45 +36,54 @@ struct TcCfg {
   static constexpr int TILES = T1 + T2 + T3;
   static constexpr int ROWS = 3 * H + H + D;              // rows of one plane
   static constexpr int NP = 2 * N;                        // B rows / accumulator columns per tile
+  static constexpr int NACC = NP / 2;                     // accumulator registers per thread (m64 x NP over 128 threads)
+  static constexpr int NV = N / 2;                        // folded (hi + lo) values per thread and tile
   static constexpr int ATOM_BYTES = NP * 128;             // one k atom of the B operand
   static constexpr int BOP_BYTES = KA * ATOM_BYTES;
-  static constexpr int STAGES = (N <= 32) ? 8 : 4;        // ring depth (boxes); divides the 2 * KA boxes of a tile
-  static constexpr int TMEM_COLS = 512;
+  static constexpr int STAGES = (N <= 32) ? 8 : 4;        // ring depth (boxes)
   static_assert(H % 128 == 0 && D % 128 == 0, "tensor-core pass: 128-row tiles");
-  static_assert(N % 16 == 0 && NP <= 256 && kTcSlots * NP <= TMEM_COLS, "accumulator slots");
-  static_assert((2 * KA) % STAGES == 0 && STAGES % 2 == 0 && KA % 2 == 0,
-                "a tile starts at ring stage 0 and boxes go in pairs (same plane, adjacent stages and k atoms)");
+  static_assert(NP == 64 || NP == 96, "wgmma instantiations: N = 32 or 48 columns");
 };
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 // shared-memory matrix descriptor, K-major, 128-byte swizzle: rows of 128 B, 8-row groups 1024 B apart
 __device__ __forceinline__ uint64_t tc_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3fff);  // start address, 16-byte units
   d |= (uint64_t)1 << 16;                  // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;        // stride byte offset between 8-row groups
-  d |= (uint64_t)1 << 46;                  // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                  // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                  // SWIZZLE_128B
   return d;
 }
-// instruction descriptor: D fp32, A/B fp16, both K-major, M = 128, N = n
-__host__ __device__ constexpr uint32_t tc_idesc_f16(int n) {
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// arrive on an mbarrier when every MMA issued so far by this thread has completed
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+
+// D (m64 x NP, fp32, registers) (+)= A (m64 x k16, fp16, shared) * B (k16 x NP, fp16, shared); both operands K-major.
+// Accumulator register 4 i + 2 h + e of lane l in warp w of the warpgroup: row 16 w + l / 4 + 8 h, column 8 i + 2 (l % 4) + e.
+template <int NP> struct Wgmma;
+template <> struct Wgmma<96> {
+  static __device__ __forceinline__ void mma(float (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(adesc), "l"(bdesc), "r"(acc)
+        : "memory");
+  }
+};
+template <> struct Wgmma<64> {
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(acc)
+        : "memory");
+  }
+};
+
 __device__ __forceinline__ void tc_tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
@@ -90,15 +91,9 @@ __device__ __forceinline__ void tc_tma_load_2d(void* dst, const CUtensorMap* map
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tc_tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr));
-}
-__device__ __forceinline__ void tc_tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// Bounded wait of the tensor-core pipeline (consumer warps, MMA issuer): a protocol error must trap -- and surface
-// as a CUDA error in uis_get_stats -- instead of hanging the device (~4 s at 2 GHz).
+// Bounded wait of the tensor-core pipeline: a protocol error must trap -- and surface as a CUDA error in
+// uis_get_stats -- instead of hanging the device (~4 s at 2 GHz).
 __device__ __forceinline__ void tc_mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
@@ -106,35 +101,6 @@ __device__ __forceinline__ void tc_mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
     if ((++spins & 0x3ffu) == 0 && clock64() - t0 > 8000000000ll) __trap();
   }
-}
-
-// Wait of a consumer warp for an accumulator tile: parked by the hardware (try_wait with a suspend-time hint) so that
-// eight waiting warps do not take issue slots from the MMA-issuing warp; bounded like tc_mbar_wait.
-__device__ __forceinline__ void tc_mbar_wait_parked(uint64_t* bar, uint32_t parity) {
-  unsigned tries = 0;
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity), "r"(20000u)  // <= 20 us per try
-        : "memory");
-    if (ok) return;
-    if (++tries > 200000u) __trap();
-  }
-}
-
-// Same, charging the time spent stalled to a counter (shared memory; only touched when the first probe fails)
-__device__ __forceinline__ void tc_mbar_wait_timed(uint64_t* bar, uint32_t parity, long long* stall) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  unsigned spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3ffu) == 0 && clock64() - t0 > 8000000000ll) __trap();
-  }
-  *stall += clock64() - t0;
 }
 
 // Wait for an mbarrier phase, giving up when the consumer warps have announced the end of the kernel.
@@ -161,15 +127,12 @@ __device__ __forceinline__ bool tc_elect_one() {
 }
 
 struct TcBars {
-  uint64_t* full;    // [STAGES]   TMA -> MMA
-  uint64_t* empty;   // [STAGES]   MMA -> TMA
-  uint64_t* tfull;   // [kTcSlots] MMA -> epilogue
-  uint64_t* tempty;  // [kTcSlots] epilogue -> MMA
-  uint64_t* bready;  // [1]        B operand written (consumer warps -> MMA)
+  uint64_t* full;    // [STAGES]   TMA -> consumer warpgroups
+  uint64_t* empty;   // [STAGES]   consumer warps -> TMA
 };
 
 // 128-row tile t of the pass -> first row inside one plane (W_hh tiles ordered (unit tile, gate): the three gate
-// tiles of a unit tile are consecutive, so the GRU epilogue of unit tile u can start after 3 tiles)
+// tiles of a unit tile are consecutive, so the GRU epilogue of unit tile u can run after 3 tiles)
 template <class TC, int H>
 __device__ __forceinline__ int tc_tile_row0(int t) {
   if (t < TC::T1) return (t % 3) * H + (t / 3) * 128;
@@ -188,9 +151,7 @@ __device__ void tc_producer_loop(const CUtensorMap* wmap, unsigned char* ring, c
       for (int pl = 0; pl < 2 && run; ++pl) {  // plane 0 = lo, 1 = hi
         for (int ka = 0; ka < TC::KA; ++ka, ++it) {
           const unsigned s = it % TC::STAGES, ph = (it / TC::STAGES) & 1;
-          // ring boxes are released in PAIRS (stages 2j, 2j + 1) by one tcgen05.commit on the odd stage's barrier: the
-          // issuing thread stalls on every commit, so halving their number shortens the pass (tc_mma_loop)
-          if (!tc_wait_or_done(&b.empty[s | kTcPairMask], ph ^ 1, done_flag)) { run = false; break; }
+          if (!tc_wait_or_done(&b.empty[s], ph ^ 1, done_flag)) { run = false; break; }
           if (tc_elect_one()) {
             mbar_arrive_expect_tx(&b.full[s], kTcBoxBytes);
             tc_tma_load_2d(ring + (size_t)s * kTcBoxBytes, wmap, ka * 64, pl * TC::ROWS + row0, &b.full[s]);
@@ -205,109 +166,52 @@ __device__ void tc_producer_loop(const CUtensorMap* wmap, unsigned char* ring, c
     tc_mbar_wait(&b.full[j % TC::STAGES], (j / TC::STAGES) & 1);
 }
 
-// ---- MMA issuer (one thread) -----------------------------------------------------------------------------------
-// The WHOLE warp runs this loop with warp-uniform values and only the tcgen05 instructions are given to one elected
-// lane: operands of UTCHMMA / UTCBAR live in uniform registers, and a loop entered by a single lane makes the compiler
-// move every operand there through a vote-and-broadcast sequence (~20 dependent instructions per MMA, measured 146
-// cycles per MMA against ~60 for the MMA itself).  Descriptors are one 64-bit constant plus the 16-byte-unit address.
-// tstat[0..3]: cycles the issuer spent stalled on (0) a ring box not yet landed, (1) an accumulator slot not yet
-// drained by the epilogue warps, (2) the B operand of the next product / the next pass; (3) cycles inside passes
-// Two issuing warps (-DUIS_TC_ISSUERS=2; an experiment that is kept because its result is the argument of DESIGN.md 4.2).
-// Between two bursts of MMAs the issuing thread needs ~300 cycles for the barrier polls, the uniform-register descriptor
-// set-up and the commit, and it cannot run ahead of the tensor pipe; the hypothesis was that this exposed work explains the
-// 128 cycles per MMA of the kernel against the 86-cycle floor of a bare loop.  With two warps taking the box pairs in turn
-// -- role 0 the even pairs of every tile, role 1 the odd ones, a token handed over through two named barriers so that the
-// bursts enter the pipe in the same order, both threads arriving on the accumulator's `tfull` barrier -- the preparation of
-// a pair overlaps the other warp's burst.  Measured on B200 (888 utterances): labels identical, 128.0 ms against 124.1 ms
-// with one issuer, 77 us of issue time per pass against 75: the issue overhead is NOT what holds the pipe back.  What does:
-// every 128 x 96 x 16 MMA moves 4 KB into shared memory (TMA) and 4 KB + 3 KB out of it (A and B operand reads), 11 KB
-// through a 128 B/clk port = 88 cycles before the consumer warps touch shared memory at all.  Default: one issuer.
-#ifndef UIS_TC_ISSUERS
-#define UIS_TC_ISSUERS 1
-#endif
-constexpr int kTcIssuers = UIS_TC_ISSUERS;
-constexpr int kTcTokenBarA = 2, kTcTokenBarB = 3;  // named barriers (0 = __syncthreads, 1 = consumer warps)
-__device__ __forceinline__ void tc_token_arrive(int id) { asm volatile("bar.arrive %0, 64;" ::"r"(id) : "memory"); }
-__device__ __forceinline__ void tc_token_wait(int id) { asm volatile("bar.sync %0, 64;" ::"r"(id) : "memory"); }
-
+// ---- one 128-row tile (consumer warpgroup `wg`: rows 64 wg .. 64 wg + 63 of it) ----------------------------------
+// 2 * KA ring boxes -- the lo plane, then the hi plane -- times 4 k-steps of 16 inside each 64-wide swizzle atom
+// (+32 bytes = +2 descriptor units each).  `box` counts the ring boxes consumed so far (identical in every consumer
+// thread).  tstat (thread 0 only, else null): [0] cycles waiting for a box to land, [1] cycles waiting for MMAs.
 template <class TC>
-__device__ void tc_mma_loop(const unsigned char* ring, const unsigned char* bop, uint32_t tmem_base, const TcBars& b,
-                            volatile int* done_flag, long long* tstat, int lane, int role, volatile int* exit_flag) {
-  constexpr uint32_t idesc = tc_idesc_f16(TC::NP);
+__device__ __forceinline__ void tc_tile(float (&acc)[TC::NACC], const unsigned char* ring, const unsigned char* bop,
+                                        const TcBars& b, unsigned& box, int wg, int lane, long long* tstat) {
   const uint64_t desc0 = tc_desc_sw128(0);  // every field but the start address
-  const uint32_t ring16 = smem_u32(ring) >> 4, bop16 = smem_u32(bop) >> 4;
-  constexpr bool kTwo = kTcIssuers == 2;
-  // token: role 0 issues first; it waits on bar B (role 1's hand-over) before every pair but the very first one
-  const int my_wait = role == 0 ? kTcTokenBarB : kTcTokenBarA, my_give = role == 0 ? kTcTokenBarA : kTcTokenBarB;
-  bool first = true;
-  unsigned tc = 0, nb = 0;
-  for (;;) {
-    for (int t = 0; t < TC::TILES; ++t, ++tc) {
-      const unsigned slot = tc % kTcSlots;
-      if (role == 0) {
-        if (t == 0 || t == TC::T1 || t == TC::T1 + TC::T2) {  // a new B operand (h_src, h', a) must be in place
-          const long long w0 = clock64();
-          if (!tc_wait_or_done(b.bready, nb & 1, done_flag)) {
-            if (kTwo) { *exit_flag = 1; __threadfence_block(); tc_token_arrive(my_give); }  // release the other issuer
-            return;
-          }
-          const long long w1 = clock64();
-          if (lane == 0) { if (t == 0) tstat[3] -= w1; else tstat[2] += w1 - w0; }
-          ++nb;
-        }
-        tc_mbar_wait(&b.tempty[slot], ((tc / kTcSlots) & 1) ^ 1);
-      }
-      const uint32_t d_tmem = tmem_base + slot * TC::NP;
-      const uint32_t tpar = (tc * (unsigned)((2 * TC::KA) / TC::STAGES)) & 1u;  // ring revolutions before this tile
-      // One tile = 2 * KA boxes (lo plane, then hi plane), a whole number of ring revolutions, so the ring stage of every
-      // box is a compile-time constant and its barrier parity is one XOR away from one.  Boxes go in pairs -- both waits,
-      // eight MMAs back to back, one commit for the pair.
+  const uint32_t a16 = (smem_u32(ring) + (uint32_t)wg * (kTcBoxBytes / 2)) >> 4, b16 = smem_u32(bop) >> 4;
+#pragma unroll
+  for (int i = 0; i < TC::NACC; ++i) acc[i] = 0.f;
+  unsigned prev = 0;
 #pragma unroll 1
-      for (int q = 0; q < 2 * TC::KA; q += 2) {  // (not unrolled: 16 precomputed descriptor pairs would spill)
-        if (kTwo && ((q >> 1) & 1) != role) continue;
-        constexpr int S = TC::STAGES;
-        const uint32_t s0 = (uint32_t)q % S, par = tpar ^ (((uint32_t)q / S) & 1u);  // boxes q, q + 1: stages s0, s0 + 1
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          if (!mbar_try_wait(&b.full[s0 + u], par)) {
-            if (role == 0) {
-              const long long w0 = clock64();
-              tc_mbar_wait(&b.full[s0 + u], par);
-              if (lane == 0) tstat[0] += clock64() - w0;
-            } else {
-              // role 1 runs ahead into the tile after the last pass: those boxes may never be loaded (the producer stops
-              // when the consumer warps announce the end), so this wait gives up with the kernel
-              if (!tc_wait_or_done(&b.full[s0 + u], par, done_flag)) return;
-            }
-          }
-        }
-        const uint64_t adesc = desc0 + (uint64_t)(ring16 + s0 * (kTcBoxBytes >> 4));
-        const uint64_t bdesc = desc0 + (uint64_t)(bop16 + ((uint32_t)q % TC::KA) * (TC::ATOM_BYTES >> 4));
-        if (kTwo) {
-          if (!first || role == 1) {
-            tc_token_wait(my_wait);  // the previous pair (other warp) has been issued
-            if (role == 1 && *exit_flag) return;
-          }
-          first = false;
-        }
-        tc_fence_after();
-        if (tc_elect_one()) {
-#pragma unroll
-          for (int u = 0; u < 2; ++u) {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)  // 4 k-steps of 16 inside the 64-wide swizzle atom: +32 bytes = +2 units each
-              tc_mma_f16(d_tmem, adesc + (uint64_t)(u * (kTcBoxBytes >> 4) + 2 * kk),
-                         bdesc + (uint64_t)(u * (TC::ATOM_BYTES >> 4) + 2 * kk), idesc, (q | u | kk) != 0);
-            if (u == 1 || !kTcPairMask) tc_commit(&b.empty[s0 + u]);  // frees the ring boxes when the MMAs above have read them
-          }
-          if (q >= 2 * TC::KA - (kTwo ? 4 : 2)) tc_commit(&b.tfull[slot]);  // this thread's last burst of the tile
-        }
-        __syncwarp();
-        if (kTwo) tc_token_arrive(my_give);
-      }
+  for (int q = 0; q < 2 * TC::KA; ++q, ++box) {
+    const unsigned s = box % TC::STAGES, par = (box / TC::STAGES) & 1u;
+    if (!mbar_try_wait(&b.full[s], par)) {
+      const long long w0 = tstat ? clock64() : 0;
+      tc_mbar_wait(&b.full[s], par);
+      if (tstat) tstat[0] += clock64() - w0;
     }
-    if (lane == 0 && role == 0) tstat[3] += clock64();  // issue time of the pass (first B operand ready -> last MMA issued)
+    const uint64_t adesc = desc0 + (uint64_t)(a16 + s * (kTcBoxBytes >> 4));
+    const uint64_t bdesc = desc0 + (uint64_t)(b16 + (uint32_t)(q % TC::KA) * (TC::ATOM_BYTES >> 4));
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) Wgmma<TC::NP>::mma(acc, adesc + 2 * kk, bdesc + 2 * kk, (q | kk) != 0);
+    wgmma_commit();
+    if (q > 0) {  // the previous box's MMAs have completed: its ring stage goes back to the producer
+      wgmma_wait<1>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&b.empty[prev]);
+    }
+    prev = s;
   }
+  const long long w0 = tstat ? clock64() : 0;
+  wgmma_wait<0>();
+  if (tstat) tstat[1] += clock64() - w0;
+  __syncwarp();
+  if (lane == 0) mbar_arrive(&b.empty[prev]);
+}
+
+// hi + lo column halves of a finished tile, scaled back: v[4 i + 2 h + e] <- row 8 h, column 8 i + 2 (lane % 4) + e
+template <class TC>
+__device__ __forceinline__ void tc_fold(const float (&acc)[TC::NACC], float (&v)[TC::NV], float inv) {
+  constexpr int LO = TC::NACC / 2;  // register offset of the lo halves (columns N .. 2N - 1)
+#pragma unroll
+  for (int i = 0; i < TC::NV; ++i) v[i] = __fmul_rn(__fadd_rn(acc[i], acc[LO + i]), inv);
 }
 
 // ---- consumer warps: B operand ---------------------------------------------------------------------------------
@@ -344,17 +248,12 @@ __device__ __forceinline__ void tc_gather_b(unsigned char* bop, SrcFn src, int M
     }
   }
 }
-// all consumer warps: make the generic-proxy writes visible to the tensor core, then tell the MMA thread
-__device__ __forceinline__ void tc_signal_b(uint64_t* bready, int lane) {
+// all consumer warps: make the generic-proxy writes of the B operand visible to the tensor cores (async proxy) and
+// wait until every warp has written its part
+template <int NTHREADS>
+__device__ __forceinline__ void tc_publish_b() {
   fence_proxy_async();
-  __syncwarp();
-  if (lane == 0) mbar_arrive(bready);
-}
-// one consumer warp releases an accumulator slot
-__device__ __forceinline__ void tc_release_slot(uint64_t* tempty, int lane) {
-  tc_fence_before();
-  __syncwarp();
-  if (lane == 0) mbar_arrive(tempty);
+  named_bar_sync(1, NTHREADS);
 }
 
 }  // namespace uis

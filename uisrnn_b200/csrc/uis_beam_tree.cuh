@@ -1,4 +1,4 @@
-// Beam search with look_ahead >= 2 (one utterance per CTA), sm_100a.
+// Beam search with look_ahead >= 2 (one utterance per CTA), sm_90a.
 //
 // Reference semantics: uisrnn/uisrnn.py:455-477 (_calculate_score enumerates every index tuple
 // (c_1..c_L), c_i <= K + #clusters opened earlier in the tuple), :388-453 (each sub-step is scored
@@ -11,7 +11,7 @@
 //   level L'      : leaves are only scored (the last sub-step's GRU never enters a score),
 //                   ranked with the reference's flat-index tie-break, and the best beam_size are
 //                   evaluated and materialised as the next generation of hypothesis tables.
-// The weight streaming / register-tiled FFMA2 passes are the ones of uis_beam.cuh (run_pass).
+// The weight streaming / register-tiled FFMA passes are the ones of uis_beam.cuh (run_pass).
 #pragma once
 #include "uis_beam.cuh"
 

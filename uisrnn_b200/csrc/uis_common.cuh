@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a UIS-RNN kernels: mbarrier, 1-D TMA bulk copies,
+// Shared device helpers for the sm_90a UIS-RNN kernels: mbarrier, 1-D TMA bulk copies,
 // cp.async, named barriers.  Everything here is plain inline PTX (no CUTLASS).
 #pragma once
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05) variant of the beam kernel: look_ahead 1, depth 1, shapes whose weight matrices tile by 128 rows.
+// Tensor-core (wgmma) variant of the beam kernel: look_ahead 1, depth 1, shapes whose weight matrices tile by 128 rows.
 #include "uis_launch.cuh"
 namespace uis {
 namespace {

@@ -1,5 +1,5 @@
 // fit() on the device: one training iteration of UISRNN.fit_concatenated
-// (/root/reference/uisrnn/uisrnn.py:252-295) as hand-written sm_100a kernels behind a C ABI:
+// (reference uisrnn/uisrnn.py:252-295) as hand-written sm_90a kernels behind a C ABI:
 //   packed-sequence GRU forward (:262-263 -> CoreRNN.forward :45-52), MLP, running mean over time
 //   (:265-271), masked weighted-MSE likelihood (:274-277, loss_func.py:19-41), sigma^2 prior
 //   (:280-284, loss_func.py:44-60), parameter-norm regulariser (:287-288, loss_func.py:63-76),
@@ -1283,7 +1283,7 @@ int run_iteration(uis_trainer* t, const int32_t* lengths, int B, int L, int mode
   const unsigned it_no = (unsigned)t->calls;  // dropout masks: a function of (seed, iteration, layer, element)
   const unsigned seed = (unsigned)(t->hp.dropout_seed ^ (t->hp.dropout_seed >> 32));
   const float keep_inv = drop ? 1.0f / (1.0f - t->hp.rnn_dropout) : 1.0f;
-  const int drop_blocks = (int)std::min<size_t>((RH + 255) / 256, 148 * 8);
+  const int drop_blocks = (int)std::min<size_t>((RH + 255) / 256, 132 * 8);
   // input sequence of layer l: the batch itself, or the (dropped) output sequence of the layer below
   auto layer_in = [&](int l) -> const float* {
     if (l == 0) return t->x.p;

@@ -3,7 +3,7 @@
 `parallel_predict`, and the module-level `CoreRNN` / `BeamState`).
 
 Inference on a CUDA device runs the whole beam search inside libuisrnn_b200.so (hand-written
-sm_100a kernels behind the C ABI in include/uisrnn_b200.h): `predict(list)` hands all utterances
+sm_90a kernels behind the C ABI in include/uisrnn_b200.h): `predict(list)` hands all utterances
 to ONE native call, which shards them over persistent CTAs; nothing but the labels comes back.
 There is no silent fallback: on a CUDA device an unsupported configuration raises.  On the CPU
 device (explicit `--enable_cuda=False`, the reference's own device rule) the decoder in
@@ -105,7 +105,7 @@ class UISRNN:
     self._native = None          # (fingerprint, NativeModel) cache for the CUDA decoder
     self._native_lock = threading.Lock()
     if self.device.type == 'cuda':
-      # say so NOW if the sm_100a kernels cannot hold this model (predict() / fit() would raise NativeError later;
+      # say so NOW if the sm_90a kernels cannot hold this model (predict() / fit() would raise NativeError later;
       # there is no silent fallback): hidden <= 1024, dim <= 512, 1..4 GRU layers (one layer above hidden 512 / dim 256)
       too_big = args.rnn_hidden_size > 1024 or self.observation_dim > 512 or args.rnn_depth > 4 or (
           args.rnn_depth > 1 and (args.rnn_hidden_size > 512 or self.observation_dim > 256))
