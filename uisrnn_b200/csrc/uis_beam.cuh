@@ -59,6 +59,12 @@ struct TabEntry {
   int pad;
 };
 
+struct SmemLayout {
+  unsigned ring, xa, xb, wv, lanes, lane_stride, cols, bars, misc, phase, xch, xbar, slist, total;
+  // offsets inside one lane block
+  unsigned l_xt, l_tabs, l_meta, l_candoff, l_keys, l_svals, l_wins, l_wcol, l_lcol, l_used, l_scored, l_ls;
+};
+
 struct BeamParams {
   // model (device pointers)
   const float* whh_t;    // [H][3H]   = gru.weight_hh_l0 transposed (k-major)
@@ -92,6 +98,7 @@ struct BeamParams {
   float tc_sh, tc_sa;                  // power-of-two scales of the hidden columns and of a = relu(W1 h' + b1)
   float tc_inv_hh, tc_inv_1, tc_inv_2; // 1 / (weight scale * operand scale) per matrix
   float* tc_scratch;                   // [ctas][N][H]  a = relu(W1 h' + b1) between the W1 and the W2 product
+  SmemLayout tc_layout;                // make_layout() of the launched instantiation (no registers held for it)
   // stationary-weights mode (uis_beam_stat.cuh)
   unsigned* stat_bar;                  // [groups][32]: word 0 of a group = arrival counter of its barrier (zero at launch; one 128-byte line per group)
   float* stat_scratch;                 // [groups][kCPCluster][H]  a = relu(W1 h' + b1), exchanged through L2
@@ -150,12 +157,6 @@ struct Cfg {
   static_assert(TG2 * R2 == D && TG1 * R1 == H, "row split");
   static_assert(KG1 * H <= 2 * H && KG2 * D <= 2 * H, "K-split scratch must fit in XA+XB");
   static_assert(D % 4 == 0 && NT % 32 == 0 && D <= NT, "shape");
-};
-
-struct SmemLayout {
-  unsigned ring, xa, xb, wv, lanes, lane_stride, cols, bars, misc, phase, xch, xbar, slist, total;
-  // offsets inside one lane block
-  unsigned l_xt, l_tabs, l_meta, l_candoff, l_keys, l_svals, l_wins, l_wcol, l_lcol, l_used, l_scored, l_ls;
 };
 
 __host__ __device__ inline unsigned align_up(unsigned v, unsigned a) { return (v + a - 1) / a * a; }
@@ -754,7 +755,11 @@ __device__ __forceinline__ void tc_run_pass(const BeamParams& p, const unsigned 
                                             Idle idle_work) {
   using TC = TcCfg<H, D, N>;
   constexpr int NT = 256, NI = N / 8;
-  const size_t lane_pool_h = (size_t)p.P * H, lane_pool_m = (size_t)p.P * D;
+  // batch sizes of the GRU (KB columns) and running-mean (WB groups of 8 columns) epilogues: larger batches spill
+  constexpr int KB = (NI == 6) ? 2 : 4, WB = (NI == 6) ? 3 : NI;
+  // slot s of lane g in the CTA's pools (g * P + s is small: 32-bit index arithmetic, no 64-bit strides held)
+  auto hslot = [&](int g, int s) { return pool_hidden_cta + (size_t)(g * p.P + s) * H; };
+  auto mslot = [&](int g, int s) { return pool_mean_cta + (size_t)(g * p.P + s) * D; };
   const int wg = warp >> 2;
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const int cq = 2 * (lane & 3);
@@ -767,9 +772,13 @@ __device__ __forceinline__ void tc_run_pass(const BeamParams& p, const unsigned 
     tc_publish_b<NT>();
     if (ts) ts[2] += clock64() - w0;
   };
+  // gi rows of the pass's lanes (3H floats each; the columns of a lane are consecutive and share its row) to L2: gi
+  // of the whole batch is far larger than L2, so the GRU epilogue would otherwise read them from HBM
+  if (tid < Mp && (tid == 0 || cc.lane[m0 + tid] != cc.lane[m0 + tid - 1]))
+    prefetch_l2_bulk(p.gi + (size_t)cc.girow[m0 + tid] * 3 * H, 3 * H * 4);
   // ---------------- B = h_src (fp16 hi / lo), then the GRU gates per 128-unit tile
   stage_b([&](int m) -> const float* {
-    return pool_hidden_cta + (size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.src[m0 + m] * H; }, p.tc_sh);
+    return hslot(cc.lane[m0 + m], cc.src[m0 + m]); }, p.tc_sh);
   if (tid == 0) { const long long now_ = clock64(); ph[1] += now_ - tmark; tmark = now_; }
   idle_work();  // the next step's Gaussian terms (their frame has landed by now)
   // (charged to the scoring phase: the TMA ring is already filled meanwhile, the MMAs wait for it)
@@ -779,47 +788,73 @@ __device__ __forceinline__ void tc_run_pass(const BeamParams& p, const unsigned 
   static_assert(H >= NT, "gate parking: 2 * (N / 2) * NT floats within the [N][H] scratch");
   float* park = scratch_cta + tid;
   for (int ut = 0; ut < TC::UT; ++ut) {
+    // gate sums + b_hh: value 4 i + 2 h + e of a tile is row j0 + 8 h, so its bias is that of row j0 + 8 h
+    const int j0 = ut * 128 + r0;
     {
       float v[TC::NV];
-      tc_tile<TC>(acc, ring, bop, tb, tbox, wg, lane, ts);
-      tc_fold<TC>(acc, v, p.tc_inv_hh);
 #pragma unroll
-      for (int q = 0; q < TC::NV; ++q) park[q * NT] = v[q];
-      tc_tile<TC>(acc, ring, bop, tb, tbox, wg, lane, ts);
-      tc_fold<TC>(acc, v, p.tc_inv_hh);
+      for (int g = 0; g < 2; ++g) {  // r, z: parked
+        tc_tile<TC>(acc, ring, bop, tb, tbox, wg, lane, ts);
+        tc_fold<TC>(acc, v, p.tc_inv_hh);
+        const float bh[2] = {__ldg(p.bhh + g * H + j0), __ldg(p.bhh + g * H + j0 + 8)};
 #pragma unroll
-      for (int q = 0; q < TC::NV; ++q) park[(TC::NV + q) * NT] = v[q];
+        for (int q = 0; q < TC::NV; ++q) park[(g * TC::NV + q) * NT] = __fadd_rn(v[q], bh[(q >> 1) & 1]);
+      }
     }
     tc_tile<TC>(acc, ring, bop, tb, tbox, wg, lane, ts);
     float an[TC::NV];
     tc_fold<TC>(acc, an, p.tc_inv_hh);
+    {
+      const float bh[2] = {__ldg(p.bhh + 2 * H + j0), __ldg(p.bhh + 2 * H + j0 + 8)};
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int j = ut * 128 + r0 + 8 * h;
-      const float bhr = __ldg(p.bhh + j), bhz = __ldg(p.bhh + H + j), bhn = __ldg(p.bhh + 2 * H + j);
+      for (int q = 0; q < TC::NV; ++q) an[q] = __fadd_rn(an[q], bh[(q >> 1) & 1]);
+    }
+    // GRU cell, PyTorch gate order r,z,n:  h' = (h - n) * z + n, for this thread's rows j0 + 8 h of every column.
+    // A batch of KB columns issues all its loads before its first store, so that their round trips to L2
+    // overlap instead of queueing behind the stores.  Taking the loads ahead of earlier stores is safe: every store
+    // goes to a new slot, which P3 took from the free bitmap, so it is never the source slot of a column of this
+    // pass, and a slot is not modified once written; `park` is this thread's own; gi is read-only for the whole
+    // kernel (non-coherent loads are fine), the slot pool is written by the kernel (coherent loads only).
 #pragma unroll
-      for (int i = 0; i < NI; ++i)
+    for (int k0 = 0; k0 < 2 * NI; k0 += KB) {  // k = 2 i + e: column 8 i + cq + e
+      float gr[KB][2], gz[KB][2], gn[KB][2], pr[KB][2], pz[KB][2], ho[KB][2];  // [k - k0][h]
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int m = 8 * i + cq + e, v = 4 * i + 2 * h + e;
-          if (m < Mp) {
-            const float* gi = p.gi + (size_t)cc.girow[m0 + m] * 3 * H;
-            const float ho = pool_hidden_cta[(size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.src[m0 + m] * H + j];
-            // GRU cell, PyTorch gate order r,z,n:  h' = (h - n) * z + n
-            const float rg = sigmoid_f32(__fadd_rn(gi[j], __fadd_rn(park[v * NT], bhr)));
-            const float zg = sigmoid_f32(__fadd_rn(gi[H + j], __fadd_rn(park[(TC::NV + v) * NT], bhz)));
-            const float ng = tanhf(__fadd_rn(gi[2 * H + j], __fmul_rn(rg, __fadd_rn(an[v], bhn))));
-            pool_hidden_cta[(size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.dst[m0 + m] * H + j] =
-                __fadd_rn(__fmul_rn(__fsub_rn(ho, ng), zg), ng);
+      for (int b = 0; b < KB; ++b) {
+        const int i = (k0 + b) >> 1, e = (k0 + b) & 1, m = 8 * i + cq + e;
+        if (m < Mp) {
+          const float* gi = p.gi + (size_t)cc.girow[m0 + m] * 3 * H + j0;
+          const float* hs = hslot(cc.lane[m0 + m], cc.src[m0 + m]) + j0;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int v = 4 * i + 2 * h + e;
+            gr[b][h] = __ldg(gi + 8 * h); gz[b][h] = __ldg(gi + H + 8 * h); gn[b][h] = __ldg(gi + 2 * H + 8 * h);
+            pr[b][h] = park[v * NT]; pz[b][h] = park[(TC::NV + v) * NT];
+            ho[b][h] = hs[8 * h];
           }
         }
+      }
+#pragma unroll
+      for (int b = 0; b < KB; ++b) {
+        const int i = (k0 + b) >> 1, e = (k0 + b) & 1, m = 8 * i + cq + e;
+        if (m < Mp) {
+          float* hd = hslot(cc.lane[m0 + m], cc.dst[m0 + m]) + j0;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int v = 4 * i + 2 * h + e;
+            const float rg = sigmoid_f32(__fadd_rn(gr[b][h], pr[b][h]));
+            const float zg = sigmoid_f32(__fadd_rn(gz[b][h], pz[b][h]));
+            const float ng = tanhf(__fadd_rn(gn[b][h], __fmul_rn(rg, an[v])));
+            hd[8 * h] = __fadd_rn(__fmul_rn(__fsub_rn(ho[b][h], ng), zg), ng);
+          }
+        }
+      }
     }
   }
   named_bar_sync(1, NT);  // h' of every column is in the slot pool (global memory, CTA-scope ordering)
   if (tid == 0) { const long long now_ = clock64(); ph[2] += now_ - tmark; tmark = now_; }
   // ---------------- B = h', a = relu(W1 h' + b1) -> scratch
   stage_b([&](int m) -> const float* {
-    return pool_hidden_cta + (size_t)cc.lane[m0 + m] * lane_pool_h + (size_t)cc.dst[m0 + m] * H; }, p.tc_sh);
+    return hslot(cc.lane[m0 + m], cc.dst[m0 + m]); }, p.tc_sh);
   for (int mt = 0; mt < TC::T2; ++mt) {
     float v1[TC::NV];
     tc_tile<TC>(acc, ring, bop, tb, tbox, wg, lane, ts);
@@ -845,24 +880,36 @@ __device__ __forceinline__ void tc_run_pass(const BeamParams& p, const unsigned 
     float v2[TC::NV];
     tc_tile<TC>(acc, ring, bop, tb, tbox, wg, lane, ts);
     tc_fold<TC>(acc, v2, p.tc_inv_2);
+    // the old means of a batch of WB column groups are loaded before the first new mean is stored (a new slot is never
+    // the source slot of a column of this pass, see the GRU epilogue)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int d = mt * 128 + r0 + 8 * h;
       const float b2d = __ldg(p.b2 + d);
 #pragma unroll
-      for (int i = 0; i < NI; ++i)
+      for (int i0 = 0; i0 < NI; i0 += WB) {
+        float mu_old[WB][2];
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int m = 8 * i + cq + e;
-          if (m < Mp) {
-            const float mu_old = pool_mean_cta[(size_t)cc.lane[m0 + m] * lane_pool_m + (size_t)cc.src[m0 + m] * D + d];
-            const float mval = __fadd_rn(v2[4 * i + 2 * h + e], b2d);
-            const int n = cc.vis[m0 + m];  // visits BEFORE this one
-            // mean_set[c] = (mean_set[c] * (n - 1) + mean) / n   -- fp32, true division
-            const float mu = (n == 0) ? mval : __fdiv_rn(__fadd_rn(__fmul_rn(mu_old, (float)(n - 1)), mval), (float)n);
-            pool_mean_cta[(size_t)cc.lane[m0 + m] * lane_pool_m + (size_t)cc.dst[m0 + m] * D + d] = mu;
+        for (int b = 0; b < WB; ++b)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int m = 8 * (i0 + b) + cq + e;
+            if (m < Mp) mu_old[b][e] = mslot(cc.lane[m0 + m], cc.src[m0 + m])[d];
           }
-        }
+#pragma unroll
+        for (int b = 0; b < WB; ++b)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int m = 8 * (i0 + b) + cq + e;
+            if (m < Mp) {
+              const float mval = __fadd_rn(v2[4 * (i0 + b) + 2 * h + e], b2d);
+              const int n = cc.vis[m0 + m];  // visits BEFORE this one
+              // mean_set[c] = (mean_set[c] * (n - 1) + mean) / n   -- fp32, true division
+              const float mu = (n == 0) ? mval : __fdiv_rn(__fadd_rn(__fmul_rn(mu_old[b][e], (float)(n - 1)), mval), (float)n);
+              mslot(cc.lane[m0 + m], cc.dst[m0 + m])[d] = mu;
+            }
+          }
+      }
     }
   }
   if (ts) ts[3] += clock64() - t_in;
@@ -890,7 +937,10 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
   unsigned char* smem = TC ? reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023)
                            : smem_raw;
   const int B = p.B, Kcap = p.Kcap, G = p.G;
-  const SmemLayout L = make_layout<H, D, C::CP, XCL, TCN, STAT>(B, Kcap, G);
+  const SmemLayout L_ = make_layout<H, D, C::CP, XCL, TCN, STAT>(B, Kcap, G);
+  const SmemLayout& L = TC ? p.tc_layout : L_;  // tensor-core engine: read from the parameter bank, no registers
+  if constexpr (TC)
+    if (p.tc_layout.total == 0) __trap();  // a launcher that did not fill tc_layout (launch_tc does)
   const int sq = STAT ? (int)(blockIdx.x % kStatGroup) : 0, sgroup = STAT ? (int)(blockIdx.x / kStatGroup) : 0;
   float* ring = reinterpret_cast<float*>(smem + L.ring);
   float* XA = reinterpret_cast<float*>(smem + L.xa);

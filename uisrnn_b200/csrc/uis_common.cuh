@@ -152,6 +152,11 @@ __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gmem_sr
       : "memory");
 }
 
+// ---- bulk prefetch of a global range into L2 (no destination, no completion; 16-byte aligned, bytes % 16 == 0) --
+__device__ __forceinline__ void prefetch_l2_bulk(const void* gmem_src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gmem_src), "r"(bytes) : "memory");
+}
+
 // ---- cp.async (LDGSTS), 16 B ---------------------------------------------------------------
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)),

@@ -7,7 +7,9 @@ cudaError_t launch_tc(const BeamParams& p, int ctas, unsigned smem, cudaStream_t
   auto kern = uis_beam_kernel<H, D, false, false, N>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  kern<<<ctas, Cfg<H, D>::BLOCK, smem, st>>>(p);
+  BeamParams q = p;
+  q.tc_layout = make_layout<H, D, kCPBeam, false, N>(p.B, p.Kcap, p.G);
+  kern<<<ctas, Cfg<H, D>::BLOCK, smem, st>>>(q);
   return cudaGetLastError();
 }
 }  // namespace
