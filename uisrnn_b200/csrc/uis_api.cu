@@ -198,6 +198,7 @@ unsigned tree_smem_bytes(int H, int D, int B, int Kcap, int L, int NI, int NLF, 
   if (H == 512 && D == 256) return uis::make_tree_layout<512, 256>(B, Kcap, L, NI, NLF, P).total;
   if (H == 256 && D == 128) return uis::make_tree_layout<256, 128>(B, Kcap, L, NI, NLF, P).total;
   if (H == 128 && D == 64) return uis::make_tree_layout<128, 64>(B, Kcap, L, NI, NLF, P).total;
+  if (H == 1024 && D == 512) return uis::make_tree_layout<1024, 512>(B, Kcap, L, NI, NLF, P).total;
   return 0xffffffffu;
 }
 
@@ -758,7 +759,7 @@ static int model_create_impl(uis_model** out, int device, int D, int H, int dept
                              const float* b2, const float* h0, const float* sigma2, double transition_bias,
                              double crp_alpha, int D_user, int H_user);
 
-// Any (hidden <= 512, dim <= 256) runs in the smallest instantiated kernel shape that holds it, zero-padded: a padded
+// Any (hidden <= 1024, dim <= 512) runs in the smallest instantiated kernel shape that holds it, zero-padded: a padded
 // hidden unit has zero weights and biases (r = z = 1/2, n = 0, so it stays at its initial 0) and feeds nothing; a
 // padded observation dimension has x = mean = 0 and adds (0 - 0)^2 * w = 0 to every Gaussian term.  Adding exact
 // zeros does not change an fp32 sum, so the results are those of a kernel instantiated for the caller's shape.
@@ -773,8 +774,6 @@ int uis_model_create(uis_model** out, int device, int D, int H, int depth, const
   if (depth < 1 || depth > uis::kMaxDepth)
     return fail(UIS_ERR_UNSUPPORTED, "rnn_depth=%d: the sm_90a kernels support 1..%d stacked GRU layers", depth, uis::kMaxDepth);
   if (D < 1 || H < 1) return fail(UIS_ERR_INVALID, "observation_dim and rnn_hidden_size must be >= 1");
-  if ((H > 512 || D > 256) && depth > 1)
-    return fail(UIS_ERR_UNSUPPORTED, "hidden=%d dim=%d with rnn_depth=%d: models above hidden=512 / dim=256 run with one GRU layer", H, D, depth);
   if (shape_supported(H, D))
     return model_create_impl(out, device, D, H, depth, w_ih, w_hh, b_ih, b_hh, w1, b1, w2, b2, h0, sigma2,
                              transition_bias, crp_alpha, D, H);

@@ -48,6 +48,10 @@ template <int H> __host__ __device__ constexpr int beam_cp() { return BeamCP<H>:
 constexpr int kCPCluster = 12;          // cluster (latency) mode: one lane per cluster, <= 12 columns per pass
 constexpr int kXchVals = 24;            // floats per thread and exchange round of the cluster K-split
 constexpr int kCPTree = 16;             // look-ahead tree kernel (shared memory goes to the node arrays instead)
+// hidden sizes above 512: at 16 columns the tree kernel's XA / XB alone would take 128 KB beside the 96 KB weight ring;
+// 8 columns leave about the node capacity of (512, 256).  make_tree_layout, the kernel and the host's sizing use this.
+template <int H> struct TreeCP { static constexpr int value = H > 512 ? 8 : kCPTree; };
+template <int H> __host__ __device__ constexpr int tree_cp() { return TreeCP<H>::value; }
 constexpr int kMaxLanes = 8;
 constexpr int kMaxBeam = 128;  // beam_size served by the look_ahead-1 kernels (phase P3 walks the winners in chunks of 32)
 constexpr int kMaxDepth = 4;             // stacked GRU layers supported on device

@@ -23,7 +23,7 @@ struct TreeLayout {
 
 template <int H, int D>
 __host__ __device__ inline TreeLayout make_tree_layout(int B, int Kcap, int L, int NI, int NLF, int P) {
-  constexpr int kCP = kCPTree;
+  constexpr int kCP = tree_cp<H>();
   TreeLayout T;
   unsigned o = 0;
   T.ring = o;     o += kStages * kStageBytes;
@@ -59,8 +59,8 @@ __host__ __device__ inline TreeLayout make_tree_layout(int B, int Kcap, int L, i
 enum { TM_PUBLISHED = 0, TM_DONE, TM_UIDX, TM_ERR, TM_NFINITE, TM_M, TM_COUNT, TM_NWIN };
 
 template <int H, int D, bool DEEP>
-__global__ void __launch_bounds__(Cfg<H, D, kCPTree>::BLOCK, 1) uis_beam_tree_kernel(const BeamParams p) {
-  using C = Cfg<H, D, kCPTree>;
+__global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tree_kernel(const BeamParams p) {
+  using C = Cfg<H, D, tree_cp<H>()>;
   constexpr int NT = C::NT, NW = C::NW, UPT = C::UPT;
   extern __shared__ __align__(128) unsigned char smem[];
   const int B = p.B, Kcap = p.Kcap, L = p.L, NI = p.node_cap, NLF = p.leaf_cap;

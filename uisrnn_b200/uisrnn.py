@@ -106,14 +106,12 @@ class UISRNN:
     self._native_lock = threading.Lock()
     if self.device.type == 'cuda':
       # say so NOW if the sm_90a kernels cannot hold this model (predict() / fit() would raise NativeError later;
-      # there is no silent fallback): hidden <= 1024, dim <= 512, 1..4 GRU layers (one layer above hidden 512 / dim 256)
-      too_big = args.rnn_hidden_size > 1024 or self.observation_dim > 512 or args.rnn_depth > 4 or (
-          args.rnn_depth > 1 and (args.rnn_hidden_size > 512 or self.observation_dim > 256))
+      # there is no silent fallback): hidden <= 1024, dim <= 512, 1..4 GRU layers at every such size
+      too_big = args.rnn_hidden_size > 1024 or self.observation_dim > 512 or args.rnn_depth > 4
       if too_big:
         self.logger.print(
             1, 'Warning: the CUDA kernels of this build hold models up to rnn_hidden_size=1024, observation_dim=512, '
-               'rnn_depth=4 (rnn_depth=1 above 512 / 256); predict() on this device will raise for this model. '
-               'Use --enable_cuda=False for it.')
+               'rnn_depth=4; predict() on this device will raise for this model. Use --enable_cuda=False for it.')
 
   def __getstate__(self):
     # the device-side twin and its lock are per-process; pickled copies (forkserver workers of
