@@ -36,7 +36,8 @@ typedef enum uis_status {
   UIS_ERR_CUDA = -3,        /* a CUDA runtime call failed; uis_last_error() has the string     */
   UIS_ERR_OVERFLOW = -4,    /* a hypothesis opened more than `kcap` clusters; retry with more  */
   UIS_ERR_NOMEM = -5,
-  UIS_ERR_CAPACITY = -6     /* look_ahead >= 2: a beam step's candidate tree outgrew on-chip storage */
+  UIS_ERR_CAPACITY = -6     /* look_ahead >= 2: a beam step's candidate tree exhausted the device-memory arena
+                               of the spill kernel (budget: UISRNN_B200_TREE_SPILL_MB)                   */
 } uis_status;
 
 typedef struct uis_model uis_model; /* opaque */

@@ -1,5 +1,5 @@
 """Decode throughput of the (hidden 1024, dim 512) kernels: frames/s for 264 x 500-frame utterances on a seeded synthetic
-model at rnn_depth 1 / 2 / 4 with look_ahead 1 and at look_ahead 2 (beam 10) with rnn_depth 1 / 2.  Labels must be
+model at rnn_depth 1 / 2 / 4 with look_ahead 1 and at look_ahead 2 and 3 (beam 10) with rnn_depth 1 / 2.  Labels must be
 identical across the repeats.  The card's name and power limit are printed by the same run.
 
 The model is untrained; sigma2 = 0.02 keeps its decodes at a handful of clusters per utterance (max_k is printed),
@@ -43,7 +43,7 @@ def main():
   labels = torch.empty(U * N, dtype=torch.int32, device='cuda')
   off = np.arange(U + 1, dtype=np.int64) * N
   start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  for depth, la in ((1, 1), (2, 1), (4, 1), (1, 2), (2, 2)):
+  for depth, la in ((1, 1), (2, 1), (4, 1), (1, 2), (2, 2), (1, 3), (2, 3)):
     model = native.NativeModel(synthetic_model(depth))
     kcap, refused = 0, None
     while True:  # grow the cluster tables until the decode fits, as UISRNN.predict does
@@ -54,7 +54,7 @@ def main():
         model.stats()  # an asynchronous call reports the utterances' status here
         break
       except native.NativeError as err:
-        if err.code == native.UIS_ERR_CAPACITY:  # a step's look-ahead tree outgrew the on-chip node arrays
+        if err.code == native.UIS_ERR_CAPACITY:  # a step's look-ahead tree exhausted the spill arena's budget
           refused = str(err)
           break
         if err.code != native.UIS_ERR_OVERFLOW or kcap >= 128:

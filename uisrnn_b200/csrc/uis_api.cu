@@ -159,11 +159,15 @@ struct uis_model {
   int log_cap = 0;
   // workspace
   DevBuf x64, x32, gi, row_off, order, pool_mean, pool_hidden, pool_mse, bp, queue_stats, labels, status;
+  DevBuf tree_arena;  // look-ahead spill kernel: [spill CTAs][make_tree_arena(..).total]
   DevBuf dbg_win, dbg_score, dbg_off, dbg_final_scores, dbg_final_k, dbg_best_mean, dbg_best_hidden,
       dbg_best_blocks;
   // last call
   uis_stats stats{};
   int last_U = 0;
+  bool last_tree_spill = false;  // the last call ran the look-ahead spill kernel (its caps name the arena in errors)
+  int last_spill_ni = 0, last_spill_nlf = 0;
+  size_t last_spill_budget = 0;
   cudaStream_t last_stream = nullptr;
   bool stats_pending = false;
   cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};  // before prepass, after prepass, after beam kernel
@@ -202,14 +206,19 @@ unsigned tree_smem_bytes(int H, int D, int B, int Kcap, int L, int NI, int NLF, 
   return 0xffffffffu;
 }
 
-int dispatch_tree(int H, int D, const uis::BeamParams& p, int ctas, cudaStream_t st) {
-  const unsigned smem = tree_smem_bytes(H, D, p.B, p.Kcap, p.L, p.node_cap, p.leaf_cap, p.P);
+// spill: the kernel whose tree-sized arrays live in p.tree_arena; its shared memory holds the rest and a small scratch
+int dispatch_tree(int H, int D, const uis::BeamParams& p, int ctas, bool spill, cudaStream_t st) {
+  const unsigned smem = spill ? tree_smem_bytes(H, D, p.B, p.Kcap, p.L, 0, 0, 0) + uis::kTreeSpillScratch
+                              : tree_smem_bytes(H, D, p.B, p.Kcap, p.L, p.node_cap, p.leaf_cap, p.P);
   if (smem > 227u * 1024u)
     return fail(UIS_ERR_UNSUPPORTED, "look_ahead=%d beam_size=%d kcap=%d needs %u B of shared memory (> 227 KB)", p.L,
                 p.B, p.Kcap, smem);
   cudaError_t e = cudaSuccess;
-  if (!uis::launch_tree_large(H, D, p, ctas, smem, st, &e) && !uis::launch_tree_small(H, D, p, ctas, smem, st, &e))
-    return fail(UIS_ERR_UNSUPPORTED, "no sm_90a kernel instantiated for hidden=%d dim=%d", H, D);
+  const bool have = spill ? uis::launch_tree_spill_large(H, D, p, ctas, smem, st, &e) ||
+                                uis::launch_tree_spill_small(H, D, p, ctas, smem, st, &e)
+                          : uis::launch_tree_large(H, D, p, ctas, smem, st, &e) ||
+                                uis::launch_tree_small(H, D, p, ctas, smem, st, &e);
+  if (!have) return fail(UIS_ERR_UNSUPPORTED, "no sm_90a kernel instantiated for hidden=%d dim=%d", H, D);
   if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "look-ahead kernel launch failed: %s", cudaGetErrorString(e));
   return 0;
 }
@@ -367,8 +376,64 @@ struct Plan {
   int tcn = 0;      // > 0: tensor-core beam kernel with this many columns per pass (uis_beam_tc.cuh)
   bool cluster_forced = false;
   int node_cap = 0, leaf_cap = 0, maxTN = 0, maxSteps = 0;  // look_ahead >= 2 only
+  // look_ahead >= 2: the spill kernel that decodes, from a device-memory arena, what outgrew shared memory
+  int spill = 0;  // 0 off, 1 after the shared-memory kernel, 2 instead of it (UISRNN_B200_TREE_SPILL=force)
+  int spill_ctas = 0, spill_ni = 0, spill_nlf = 0, spill_P = 0;
+  size_t spill_arena = 0, spill_budget = 0;  // arena bytes per spill CTA; the budget they were sized from
   long long rows;
 };
+
+// Pool slots held by a plan's CTAs: the shared-memory kernel's and the spill kernel's run one after the other on the
+// same stream and share the pools.
+size_t pool_slots(const Plan& pl) {
+  return std::max((size_t)pl.ctas * pl.G * pl.P, (size_t)pl.spill_ctas * pl.spill_P);
+}
+
+// Sizes the spill kernel of a look-ahead plan.  The worst-case tree of one beam step at (B, Kcap, L) has
+// B * sum_{i=1}^{L-1} prod_{j<i} (Kcap + 1 + j) interior nodes plus the B winners, and B * prod_{j<L} (Kcap + 1 + j)
+// leaves.  Each spill CTA needs an arena for that tree and slot pools for its P; both are clipped (in proportion) to
+// the byte budget: UISRNN_B200_TREE_SPILL_MB, else the smaller of 2 GiB and a quarter of the free device memory.
+void plan_tree_spill(uis_model* m, Plan* pl) {
+  pl->spill = 1;
+  if (const char* env = std::getenv("UISRNN_B200_TREE_SPILL")) {
+    if (std::strcmp(env, "force") == 0) pl->spill = 2;
+    else if (env[0] == '0') pl->spill = 0;
+  }
+  if (!pl->spill) return;
+  size_t budget;
+  if (const char* env = std::getenv("UISRNN_B200_TREE_SPILL_MB")) {
+    budget = (size_t)std::max(0ll, std::atoll(env)) << 20;
+  } else {
+    size_t free_b = 0, total_b = 0;
+    uis::DeviceGuard g(m->device);
+    if (g.status != cudaSuccess || cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { (void)cudaGetLastError(); free_b = 0; }
+    budget = std::min<size_t>((size_t)2 << 30, (free_b + m->tree_arena.cap) / 4);  // the arena held is re-used
+  }
+  const int B = pl->B, K = pl->Kcap, L = pl->L;
+  const double slot_bytes = 4.0 * (m->D + m->depth * m->H + 1);
+  double ni = B, prod = 1;
+  for (int i = 1; i < L; ++i) { prod *= K + i; ni += B * prod; }
+  double nlf = B * prod * (K + L);
+  auto cost = [&](double n, double l) {
+    const int P = B * K + (int)n + B + 1;
+    return (double)uis::make_tree_arena((int)n, (int)l, P).total + P * slot_bytes;
+  };
+  // leaf positions are stored in 32 bits, parent node indices in 24 (l_pc = parent << 8 | cluster)
+  const double kMaxNi = (1 << 24) - 1, kMaxLeaves = 1 << 30;
+  if (ni > kMaxNi) { nlf *= kMaxNi / ni; ni = kMaxNi; }
+  if (nlf > kMaxLeaves) { ni *= kMaxLeaves / nlf; nlf = kMaxLeaves; }
+  for (double f = std::min(1.0, (double)budget / cost(ni, nlf)); cost(ni, nlf) > (double)budget && ni > 64; f = 0.9) {
+    ni = std::floor(ni * f);
+    nlf = std::floor(nlf * f);
+  }
+  pl->spill_ni = std::max(64, (int)ni);  // floor: one CTA with about the smallest on-chip tree
+  pl->spill_nlf = std::max(8 * 64, (int)nlf);
+  pl->spill_P = B * K + pl->spill_ni + B + 1;
+  const double per_cta = cost(pl->spill_ni, pl->spill_nlf);
+  pl->spill_ctas = (int)std::max(1.0, std::min((double)pl->ctas, std::floor((double)budget / per_cta)));
+  pl->spill_arena = uis::make_tree_arena(pl->spill_ni, pl->spill_nlf, pl->spill_P).total;
+  pl->spill_budget = budget;
+}
 
 int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o, Plan* pl, bool has_taps = false) {
   if (!m || !o || (U > 0 && !off)) return fail(UIS_ERR_INVALID, "null argument");
@@ -460,6 +525,7 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
   if (tree && o->engine == 2) return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: look_ahead must be 1");
   pl->G = G;
   pl->ctas = std::max(1, std::min(ctas, std::max((U + G - 1) / G, 1)));
+  if (tree) plan_tree_spill(m, pl);
   // Cluster (latency) mode: with fewer utterances than SMs, a thread-block cluster of 2/4/8 CTAs works on
   // each utterance (k-split of every weight matrix, uis_beam.cuh).  opts->cluster: 0 = auto (largest of 4, 2
   // that still gives every utterance its own cluster), -1 = off, 2/4/8 = forced; UISRNN_B200_CLUSTER=0 disables
@@ -518,7 +584,8 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
 size_t workspace_bytes(const uis_model* m, const Plan& pl, int U) {
   size_t b = 0;
   b += (size_t)pl.rows * 3 * m->H * 4;                                  // gi
-  b += (size_t)pl.ctas * pl.G * pl.P * (m->D + m->depth * m->H + 1) * 4;  // slot pools (+ Gaussian term per slot)
+  b += pool_slots(pl) * (m->D + m->depth * m->H + 1) * 4;            // slot pools (+ Gaussian term per slot)
+  b += (size_t)pl.spill_ctas * pl.spill_arena;                          // look-ahead spill arenas
   b += (size_t)pl.ctas * pl.G * (pl.L > 1 ? (size_t)pl.maxTN + pl.maxSteps : (size_t)pl.maxN) * pl.B * 4;  // back-pointers
   b += (size_t)(U + 1) * 8 + (size_t)U * 8 + 256;                       // offsets, order, status
   if (pl.tcn) b += (size_t)pl.ctas * pl.tcn * m->H * 4;                 // a = relu(W1 h' + b1) between two products
@@ -535,6 +602,8 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   m->stats.lanes = pl.G;
   m->stats.cluster = pl.cluster;
   m->last_U = U;
+  m->last_tree_spill = pl.L > 1 && pl.spill;
+  m->last_spill_ni = pl.spill_ni; m->last_spill_nlf = pl.spill_nlf; m->last_spill_budget = pl.spill_budget;
   m->last_stream = st;
   m->stats_pending = false;
   if (U == 0 || pl.rows == 0) {
@@ -556,9 +625,11 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   if (int rc = m->status.ensure(U * sizeof(int))) return rc;
   if (int rc = m->queue_stats.ensure(40 * sizeof(unsigned long long))) return rc;
   if (int rc = m->gi.ensure((size_t)pl.rows * 3 * H * sizeof(float))) return rc;
-  if (int rc = m->pool_mean.ensure((size_t)pl.ctas * pl.G * pl.P * D * sizeof(float))) return rc;
-  if (int rc = m->pool_hidden.ensure((size_t)pl.ctas * pl.G * pl.P * m->depth * H * sizeof(float))) return rc;
-  if (int rc = m->pool_mse.ensure((size_t)pl.ctas * pl.G * pl.P * sizeof(float))) return rc;
+  if (int rc = m->pool_mean.ensure(pool_slots(pl) * D * sizeof(float))) return rc;
+  if (int rc = m->pool_hidden.ensure(pool_slots(pl) * m->depth * H * sizeof(float))) return rc;
+  if (int rc = m->pool_mse.ensure(pool_slots(pl) * sizeof(float))) return rc;
+  if (pl.spill)
+    if (int rc = m->tree_arena.ensure((size_t)pl.spill_ctas * pl.spill_arena)) return rc;
   if (int rc = m->bp.ensure((size_t)pl.ctas * pl.G * (pl.L > 1 ? (size_t)pl.maxTN + pl.maxSteps : (size_t)pl.maxN) * pl.B *
                             sizeof(unsigned)))
     return rc;
@@ -678,15 +749,27 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
     if (!uis::launch_beam_tc(H, D, pl.tcn, p, pl.ctas, uis::beam_tc_smem(H, D, pl.tcn, pl.B, pl.Kcap, pl.G), st, &e))
       return fail(UIS_ERR_UNSUPPORTED, "no tensor-core kernel for hidden=%d dim=%d columns=%d", H, D, pl.tcn);
     if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "tensor-core beam kernel launch failed: %s", cudaGetErrorString(e));
-  } else if (int rc = (pl.L > 1 ? dispatch_tree(H, D, p, pl.ctas, st)
-                                : dispatch_beam(H, D, p, pl.ctas, &cluster_used, pl.cluster_forced, st))) {
+  } else if (pl.L > 1) {
+    if (pl.spill != 2)
+      if (int rc = dispatch_tree(H, D, p, pl.ctas, false, st)) return rc;
+    if (pl.spill) {
+      // right behind it on the same stream: the utterances it left at status -5 (every one when forced), from a
+      // second queue; its CTAs find nothing to do and exit when every tree fitted
+      uis::BeamParams ps = p;
+      ps.node_cap = pl.spill_ni; ps.leaf_cap = pl.spill_nlf; ps.P = pl.spill_P;
+      ps.queue = p.queue + 1;
+      ps.tree_arena = m->tree_arena.as<unsigned char>();
+      ps.tree_spill_all = pl.spill == 2;
+      if (int rc = dispatch_tree(H, D, ps, pl.spill_ctas, true, st)) return rc;
+    }
+  } else if (int rc = dispatch_beam(H, D, p, pl.ctas, &cluster_used, pl.cluster_forced, st)) {
     return rc;
   }
   m->stats.cluster = cluster_used;
   m->stats.engine = pl.tcn ? 2 : 1;
   m->stats.tc_columns = pl.tcn;
   CU(cudaEventRecord(m->ev[2], st));
-  m->stats.kernel_launches = 2;
+  m->stats.kernel_launches = 2 + (pl.L > 1 && pl.spill == 1 ? 1 : 0);
   m->stats_pending = true;
 
   if (taps) {
@@ -738,6 +821,10 @@ int collect(uis_model* m) {
     else if (v == -5) ++capacity;
     else if (v != 0) ++bad;
   }
+  if (capacity && m->last_tree_spill)
+    return fail(UIS_ERR_CAPACITY, "%d utterance(s): the look-ahead tree of one beam step exhausted the device-memory arena "
+                "(%d nodes / %d leaves per CTA from a budget of %zu MiB; raise UISRNN_B200_TREE_SPILL_MB or lower "
+                "beam_size / look_ahead / kcap)", capacity, m->last_spill_ni, m->last_spill_nlf, m->last_spill_budget >> 20);
   if (capacity)
     return fail(UIS_ERR_CAPACITY, "%d utterance(s): the look-ahead tree of one beam step outgrew the on-chip node arrays "
                 "(lower beam_size / look_ahead / kcap)", capacity);
@@ -932,7 +1019,8 @@ int uis_model_destroy(uis_model* m) {
                     &m->hidden0, &m->wih_up_t, &m->logn, &m->logtot, &m->x64, &m->x32, &m->gi, &m->row_off, &m->order,
                     &m->pool_mean, &m->pool_hidden, &m->bp, &m->queue_stats, &m->labels, &m->status, &m->dbg_win,
                     &m->dbg_score, &m->dbg_off, &m->dbg_final_scores, &m->dbg_final_k, &m->dbg_best_mean,
-                    &m->dbg_best_hidden, &m->dbg_best_blocks, &m->tc_planes, &m->tc_scratch, &m->pool_mse, &m->stat_bar, &m->stat_scratch};
+                    &m->dbg_best_hidden, &m->dbg_best_blocks, &m->tc_planes, &m->tc_scratch, &m->pool_mse, &m->stat_bar, &m->stat_scratch,
+                    &m->tree_arena};
   for (DevBuf* b : bufs) b->release();
   for (auto& e : m->ev)
     if (e) cudaEventDestroy(e);
@@ -1151,7 +1239,7 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
   }
   CU(cudaEventRecord(m->ev_h2d[1], cs));
   if (int rc = run_device(m, m->x32.as<float>(), off, U, pl, m->labels.as<int32_t>(), taps, st, /*gi_ready=*/true)) return rc;
-  m->stats.kernel_launches = 1 + 2 * (int64_t)n_chunks;
+  m->stats.kernel_launches = 1 + 2 * (int64_t)n_chunks + (pl.L > 1 && pl.spill == 1 ? 1 : 0);
   m->stats.chunks = n_chunks;
   m->stats.staged = staged ? 1 : 0;
   CU(cudaMemcpyAsync(m->labels_pin, m->labels.p, rows * 4, cudaMemcpyDeviceToHost, st));

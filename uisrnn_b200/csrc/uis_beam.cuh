@@ -127,6 +127,9 @@ struct BeamParams {
   float* dbg_best_mean;    // [Kcap][D]
   float* dbg_best_hidden;  // [Kcap][depth][H]
   int* dbg_best_blocks;    // [Kcap]
+  // look-ahead spill kernel (uis_beam_tree.cuh, SPILL = true); these fit the struct's tail padding (sizeof stays 768)
+  unsigned char* tree_arena;  // [ctas][make_tree_arena(node_cap, leaf_cap, P).total]
+  int tree_spill_all;         // 1: decode every utterance, not only those the shared-memory kernel left at status -5
 };
 
 template <int V> struct Pow2Floor { static constexpr int value = (V >= 2) ? 2 * Pow2Floor<V / 2>::value : 1; };

@@ -56,15 +56,130 @@ __host__ __device__ inline TreeLayout make_tree_layout(int B, int Kcap, int L, i
   return T;
 }
 
+// Spill policy: the arrays whose size follows the tree (nodes, leaves, columns, slot map and free bitmap) live in a
+// per-CTA arena in device memory; everything else keeps its shared-memory place (make_tree_layout with no nodes).
+struct TreeArena {
+  size_t n_parent, n_c, n_nl, n_k, n_tot, n_ov, l_pc, l_key, colsrc, colnew, colvis, colrow, collane, colmap, used, total;
+};
+
+__host__ __device__ inline TreeArena make_tree_arena(int NI, int NLF, int P) {
+  TreeArena A;
+  size_t o = 0;
+  const size_t ni = (size_t)NI, nl = (size_t)NLF, np = (size_t)P;
+  auto take = [&](size_t bytes) { const size_t at = o; o += (bytes + 127) / 128 * 128; return at; };
+  A.n_parent = take(ni * 4); A.n_c = take(ni * 4); A.n_nl = take(ni * 4); A.n_k = take(ni * 4); A.n_tot = take(ni * 4);
+  A.n_ov = take(ni * 16);
+  A.l_pc = take(nl * 4); A.l_key = take(nl * 8);
+  A.colsrc = take(ni * 4); A.colnew = take(ni * 4); A.colvis = take(ni * 4); A.colrow = take(ni * 8); A.collane = take(ni * 4);
+  A.colmap = take(np * 4); A.used = take((np + 31) / 32 * 4);
+  A.total = o;
+  return A;
+}
+
+// Shared scratch of the spill kernel, after make_tree_layout(..).total: the survivors of the leaf selection
+// (<= 32 keys), the 256-bucket radix histogram, the warp totals of the block scan and 4 broadcast words.
+constexpr unsigned kTreeSpillScratch = 32 * 8 + 256 * 4 + 36 * 4 + 4 * 4;
+
+// Exclusive prefix sum of v over the NT consumer threads; *total = the sum of all.  sc: >= 33 ints of shared memory.
+template <int NT>
+__device__ __forceinline__ int block_excl_scan(int v, int* sc, int* total, int lane, int warp) {
+  int incl = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+  if (lane == 31) sc[warp] = incl;
+  named_bar_sync(1, NT);
+  if (warp == 0) {
+    const int w = (lane < NT / 32) ? sc[lane] : 0;
+    int wi = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, wi, o); if (lane >= o) wi += t; }
+    sc[lane] = wi - w;
+    if (lane == 31) sc[32] = wi;
+  }
+  named_bar_sync(1, NT);
+  const int r = sc[warp] + incl - v;
+  *total = sc[32];
+  named_bar_sync(1, NT);
+  return r;
+}
+
+// Leaf positions of the nwin (1..32) smallest of the n unique keys, in ascending key order, into wins[0..nwin).
+// MSD radix select over 8-bit digits finds the nwin-th smallest key; the nwin keys at or below it are then ranked.
+// Any exact selection of unique keys gives what the on-chip counting rank gives.
+template <int NT>
+__device__ void tree_select_smallest(const unsigned long long* key, int n, int nwin, int* wins, unsigned char* scratch,
+                                     int tid, int lane, int warp) {
+  unsigned long long* surv = reinterpret_cast<unsigned long long*>(scratch);
+  unsigned* hist = reinterpret_cast<unsigned*>(scratch + 32 * 8);
+  volatile int* sel = reinterpret_cast<volatile int*>(scratch + 32 * 8 + 256 * 4 + 36 * 4);
+  unsigned long long prefix = 0, mask = 0;
+  int k = nwin;  // rank of the nwin-th smallest key among the keys that equal `prefix` under `mask`
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    for (int i = tid; i < 256; i += NT) hist[i] = 0;
+    named_bar_sync(1, NT);
+    for (int f0 = warp * 32; f0 < n; f0 += NT) {
+      const int f = f0 + lane;
+      unsigned d = 256;
+      if (f < n) { const unsigned long long x = key[f]; if ((x & mask) == prefix) d = (unsigned)(x >> shift) & 255u; }
+      const unsigned peers = __match_any_sync(0xffffffffu, d);
+      if (d < 256 && lane == __ffs(peers) - 1) atomicAdd(&hist[d], (unsigned)__popc(peers));
+    }
+    named_bar_sync(1, NT);
+    if (warp == 0) {  // the bucket that holds the k-th key: lane l owns buckets 8l .. 8l+7
+      unsigned c[8];
+      int s = 0;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { c[i] = hist[8 * lane + i]; s += (int)c[i]; }
+      int incl = s;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+      const int excl = incl - s;
+      if (excl < k && k <= incl) {
+        int cum = excl;
+        for (int i = 0; i < 8; ++i) {
+          if (cum + (int)c[i] >= k) { sel[0] = 8 * lane + i; sel[1] = k - cum; sel[2] = (int)c[i]; break; }
+          cum += (int)c[i];
+        }
+      }
+    }
+    named_bar_sync(1, NT);
+    prefix |= (unsigned long long)sel[0] << shift;
+    mask |= 255ull << shift;
+    k = sel[1];
+    if (sel[2] == 1) break;  // the nwin-th smallest key is the only one with this prefix
+  }
+  // the keys below `prefix` under `mask` plus the one equal to it: exactly the nwin smallest
+  if (tid == 0) sel[3] = 0;
+  named_bar_sync(1, NT);
+  for (int f = tid; f < n; f += NT) {
+    const unsigned long long x = key[f];
+    if ((x & mask) <= prefix) {
+      const int s = atomicAdd((int*)&sel[3], 1);
+      if (s < nwin) surv[s] = x;
+    }
+  }
+  named_bar_sync(1, NT);
+  if (tid < nwin) {
+    const unsigned long long x = surv[tid];
+    int rank = 0;
+    for (int q = 0; q < nwin; ++q) rank += (surv[q] < x) ? 1 : 0;
+    wins[rank] = (int)(unsigned)x;  // low 32 bits: the leaf position
+  }
+}
+
 enum { TM_PUBLISHED = 0, TM_DONE, TM_UIDX, TM_ERR, TM_NFINITE, TM_M, TM_COUNT, TM_NWIN };
 
-template <int H, int D, bool DEEP>
+// SPILL = false: the whole tree of a beam step lives in shared memory (node_cap / leaf_cap sized by the host to what
+// fits), and an utterance whose tree outgrows it ends with status -5.  SPILL = true: the tree-sized arrays live in a
+// device-memory arena of node_cap / leaf_cap entries per CTA (p.tree_arena), and the kernel decodes only the
+// utterances left at status -5 by the shared-memory kernel (all of them with p.tree_spill_all).
+template <int H, int D, bool DEEP, bool SPILL = false>
 __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tree_kernel(const BeamParams p) {
   using C = Cfg<H, D, tree_cp<H>()>;
   constexpr int NT = C::NT, NW = C::NW, UPT = C::UPT;
   extern __shared__ __align__(128) unsigned char smem[];
   const int B = p.B, Kcap = p.Kcap, L = p.L, NI = p.node_cap, NLF = p.leaf_cap;
-  const TreeLayout T = make_tree_layout<H, D>(B, Kcap, L, NI, NLF, p.P);
+  const TreeLayout T = make_tree_layout<H, D>(B, Kcap, L, SPILL ? 0 : NI, SPILL ? 0 : NLF, SPILL ? 0 : p.P);
   float* ring = reinterpret_cast<float*>(smem + T.ring);
   float* XA = reinterpret_cast<float*>(smem + T.xa);
   float* XB = reinterpret_cast<float*>(smem + T.xb);
@@ -89,6 +204,26 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
   int* colmap = reinterpret_cast<int*>(smem + T.colmap);
   unsigned* used = reinterpret_cast<unsigned*>(smem + T.used);
   int* wins = reinterpret_cast<int*>(smem + T.wins);
+  if constexpr (SPILL) {  // the tree-sized arrays move to this CTA's arena
+    const TreeArena A = make_tree_arena(NI, NLF, p.P);
+    unsigned char* const ar = p.tree_arena + (size_t)blockIdx.x * A.total;
+    n_parent = reinterpret_cast<int*>(ar + A.n_parent);
+    n_c = reinterpret_cast<int*>(ar + A.n_c);
+    n_nl = reinterpret_cast<float*>(ar + A.n_nl);
+    n_k = reinterpret_cast<int*>(ar + A.n_k);
+    n_tot = reinterpret_cast<int*>(ar + A.n_tot);
+    n_ov = reinterpret_cast<TabEntry*>(ar + A.n_ov);
+    l_pc = reinterpret_cast<unsigned*>(ar + A.l_pc);
+    l_key = reinterpret_cast<unsigned long long*>(ar + A.l_key);
+    colsrc = reinterpret_cast<int*>(ar + A.colsrc);
+    colnew = reinterpret_cast<int*>(ar + A.colnew);
+    colvis = reinterpret_cast<int*>(ar + A.colvis);
+    colrow = reinterpret_cast<long long*>(ar + A.colrow);
+    collane = reinterpret_cast<int*>(ar + A.collane);
+    colmap = reinterpret_cast<int*>(ar + A.colmap);
+    used = reinterpret_cast<unsigned*>(ar + A.used);
+  }
+  unsigned char* const spill_scratch = smem + T.total;  // kTreeSpillScratch bytes, SPILL only
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + T.bars);
   uint64_t* empty = full + kStages;
   volatile int* misc = reinterpret_cast<volatile int*>(smem + T.misc);
@@ -241,6 +376,9 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
     const int uidx = misc[TM_UIDX];
     if (uidx >= p.U) break;
     const int u = p.order[uidx];
+    if constexpr (SPILL) {  // decoded by the shared-memory kernel (or failed there for another reason)
+      if (!p.tree_spill_all && p.status[u] != -5) { named_bar_sync(1, NT); continue; }
+    }
     const long long row0 = p.row_off[u];
     const int N = (int)(p.row_off[u + 1] - row0);
     const int TN = p.T * N;
@@ -286,8 +424,30 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
       for (int level = 1; level <= Lc; ++level) {
         const bool last = (level == Lc);
         const int pa = (level == 1) ? 0 : lvl[level - 1], pb = (level == 1) ? nb : lvl[level];
-        // children offsets (serial over parents; at most a few hundred)
-        if (tid == 0) {
+        if constexpr (SPILL) {
+          // children offsets: block-wide prefix sum over the parents' K + 1 fan-outs, NT parents at a time
+          const int base = lvl[level];
+          const int cap = last ? NLF : NI - base;
+          int* sc = reinterpret_cast<int*>(spill_scratch + 32 * 8 + 256 * 4);
+          int tot = 0;
+          for (int q0 = pa; q0 < pb; q0 += NT) {
+            const int q = q0 + tid;
+            const int Kp = (q < pb) ? ((level == 1) ? mK[q] : n_k[q]) : -1;
+            int chunk;
+            const int o = tot + block_excl_scan<NT>(Kp + 1, sc, &chunk, lane, warp);
+            if (chunk > cap - tot) { if (tid == 0) misc[TM_ERR] = 3; break; }
+            for (int c = 0; c <= Kp; ++c) {
+              if (last) l_pc[o + c] = ((unsigned)q << 8) | (unsigned)c;
+              else { n_parent[base + o + c] = q; n_c[base + o + c] = c; }
+            }
+            tot += chunk;
+          }
+          if (tid == 0) {
+            misc[TM_COUNT] = tot;
+            if (!last) lvl[level + 1] = base + tot;
+            st_cand += tot;
+          }
+        } else if (tid == 0) {  // children offsets (serial over parents; at most a few hundred)
           int tot = 0;
           const int base = lvl[level];
           for (int q = pa; q < pb; ++q) {
@@ -368,7 +528,20 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
       // ---- rank the leaves (uisrnn.py:546-552): key = (score, flat index of the index tuple)
       if (tid == 0) misc[TM_NFINITE] = 0;
       named_bar_sync(1, NT);
-      for (int f = tid; f < n_leaves; f += NT) {
+      if constexpr (SPILL) {
+        // Leaves are enumerated in lexicographic order of their index tuples (hypothesis, c_1 .. c_L'), the order of
+        // the flat index, so the leaf position breaks ties exactly as the flat index does.  It is below leaf_cap, so
+        // it fits the low 32 bits at any arena size, where the flat index itself may not.
+        int fin = 0;
+        for (int f = tid; f < n_leaves; f += NT) {
+          const unsigned skey = (unsigned)(l_key[f] >> 32);
+          l_key[f] = ((unsigned long long)skey << 32) | (unsigned)f;
+          fin += (skey < float_order_key(INF)) ? 1 : 0;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) fin += __shfl_xor_sync(0xffffffffu, fin, o);
+        if (lane == 0 && fin) atomicAdd((int*)&misc[TM_NFINITE], fin);
+      } else for (int f = tid; f < n_leaves; f += NT) {
         int chain[8];
         int lev = Lc - 1, n = (int)(l_pc[f] >> 8);
         chain[Lc - 1] = (int)(l_pc[f] & 255u);
@@ -381,7 +554,9 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
       }
       named_bar_sync(1, NT);
       const int nwin = min((int)misc[TM_NFINITE], B);
-      for (int f = tid; f < n_leaves; f += NT) {
+      if constexpr (SPILL) {
+        if (nwin > 0) tree_select_smallest<NT>(l_key, n_leaves, nwin, wins, spill_scratch, tid, lane, warp);
+      } else for (int f = tid; f < n_leaves; f += NT) {
         const unsigned long long k = l_key[f];
         int rank = 0;
         for (int q = 0; q < n_leaves; ++q) rank += (l_key[q] < k) ? 1 : 0;

@@ -21,6 +21,9 @@ unsigned beam_tc_smem(int H, int D, int N, int B, int Kcap, int G);
 bool launch_beam_tc(int H, int D, int N, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st, cudaError_t* err);
 bool launch_tree_large(int H, int D, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st, cudaError_t* err);
 bool launch_tree_small(int H, int D, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st, cudaError_t* err);
+// the same shapes with the tree-sized arrays in a device-memory arena (p.tree_arena)
+bool launch_tree_spill_large(int H, int D, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st, cudaError_t* err);
+bool launch_tree_spill_small(int H, int D, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st, cudaError_t* err);
 
 template <class Kern>
 inline cudaError_t launch_with_smem(Kern kern, const BeamParams& p, int ctas, int block, unsigned smem, cudaStream_t st) {
