@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define UIS_ABI_VERSION 4
+#define UIS_ABI_VERSION 5
 
 typedef enum uis_status {
   UIS_OK = 0,
@@ -164,6 +164,31 @@ int uis_predict(uis_model* m, const double* const* seqs, const int64_t* n_frames
 int uis_predict_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
                        const uis_predict_opts* opts, int32_t* labels_dev,
                        const uis_debug_taps* taps, void* stream);
+
+/*
+ * ABI 5: the same searches with a bound on the number of speakers (clusters) per utterance.  Not in the reference,
+ * whose only knob is crp_alpha.  The three extra arguments, any of which may be NULL:
+ *   max_speakers [U] HOST int32: 0 = no bound, else >= 1.  A candidate that would take its hypothesis past
+ *                    max_speakers clusters scores +inf (it is never generated), so every label is < max_speakers
+ *                    and, with kcap >= max_speakers, UIS_ERR_OVERFLOW cannot occur for that utterance.  Ranking and
+ *                    tie-breaking are those of the unbounded search.
+ *   min_speakers [U] HOST int32: 0 = no bound, else <= max_speakers when that is set.  Applied at the end only: the
+ *                    labels come from the best-ranked final hypothesis with at least min_speakers clusters, or from
+ *                    rank 0 when the final beam holds none (speakers_out then reports fewer than min_speakers).
+ *   speakers_out [U] int32 (HOST for uis_predict_bounded, DEVICE for uis_predict_device_bounded): clusters of the
+ *                    returned hypothesis, 0 for an empty or failed utterance.
+ * "Speakers" counts clusters over the whole tiled decode (test_iteration copies): with test_iteration > 1 the
+ * returned last copy may use fewer distinct ids.  Any other value is UIS_ERR_INVALID.  Both bounds NULL (or 0)
+ * decode exactly as uis_predict / uis_predict_device, which are these calls with three NULLs.
+ * Workspace: a call with bounds holds 8 * U more device bytes, and uis_predict_bounded with speakers_out 4 * U more,
+ * beyond uis_predict_workspace_bytes().
+ */
+int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                        const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
+                        const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out);
+int uis_predict_device_bounded(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                               const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
+                               const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev);
 
 /* Device bytes uis_predict_device() will hold for this problem (workspace is cached in the handle). */
 size_t uis_predict_workspace_bytes(uis_model* m, const int64_t* frame_offsets, int U,

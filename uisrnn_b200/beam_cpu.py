@@ -93,7 +93,7 @@ class CpuBeamSearch:
         break
     return child
 
-  def _score_table(self, hyp, frames):
+  def _score_table(self, hyp, frames, max_speakers=0):
     depth = frames.shape[0]
     count = len(hyp.means)
     table = np.full([count + 1 + i for i in range(depth)], np.inf)
@@ -101,6 +101,8 @@ class CpuBeamSearch:
     def walk(state, level, prefix):
       last = level == depth - 1
       for cluster in range(table.shape[level]):
+        if max_speakers and cluster >= len(state.means) >= max_speakers:
+          continue  # would open a cluster past max_speakers: the whole sub-tree stays +inf
         child = _Hypothesis(state)
         if not self._advance(child, frames[level], cluster, not last):
           continue
@@ -113,8 +115,14 @@ class CpuBeamSearch:
     return table
 
   @torch.no_grad()
-  def decode(self, sequence, beam_size, look_ahead, test_iteration):
-    """`sequence`: float64 [N, D] ndarray.  Returns the N labels of the last tiled copy."""
+  def decode(self, sequence, beam_size, look_ahead, test_iteration, max_speakers=0, min_speakers=0,
+             return_speakers=False):
+    """`sequence`: float64 [N, D] ndarray.  Returns the N labels of the last tiled copy (and, with
+    return_speakers, the cluster count of the returned hypothesis).
+
+    Speaker bounds (0 = none): an index tuple that would take its hypothesis past `max_speakers` clusters
+    scores +inf; the returned hypothesis is the best-ranked final one with at least `min_speakers` clusters,
+    or rank 0 when there is none."""
     self.rnn.eval()
     length = sequence.shape[0]
     tiled = torch.from_numpy(np.tile(sequence, (test_iteration, 1))).float().to(self.device)
@@ -125,7 +133,7 @@ class CpuBeamSearch:
       widest = max(len(h.means) for h in beam)
       scores = np.full([beam_size] + [widest + 1 + i for i in range(depth)], np.inf)
       for rank, hyp in enumerate(beam):
-        table = self._score_table(hyp, frames)
+        table = self._score_table(hyp, frames, max_speakers)
         scores[rank] = np.pad(table, [(0, widest - len(hyp.means))] * depth, 'constant',
                               constant_values=np.inf)
       ranked = np.sort(scores, axis=None)
@@ -137,4 +145,6 @@ class CpuBeamSearch:
         index = np.unravel_index(order[rank], scores.shape)
         survivors.append(self._expand(beam[int(index[0])], frames, index[1:]))
       beam = survivors
-    return [int(c) for c in beam[0].trace[-length:]]
+    best = next((h for h in beam if len(h.means) >= min_speakers), beam[0])
+    labels = [int(c) for c in best.trace[-length:]]
+    return (labels, len(best.means)) if return_speakers else labels

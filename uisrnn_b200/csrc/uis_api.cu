@@ -159,6 +159,7 @@ struct uis_model {
   int log_cap = 0;
   // workspace
   DevBuf x64, x32, gi, row_off, order, pool_mean, pool_hidden, pool_mse, bp, queue_stats, labels, status;
+  DevBuf spk_bound, spk_out;  // bounded calls only: [U][2] speaker bounds; [U] speaker counts (host-buffer entry point)
   DevBuf tree_arena;  // look-ahead spill kernel: [spill CTAs][make_tree_arena(..).total]
   DevBuf dbg_win, dbg_score, dbg_off, dbg_final_scores, dbg_final_k, dbg_best_mean, dbg_best_hidden,
       dbg_best_blocks;
@@ -592,9 +593,30 @@ size_t workspace_bytes(const uis_model* m, const Plan& pl, int U) {
   return b;
 }
 
+// Speaker bounds of a bounded call (host arrays, either may be NULL): 0 = no bound, max >= 1, 0 <= min <= max.
+struct SpeakerBounds {
+  const int32_t* max = nullptr;
+  const int32_t* min = nullptr;
+  int32_t* out_dev = nullptr;  // [U] device, may be NULL
+  SpeakerBounds at(int u0) const {
+    return SpeakerBounds{max ? max + u0 : nullptr, min ? min + u0 : nullptr, out_dev ? out_dev + u0 : nullptr};
+  }
+};
+
+int check_bounds(int U, const int32_t* mx, const int32_t* mn) {
+  for (int u = 0; u < U; ++u) {
+    const int a = mx ? mx[u] : 0, b = mn ? mn[u] : 0;
+    if (a < 0 || b < 0 || (a > 0 && b > a))
+      return fail(UIS_ERR_INVALID, "utterance %d: max_speakers=%d min_speakers=%d (need max >= 1 or 0 = none, "
+                  "min >= 0, min <= max)", u, a, b);
+  }
+  return 0;
+}
+
 int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, const Plan& pl, int32_t* labels_dev,
-               const uis_debug_taps* taps, cudaStream_t st, bool gi_ready = false) {
+               const uis_debug_taps* taps, cudaStream_t st, const SpeakerBounds& sb, bool gi_ready = false) {
   const int H = m->H, D = m->D;
+  if (sb.out_dev && U > 0) CU(cudaMemsetAsync(sb.out_dev, 0, (size_t)U * sizeof(int32_t), st));  // empty inputs: 0
   m->stats = uis_stats{};
   m->stats.utterances = U;
   m->stats.frames = pl.rows;
@@ -672,6 +694,14 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   p.queue = m->queue_stats.as<int>();
   p.stats = m->queue_stats.as<unsigned long long>() + 8;
   p.labels = labels_dev; p.status = m->status.as<int>();
+  if (sb.max || sb.min) {
+    std::vector<int32_t> kb(2 * (size_t)U);
+    for (int u = 0; u < U; ++u) { kb[2 * u] = sb.max ? sb.max[u] : 0; kb[2 * u + 1] = sb.min ? sb.min[u] : 0; }
+    if (int rc = m->spk_bound.ensure(kb.size() * sizeof(int32_t))) return rc;
+    CU(cudaMemcpyAsync(m->spk_bound.p, kb.data(), kb.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    p.spk_bound = m->spk_bound.as<int>();
+  }
+  p.spk_out = sb.out_dev;
   p.trace_utt = -1;
   if (pl.stat) {
     p.stat_bar = m->stat_bar.as<unsigned>();
@@ -1060,8 +1090,15 @@ size_t uis_predict_workspace_bytes(uis_model* m, const int64_t* frame_offsets, i
 
 int uis_predict_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
                        const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream) {
+  return uis_predict_device_bounded(m, x_dev, frame_offsets, U, opts, labels_dev, taps, stream, nullptr, nullptr, nullptr);
+}
+
+int uis_predict_device_bounded(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                               const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
+                               const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev) {
   Plan pl;
   if (int rc = make_plan(m, frame_offsets, U, opts, &pl, taps != nullptr)) return rc;
+  if (int rc = check_bounds(U, max_speakers, min_speakers)) return rc;
   if (U > 0 && pl.rows > 0 && (!x_dev || !labels_dev)) return fail(UIS_ERR_INVALID, "null device buffer");
   uis::DeviceGuard device_guard_(m->device);
   CU(device_guard_.status);
@@ -1074,7 +1111,8 @@ int uis_predict_device(uis_model* m, const float* x_dev, const int64_t* frame_of
     CU(cudaGetLastError());
     x_dev = m->x32.as<float>();
   }
-  return run_device(m, x_dev, frame_offsets, U, pl, labels_dev, taps, st);
+  return run_device(m, x_dev, frame_offsets, U, pl, labels_dev, taps, st,
+                    SpeakerBounds{max_speakers, min_speakers, speakers_dev});
 }
 
 }  // extern "C"
@@ -1106,11 +1144,13 @@ size_t staging_chunk_rows(int d_user) {
 // One group of utterances, host buffers in, host buffers out: chunked H2D on the copy stream || cast + input
 // projection on `st`, then the beam kernel, then one D2H copy of all labels.
 int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
-                            const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st);
+                            const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
+                            const SpeakerBounds& sb, int32_t* speakers_out);
 
 int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
-                       const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st) {
-  const int rc = predict_host_group_impl(m, seqs, n_frames, U, off, pl, labels_out, taps, st);
+                       const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
+                       const SpeakerBounds& sb, int32_t* speakers_out) {
+  const int rc = predict_host_group_impl(m, seqs, n_frames, U, off, pl, labels_out, taps, st, sb, speakers_out);
   if (rc != 0 && rc != UIS_ERR_OVERFLOW && rc != UIS_ERR_CAPACITY) {
     // a failed call may leave copies / kernels in flight on either stream: drain them (the error already recorded in
     // uis_last_error() is the one reported) so that the staging ring and the workspace are quiescent for the next call
@@ -1124,7 +1164,8 @@ int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n
 }
 
 int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
-                            const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st) {
+                            const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
+                            const SpeakerBounds& sb_host, int32_t* speakers_out) {
   const int D = m->D_user, H = m->H;  // the caller's rows; the device rows are padded to m->D floats
   const size_t rows = (size_t)pl.rows;
   if (rows == 0) {
@@ -1140,6 +1181,11 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
   if (int rc = m->x32.ensure(rows * m->D * 4)) return rc;
   if (int rc = m->gi.ensure(rows * 3 * H * sizeof(float))) return rc;
   if (int rc = m->labels.ensure(rows * 4)) return rc;
+  SpeakerBounds sb = sb_host;  // speaker counts land in the handle's device buffer, then in `speakers_out`
+  if (speakers_out) {
+    if (int rc = m->spk_out.ensure((size_t)U * 4)) return rc;
+    sb.out_dev = m->spk_out.as<int32_t>();
+  }
   if (rows * 4 > m->labels_pin_cap) {
     if (m->labels_pin) cudaFreeHost(m->labels_pin);
     m->labels_pin = nullptr;
@@ -1238,7 +1284,8 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
     r0 = r1;
   }
   CU(cudaEventRecord(m->ev_h2d[1], cs));
-  if (int rc = run_device(m, m->x32.as<float>(), off, U, pl, m->labels.as<int32_t>(), taps, st, /*gi_ready=*/true)) return rc;
+  if (int rc = run_device(m, m->x32.as<float>(), off, U, pl, m->labels.as<int32_t>(), taps, st, sb, /*gi_ready=*/true))
+    return rc;
   m->stats.kernel_launches = 1 + 2 * (int64_t)n_chunks + (pl.L > 1 && pl.spill == 1 ? 1 : 0);
   m->stats.chunks = n_chunks;
   m->stats.staged = staged ? 1 : 0;
@@ -1246,6 +1293,7 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
   CU(cudaStreamSynchronize(st));
   for (int q = 0; q < U; ++q)
     if (n_frames[q] > 0) std::memcpy(labels_out[q], m->labels_pin + off[q], (size_t)n_frames[q] * 4);
+  if (speakers_out) CU(cudaMemcpy(speakers_out, sb.out_dev, (size_t)U * 4, cudaMemcpyDeviceToHost));
   if (int rc = collect(m)) return rc;
   CU(cudaEventElapsedTime(&m->stats.h2d_ms, m->ev_h2d[0], m->ev_h2d[1]));
   CU(cudaEventElapsedTime(&m->stats.pipeline_ms, m->ev_pipe, m->ev[1]));  // first cast -> beam kernel start
@@ -1270,8 +1318,16 @@ extern "C" {
 
 int uis_predict(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const uis_predict_opts* opts,
                 int32_t* const* labels_out, const uis_debug_taps* taps, void* stream) {
+  return uis_predict_bounded(m, seqs, n_frames, U, opts, labels_out, taps, stream, nullptr, nullptr, nullptr);
+}
+
+int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                        const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
+                        const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out) {
   if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
   if (U < 0 || (U > 0 && (!seqs || !n_frames || !labels_out))) return fail(UIS_ERR_INVALID, "null argument");
+  if (int rc = check_bounds(U, max_speakers, min_speakers)) return rc;
+  if (speakers_out && U > 0) std::memset(speakers_out, 0, (size_t)U * sizeof(int32_t));  // empty inputs: 0
   const auto t_begin = std::chrono::steady_clock::now();
   std::vector<int64_t> off(U + 1, 0);
   for (int u = 0; u < U; ++u) {
@@ -1301,7 +1357,9 @@ int uis_predict(uis_model* m, const double* const* seqs, const int64_t* n_frames
     max_rows = budget > (double)per_row ? (size_t)(budget / (double)per_row) : 1;
   }
   if ((size_t)pl.rows <= max_rows || taps || U <= 1) {
-    if (int rc = predict_host_group(m, seqs, n_frames, U, off.data(), pl, labels_out, taps, st)) return rc;
+    if (int rc = predict_host_group(m, seqs, n_frames, U, off.data(), pl, labels_out, taps, st,
+                                    SpeakerBounds{max_speakers, min_speakers}, speakers_out))
+      return rc;
     m->stats.groups = 1;
   } else {
     uis_stats total{};
@@ -1313,7 +1371,9 @@ int uis_predict(uis_model* m, const double* const* seqs, const int64_t* n_frames
       for (int q = u0; q <= u1; ++q) goff[q - u0] = off[q] - off[u0];
       Plan gp;
       if (int rc = make_plan(m, goff.data(), u1 - u0, opts, &gp, false)) return rc;
-      if (int rc = predict_host_group(m, seqs + u0, n_frames + u0, u1 - u0, goff.data(), gp, labels_out + u0, nullptr, st))
+      if (int rc = predict_host_group(m, seqs + u0, n_frames + u0, u1 - u0, goff.data(), gp, labels_out + u0, nullptr, st,
+                                      SpeakerBounds{max_speakers, min_speakers}.at(u0),
+                                      speakers_out ? speakers_out + u0 : nullptr))
         return rc;
       m->stats.groups = 1;
       add_stats(&total, m->stats);

@@ -130,7 +130,25 @@ struct BeamParams {
   // look-ahead spill kernel (uis_beam_tree.cuh, SPILL = true); these fit the struct's tail padding (sizeof stays 768)
   unsigned char* tree_arena;  // [ctas][make_tree_arena(node_cap, leaf_cap, P).total]
   int tree_spill_all;         // 1: decode every utterance, not only those the shared-memory kernel left at status -5
+  // speaker bounds (uis_predict*_bounded), indexed by utterance id; null = unbounded
+  const int* spk_bound;  // [U][2]: max_speakers (0 = none), min_speakers
+  int* spk_out;          // [U]    clusters of the returned hypothesis, 0 for a failed utterance
 };
+
+// Per-utterance speaker bounds: a hypothesis may hold at most spk_max clusters; the returned one is the best-ranked
+// final hypothesis with at least spk_min clusters (rank 0 if there is none).
+__device__ inline int spk_max(const BeamParams& p, int u) {
+  const int v = p.spk_bound ? p.spk_bound[2 * u] : 0;
+  return v > 0 ? v : 0x7fffffff;
+}
+__device__ inline int spk_min(const BeamParams& p, int u) { return p.spk_bound ? p.spk_bound[2 * u + 1] : 0; }
+// First rank r < n with K[r] >= kmin, else 0.
+__device__ inline int spk_pick(const int* K, int n, int kmin) {
+#pragma unroll 1
+  for (int r = 0; r < n; ++r)
+    if (K[r] >= kmin) return r;
+  return 0;
+}
 
 template <int V> struct Pow2Floor { static constexpr int value = (V >= 2) ? 2 * Pow2Floor<V / 2>::value : 1; };
 template <> struct Pow2Floor<1> { static constexpr int value = 1; };
@@ -171,7 +189,7 @@ __host__ __device__ inline unsigned align_up(unsigned v, unsigned a) { return (v
 // lane scalars (ints) ------------------------------------------------------------------------
 enum { LS_U = 0, LS_N, LS_TN, LS_T, LS_NB, LS_GEN, LS_ACTIVE, LS_FAILED, LS_TRACED, LS_NFINITE, LS_KMAX,
        LS_NWIN, LS_ERR, LS_M, LS_COLBASE, LS_NE, LS_ROW0_LO, LS_ROW0_HI, LS_DBGROWS_LO, LS_DBGROWS_HI,
-       LS_FRESH, LS_COUNT = 24 };
+       LS_FRESH, LS_PICK, LS_KHI, LS_KLO, LS_COUNT = 24 };  // LS_KHI / LS_KLO: speaker bounds
 // CTA scalars
 enum { MI_PUBLISHED = 0, MI_DONE, MI_MTOT, MI_QNEXT, MI_NLIST, MI_MAXK };
 
@@ -1081,6 +1099,7 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
       const int N = (int)(p.row_off[u + 1] - row0);
       if (N == 0) {
         p.status[u] = 0;
+        if (p.spk_out) p.spk_out[u] = 0;
         if (p.dbg_final_scores) {
           for (int b = 0; b < B; ++b) p.dbg_final_scores[(size_t)u * B + b] = INF;
           if (p.dbg_final_k) p.dbg_final_k[u] = 0;
@@ -1091,6 +1110,7 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
       ls[LS_ACTIVE] = 1; ls[LS_FAILED] = 0; ls[LS_TRACED] = (u == p.trace_utt); ls[LS_ERR] = 0;
       ls[LS_ROW0_LO] = (int)(row0 & 0xffffffffll); ls[LS_ROW0_HI] = (int)(row0 >> 32);
       ls[LS_DBGROWS_LO] = 0; ls[LS_DBGROWS_HI] = 0; ls[LS_FRESH] = 1;
+      ls[LS_KHI] = spk_max(p, u); ls[LS_KLO] = spk_min(p, u);
       for (unsigned w = 0; w < PW; ++w) reinterpret_cast<unsigned*>(lane_base(g) + L.l_scored)[w] = 0;
       int* meta = reinterpret_cast<int*>(lane_base(g) + L.l_meta);  // [gen][field][B]: K,last,tot,nl
       meta[0] = 0; meta[B] = -1; meta[2 * B] = 0; reinterpret_cast<float*>(meta)[3 * B] = 0.f;
@@ -1234,8 +1254,10 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
         const int* mK = reinterpret_cast<const int*>(lane_base(g) + L.l_meta) + ls[LS_GEN] * 4 * B;
         int* candoff = reinterpret_cast<int*>(lane_base(g) + L.l_candoff);
         int off = 0, kmax = 0;
-        const int nb = ls[LS_NB];
-        for (int b = 0; b < nb; ++b) { candoff[b] = off; off += mK[b] + 1; kmax = max(kmax, mK[b]); }
+        const int nb = ls[LS_NB], khi = ls[LS_KHI];
+        // a hypothesis at max_speakers clusters has no new-cluster candidate (its score would be +inf); the flat
+        // tie-break index below keeps the unbounded (kmax + 1) stride
+        for (int b = 0; b < nb; ++b) { candoff[b] = off; off += mK[b] + (mK[b] < khi ? 1 : 0); kmax = max(kmax, mK[b]); }
         candoff[nb] = off;
         ls[LS_NFINITE] = 0; ls[LS_KMAX] = kmax; ls[LS_NE] = off;
       }
@@ -1642,6 +1664,11 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
       const bool ok = !ls[LS_ERR] && nwin > 0;
       const int* fK = reinterpret_cast<const int*>(lane_base(g) + L.l_meta) + ngen * 4 * B;
       const float* fNl = reinterpret_cast<const float*>(fK + 3 * B);
+      if (tid == 0) {  // the returned hypothesis: the first final rank with min_speakers clusters (else rank 0)
+        const int r = ok ? spk_pick(fK, nwin, ls[LS_KLO]) : 0;
+        ls[LS_PICK] = r;
+        if (p.spk_out && !(STAT && sq != 0)) p.spk_out[u] = ok ? fK[r] : 0;
+      }
       if (p.dbg_final_scores) {
         if (tid < B) p.dbg_final_scores[(size_t)u * B + tid] = (ok && tid < nwin) ? fNl[tid] : INF;
         if (tid == 0 && p.dbg_final_k) p.dbg_final_k[u] = ok ? fK[0] : 0;
@@ -1673,7 +1700,7 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
           } else {
             p.status[u] = 0;
             const unsigned* bp = bp_cta + (size_t)g * p.maxN * B;
-            int r = 0;
+            int r = ls[LS_PICK];
             for (int i = N - 1; i >= 0; --i) {
               const unsigned e = bp[(size_t)i * B + r];
               p.labels[row0 + i] = (int)(e & 0xffffu);

@@ -433,10 +433,11 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
           for (int q0 = pa; q0 < pb; q0 += NT) {
             const int q = q0 + tid;
             const int Kp = (q < pb) ? ((level == 1) ? mK[q] : n_k[q]) : -1;
+            const int fan = Kp + (Kp < spk_max(p, u) ? 1 : 0);  // at max_speakers: no new-cluster child
             int chunk;
-            const int o = tot + block_excl_scan<NT>(Kp + 1, sc, &chunk, lane, warp);
+            const int o = tot + block_excl_scan<NT>(fan, sc, &chunk, lane, warp);
             if (chunk > cap - tot) { if (tid == 0) misc[TM_ERR] = 3; break; }
-            for (int c = 0; c <= Kp; ++c) {
+            for (int c = 0; c < fan; ++c) {
               if (last) l_pc[o + c] = ((unsigned)q << 8) | (unsigned)c;
               else { n_parent[base + o + c] = q; n_c[base + o + c] = c; }
             }
@@ -452,13 +453,14 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
           const int base = lvl[level];
           for (int q = pa; q < pb; ++q) {
             const int Kp = (level == 1) ? mK[q] : n_k[q];
+            const int fan = Kp + (Kp < spk_max(p, u) ? 1 : 0);  // at max_speakers: no new-cluster child
             const int cap = last ? NLF : NI - base;
-            if (tot + Kp + 1 > cap) { misc[TM_ERR] = 3; break; }
-            for (int c = 0; c <= Kp; ++c) {
+            if (tot + fan > cap) { misc[TM_ERR] = 3; break; }
+            for (int c = 0; c < fan; ++c) {
               if (last) l_pc[tot + c] = ((unsigned)q << 8) | (unsigned)c;
               else { n_parent[base + tot + c] = q; n_c[base + tot + c] = c; }
             }
-            tot += Kp + 1;
+            tot += fan;
           }
           misc[TM_COUNT] = tot;
           if (!last) lvl[level + 1] = base + tot;
@@ -632,8 +634,14 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
         for (int i = 0; i < N; ++i) p.labels[row0 + i] = -1;
       } else {
         p.status[u] = 0;
-        int r = 0;
         const int nsteps = (TN + L - 1) / L;
+        const int pick = spk_pick(meta + gen * 4 * B, nb, spk_min(p, u));
+        if (pick != 0) {  // back-track from rank `pick`: its last-step back-pointers move to column 0
+          const int t0 = (nsteps - 1) * L, Lc = min(L, TN - t0);
+          for (int i = 0; i < Lc; ++i) bp_lab[(size_t)(t0 + i) * B] = bp_lab[(size_t)(t0 + i) * B + pick];
+          bp_par[(size_t)(nsteps - 1) * B] = bp_par[(size_t)(nsteps - 1) * B + pick];
+        }
+        int r = 0;
         for (int s = nsteps - 1; s >= 0 && (long long)s * L + L > TN - N; --s) {
           const int t0 = s * L, Lc = min(L, TN - t0);
           for (int i = Lc - 1; i >= 0; --i) {
@@ -645,6 +653,9 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
       }
     }
     const bool ok = !(failed || misc[TM_ERR]);
+    // clusters of the returned hypothesis, 0 for a failed utterance (stored apart from the back-track: there it
+    // costs the (1024, 512) kernels spill)
+    if (tid == 0 && p.spk_out) p.spk_out[u] = ok ? meta[gen * 4 * B + spk_pick(meta + gen * 4 * B, nb, spk_min(p, u))] : 0;
     if (p.dbg_final_scores) {
       const float* fNl = reinterpret_cast<const float*>(meta + gen * 4 * B + 3 * B);
       if (tid < B) p.dbg_final_scores[(size_t)u * B + tid] = (ok && tid < nb) ? fNl[tid] : INF;

@@ -9,10 +9,12 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from .uisrnn import shard_by_frames
+from . import native
+from .uisrnn import _warn_min_speakers, shard_by_frames
 
 
-def predict_sharded(model, test_sequences, args, group=None, lengths=None, root=None, as_arrays=False):
+def predict_sharded(model, test_sequences, args, group=None, lengths=None, root=None, as_arrays=False, *,
+                    max_speakers=None, min_speakers=None):
   """Every rank passes the same list; rank r decodes the r-th shard (longest-first partition by
   frame count) with `model.predict`, and every rank returns the complete, ordered result.
 
@@ -26,20 +28,28 @@ def predict_sharded(model, test_sequences, args, group=None, lengths=None, root=
   result (what the reference's `parallel_predict` caller gets, uisrnn.py:619-623); the other ranks return
   their own shard in place and None elsewhere.  `as_arrays=True`: entries are numpy int32 arrays instead of
   lists of Python ints (building Python ints costs ~10 ns per label in one thread, which at several million
-  frames per second per GPU is the slowest stage of an 8-GPU job)."""
+  frames per second per GPU is the slowest stage of an 8-GPU job).
+
+  `max_speakers` / `min_speakers`: speaker bounds as in `UISRNN.predict` (an int, or one value per utterance, which
+  travels with its shard); each rank warns about the utterances of its own shard that fell short of min_speakers."""
   if not isinstance(test_sequences, list):
     raise TypeError('test_sequences must be a list.')
   if lengths is not None and len(lengths) != len(test_sequences):
     raise ValueError('lengths must have one entry per test sequence.')
+  bounded = max_speakers is not None or min_speakers is not None
+  bounds = native.speaker_bounds(len(test_sequences), max_speakers, min_speakers) if bounded else (None, None)
   if not (dist.is_available() and dist.is_initialized()):
-    if as_arrays:
-      return _predict_arrays(model, [_materialise(s) for s in test_sequences], args)
+    if as_arrays or bounded:
+      labels = _predict_arrays(model, [_materialise(s) for s in test_sequences], args, range(len(test_sequences)),
+                               bounds)
+      return labels if as_arrays else [lab.tolist() for lab in labels]
     return model.predict([_materialise(s) for s in test_sequences], args)
   world = dist.get_world_size(group)
   rank = dist.get_rank(group)
   lengths = [len(s) for s in test_sequences] if lengths is None else [int(n) for n in lengths]
   shards = shard_by_frames(lengths, world)
-  mine = _predict_arrays(model, [_materialise(test_sequences[i]) for i in shards[rank]], args) if shards[rank] else []
+  mine = _predict_arrays(model, [_materialise(test_sequences[i]) for i in shards[rank]], args, shards[rank],
+                         bounds) if shards[rank] else []
   counts = [sum(lengths[i] for i in shard) for shard in shards]
   use_cuda = getattr(model, 'device', None) is not None and model.device.type == 'cuda' and \
       dist.get_backend(group) == 'nccl'
@@ -72,8 +82,18 @@ def predict_sharded(model, test_sequences, args, group=None, lengths=None, root=
   return merged
 
 
-def _predict_arrays(model, sequences, args):
-  """model.predict, but int32 arrays straight from the device when the model has the native path."""
+def _predict_arrays(model, sequences, args, indices, bounds):
+  """model.predict, but int32 arrays straight from the device when the model has the native path.  `indices`: the
+  positions of `sequences` in the caller's list; `bounds`: speaker bounds over that whole list (None = absent)."""
+  if bounds[0] is not None or bounds[1] is not None:
+    from .uisrnn import _check_test_sequence
+    for sequence in sequences:
+      _check_test_sequence(sequence, model.observation_dim)
+    indices = list(indices)
+    mine = tuple(b[indices] if b is not None else None for b in bounds)
+    labels, speakers = model._predict_bounded(sequences, args, mine, as_arrays=True)  # pylint: disable=protected-access
+    _warn_min_speakers(indices, [len(s) for s in sequences], speakers, mine[1])
+    return labels
   if getattr(model, 'device', None) is not None and model.device.type == 'cuda' and hasattr(model, '_predict_cuda'):
     from .uisrnn import _check_test_sequence
     for sequence in sequences:

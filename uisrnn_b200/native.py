@@ -20,7 +20,7 @@ UIS_ERR_CUDA = -3
 UIS_ERR_OVERFLOW = -4
 UIS_ERR_NOMEM = -5
 UIS_ERR_CAPACITY = -6
-UIS_ABI_VERSION = 4  # include/uisrnn_b200.h
+UIS_ABI_VERSION = 5  # include/uisrnn_b200.h
 
 
 class NativeError(RuntimeError):
@@ -62,7 +62,8 @@ class Stats(C.Structure):
 
 # Every symbol include/uisrnn_b200.h declares (tests check the .so exports all of them).
 EXPORTS = ('uis_version', 'uis_last_error', 'uis_model_create', 'uis_model_destroy',
-           'uis_model_constants', 'uis_predict', 'uis_predict_device',
+           'uis_model_constants', 'uis_predict', 'uis_predict_device', 'uis_predict_bounded',
+           'uis_predict_device_bounded',
            'uis_predict_workspace_bytes', 'uis_get_stats', 'uis_trainer_create',
            'uis_trainer_destroy', 'uis_trainer_step', 'uis_trainer_get', 'uis_trainer_losses',
            'uis_trainer_comm_size', 'uis_trainer_comm_export', 'uis_trainer_comm_apply',
@@ -146,6 +147,10 @@ def load_library():
   lib.uis_predict_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int,
                                      C.POINTER(PredictOpts), C.c_void_p, C.POINTER(DebugTaps),
                                      C.c_void_p]
+  lib.uis_predict_bounded.restype = C.c_int
+  lib.uis_predict_bounded.argtypes = lib.uis_predict.argtypes + [ip, ip, ip]
+  lib.uis_predict_device_bounded.restype = C.c_int
+  lib.uis_predict_device_bounded.argtypes = lib.uis_predict_device.argtypes + [ip, ip, C.c_void_p]
   lib.uis_predict_workspace_bytes.restype = C.c_size_t
   lib.uis_predict_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.c_int,
                                               C.POINTER(PredictOpts)]
@@ -173,7 +178,6 @@ def load_library():
   lib.uis_trainer_comm_export.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
   lib.uis_trainer_comm_apply.restype = C.c_int
   lib.uis_trainer_comm_apply.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-  del ip
   _lib = lib
   return lib
 
@@ -185,6 +189,31 @@ def _check(lib, rc):
 
 def _f32(a):
   return np.ascontiguousarray(a, dtype=np.float32)
+
+
+def speaker_bounds(n, max_speakers=None, min_speakers=None):
+  """(max, min) as int32 arrays of length n, or None for an absent bound.  An int applies to every utterance, a
+  sequence gives one value per utterance; 0 means no bound.  Raises ValueError for a value that is not an integer (floats
+  and bools included, scalar or not), a negative value, a wrong length, or min > max where both are set."""
+  out = []
+  for name, v in (('max_speakers', max_speakers), ('min_speakers', min_speakers)):
+    if v is None:
+      out.append(None)
+      continue
+    a = np.asarray(v)
+    if a.ndim == 0:
+      a = np.full(n, v, a.dtype)
+    elif a.ndim != 1 or len(a) != n:
+      raise ValueError('{} needs one value per utterance ({}), got shape {}'.format(name, n, a.shape))
+    if (a.size or np.ndim(v) == 0) and not np.issubdtype(a.dtype, np.integer):  # (an empty list has a float dtype)
+      raise ValueError('{} must be integers, got {}'.format(name, a.dtype))
+    if (a < 0).any():
+      raise ValueError('{} must be >= 0 (0 = no bound)'.format(name))
+    out.append(np.ascontiguousarray(a, dtype=np.int32))
+  mx, mn = out
+  if mx is not None and mn is not None and ((mx > 0) & (mn > mx)).any():
+    raise ValueError('min_speakers must not exceed max_speakers')
+  return mx, mn
 
 
 class NativeModel:
@@ -267,10 +296,16 @@ class NativeModel:
     return t, bufs
 
   def predict(self, seqs, beam_size=10, look_ahead=1, test_iteration=2, kcap=0, n_ctas=0,
-              trace_utt=None, stream=0, lanes=0, cluster=0, engine=0):
+              trace_utt=None, stream=0, lanes=0, cluster=0, engine=0, max_speakers=None, min_speakers=None,
+              return_speakers=False):
     """seqs: list of C-contiguous float64 [N_u, D] arrays (host).  Returns a list of int32
-    label arrays (and a dict of debug arrays when trace_utt is not None)."""
+    label arrays (and a dict of debug arrays when trace_utt is not None).
+
+    max_speakers / min_speakers: an int for every utterance or one value per utterance, 0 = no bound
+    (uis_predict_bounded in include/uisrnn_b200.h).  return_speakers=True appends an int32 array with the
+    cluster count of every returned hypothesis to the result."""
     n = len(seqs)
+    mx, mn = speaker_bounds(n, max_speakers, min_speakers)
     keep = [s if (type(s) is np.ndarray and s.dtype == np.float64 and s.flags.c_contiguous)
             else np.ascontiguousarray(s, dtype=np.float64) for s in seqs]
     for s in keep:
@@ -293,9 +328,14 @@ class NativeModel:
       taps, bufs = self._taps(trace_utt, n, [s.shape[0] for s in keep], beam_size, look_ahead,
                               test_iteration, kcap)
       tp = C.byref(taps)
-    rc = self._lib.uis_predict(self._h, in_ptrs, lengths, n, C.byref(opts), out_ptrs, tp,
-                               C.c_void_p(stream))
+    ip = C.POINTER(C.c_int32)
+    spk = np.zeros(max(n, 1), np.int32) if return_speakers else None
+    arg = lambda a: a.ctypes.data_as(ip) if a is not None else None
+    rc = self._lib.uis_predict_bounded(self._h, in_ptrs, lengths, n, C.byref(opts), out_ptrs, tp,
+                                       C.c_void_p(stream), arg(mx), arg(mn), arg(spk))
     _check(self._lib, rc)
+    if return_speakers:
+      outs = (outs, spk[:n])
     if bufs is not None:
       nrows = int(bufs['off'][-1]) if len(bufs['off']) else 0
       bufs['win'] = bufs['win'][:nrows]
@@ -308,15 +348,22 @@ class NativeModel:
     return outs
 
   def predict_device(self, x_ptr, frame_offsets, labels_ptr, beam_size=10, look_ahead=1,
-                     test_iteration=2, kcap=0, n_ctas=0, stream=0, lanes=0, cluster=0, engine=0):
+                     test_iteration=2, kcap=0, n_ctas=0, stream=0, lanes=0, cluster=0, engine=0,
+                     max_speakers=None, min_speakers=None, speakers_ptr=0):
     """Device-resident variant: x_ptr -> fp32 [rows, D], labels_ptr -> int32 [rows] (raw
-    device addresses, e.g. torch.Tensor.data_ptr()).  Asynchronous on `stream`."""
+    device addresses, e.g. torch.Tensor.data_ptr()).  Asynchronous on `stream`.  Speaker bounds as in
+    predict(); speakers_ptr (device int32 [U], 0 = none) receives the cluster counts."""
     off = np.ascontiguousarray(frame_offsets, dtype=np.int64)
+    mx, mn = speaker_bounds(len(off) - 1, max_speakers, min_speakers)
+    ip = C.POINTER(C.c_int32)
     opts = self._opts(beam_size, look_ahead, test_iteration, kcap, n_ctas, lanes, cluster, engine)
-    rc = self._lib.uis_predict_device(self._h, C.c_void_p(x_ptr),
-                                      off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1,
-                                      C.byref(opts), C.c_void_p(labels_ptr), None,
-                                      C.c_void_p(stream))
+    rc = self._lib.uis_predict_device_bounded(self._h, C.c_void_p(x_ptr),
+                                              off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1,
+                                              C.byref(opts), C.c_void_p(labels_ptr), None,
+                                              C.c_void_p(stream),
+                                              mx.ctypes.data_as(ip) if mx is not None else None,
+                                              mn.ctypes.data_as(ip) if mn is not None else None,
+                                              C.c_void_p(speakers_ptr))
     _check(self._lib, rc)
 
   def stats(self):

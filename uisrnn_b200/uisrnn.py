@@ -11,6 +11,7 @@ device (explicit `--enable_cuda=False`, the reference's own device rule) the dec
 """
 import functools
 import threading
+import warnings
 
 import numpy as np
 import torch
@@ -412,35 +413,63 @@ class UISRNN:
         self._native = (key, native.NativeModel(self.export_weights(), device=index))
       return self._native[1]
 
-  def _predict_cuda(self, sequences, args, device_index=None, as_arrays=False):
-    from . import native
-    model = self._native_model(device_index)
-    kcap = _DEFAULT_KCAP
-    while True:
-      try:
-        with model.lock:  # a uis_model handle (one workspace) is not re-entrant
-          labels = model.predict(sequences, beam_size=args.beam_size, look_ahead=args.look_ahead,
-                                 test_iteration=args.test_iteration, kcap=kcap)
-        return labels if as_arrays else [lab.tolist() for lab in labels]
-      except native.NativeError as err:
-        if err.code != native.UIS_ERR_OVERFLOW or kcap >= 1024:
-          raise
-        kcap = 32 if kcap == 0 else kcap * 2  # a hypothesis opened more clusters than the device tables hold: grow and retry
+  def _predict_cuda(self, sequences, args, device_index=None, as_arrays=False, bounds=(None, None)):
+    """Labels of `sequences` from the native library; with speaker bounds (int32 arrays from
+    native.speaker_bounds, None = absent) returns (labels, cluster counts)."""
+    return _native_predict(self._native_model(device_index), sequences, args, as_arrays, bounds)
 
-  def predict_single(self, test_sequence, args):
-    """Labels (list of N ints) for one test sequence [N, D] float64 (uisrnn.py:479-562)."""
-    _check_test_sequence(test_sequence, self.observation_dim)
-    if self.device.type == 'cuda':
-      return self._predict_cuda([test_sequence], args)[0]
+  def _decode_cpu(self, sequence, args, max_speakers=0, min_speakers=0):
+    """(labels, cluster count) of one sequence on the CPU device."""
     decoder = beam_cpu.CpuBeamSearch(self)
-    return decoder.decode(test_sequence, args.beam_size, args.look_ahead, args.test_iteration)
+    return decoder.decode(sequence, args.beam_size, args.look_ahead, args.test_iteration, int(max_speakers),
+                          int(min_speakers), return_speakers=True)
 
-  def predict(self, test_sequences, args):
+  def _predict_bounded(self, sequences, args, bounds, as_arrays=False):
+    """(labels, cluster counts) of a checked list of sequences under per-utterance speaker bounds."""
+    if self.device.type == 'cuda':
+      return self._predict_cuda(sequences, args, as_arrays=as_arrays, bounds=bounds)
+    mx, mn = bounds
+    out = [self._decode_cpu(s, args, mx[i] if mx is not None else 0, mn[i] if mn is not None else 0)
+           for i, s in enumerate(sequences)]
+    labels = [np.asarray(o[0], np.int32) if as_arrays else o[0] for o in out]
+    return labels, np.array([o[1] for o in out], np.int32)
+
+  def predict_single(self, test_sequence, args, *, max_speakers=None, min_speakers=None):
+    """Labels (list of N ints) for one test sequence [N, D] float64 (uisrnn.py:479-562).
+
+    max_speakers / min_speakers (ints, 0 or None = no bound) bound the number of speakers: see `predict`."""
+    _check_test_sequence(test_sequence, self.observation_dim)
+    if max_speakers is None and min_speakers is None:
+      if self.device.type == 'cuda':
+        return self._predict_cuda([test_sequence], args)[0]
+      return self._decode_cpu(test_sequence, args)[0]
+    if np.ndim(max_speakers) or np.ndim(min_speakers):
+      raise ValueError('predict_single takes one int per bound')
+    bounds = _speaker_bounds(1, max_speakers, min_speakers)
+    labels, speakers = self._predict_bounded([test_sequence], args, bounds)
+    _warn_min_speakers([0], [len(test_sequence)], speakers, bounds[1])
+    return labels[0]
+
+  def predict(self, test_sequences, args, *, max_speakers=None, min_speakers=None):
     """Labels for one sequence (ndarray -> list of ints) or many (list -> list of lists)
-    (uisrnn.py:564-590).  On CUDA a list is decoded by a single native call."""
+    (uisrnn.py:564-590).  On CUDA a list is decoded by a single native call.
+
+    Speaker bounds (not in the reference): `max_speakers` / `min_speakers` is an int for every utterance or one
+    value per utterance, 0 or None = no bound.  A hypothesis never holds more than max_speakers clusters, so every
+    label is < max_speakers.  The labels come from the best-ranked final hypothesis with at least min_speakers
+    clusters; when the final beam holds none, rank 0's labels are returned and one warning names those utterances.
+    Clusters are counted over the whole decode (test_iteration tiled copies), so with test_iteration > 1 the
+    returned labels may use fewer distinct ids than min_speakers."""
     if isinstance(test_sequences, np.ndarray):
-      return self.predict_single(test_sequences, args)
+      return self.predict_single(test_sequences, args, max_speakers=max_speakers, min_speakers=min_speakers)
     if isinstance(test_sequences, list):
+      if max_speakers is not None or min_speakers is not None:
+        for sequence in test_sequences:
+          _check_test_sequence(sequence, self.observation_dim)
+        bounds = _speaker_bounds(len(test_sequences), max_speakers, min_speakers)
+        labels, speakers = self._predict_bounded(test_sequences, args, bounds)
+        _warn_min_speakers(range(len(test_sequences)), [len(s) for s in test_sequences], speakers, bounds[1])
+        return labels
       if self.device.type == 'cuda':
         for sequence in test_sequences:
           _check_test_sequence(sequence, self.observation_dim)
@@ -449,47 +478,115 @@ class UISRNN:
     raise TypeError('test_sequences should be either a list or numpy array.')
 
 
-def _predict_shard(model, args, device_index, sequences, out, position):
-  out[position] = model._predict_cuda(sequences, args, device_index)  # pylint: disable=protected-access
+def _speaker_bounds(n, max_speakers, min_speakers):
+  from . import native  # validation only: the library is not loaded
+  return native.speaker_bounds(n, max_speakers, min_speakers)
 
 
-def parallel_predict(model, test_sequences, args, num_processes=4):
+def _warn_min_speakers(indices, lengths, speakers, min_speakers):
+  """One warning naming the utterances (by `indices`) whose final beam held no hypothesis with min_speakers
+  clusters."""
+  if min_speakers is None:
+    return
+  short = [int(i) for i, n, k, lo in zip(indices, lengths, speakers, min_speakers) if n > 0 and k < lo]
+  if short:
+    warnings.warn('min_speakers: the final beam of utterance(s) {} held no hypothesis with that many speakers; '
+                  'the best hypothesis was returned instead'.format(short), RuntimeWarning, stacklevel=3)
+
+
+def _native_predict(model, sequences, args, as_arrays, bounds):
+  """NativeModel.predict with the kcap retry: a hypothesis that opened more clusters than the device tables hold
+  fails with UIS_ERR_OVERFLOW, and the call is repeated with larger tables."""
+  from . import native
+  mx, mn = bounds
+  bounded = mx is not None or mn is not None
+  kcap = _DEFAULT_KCAP
+  while True:
+    try:
+      with model.lock:  # a uis_model handle (one workspace) is not re-entrant
+        out = model.predict(sequences, beam_size=args.beam_size, look_ahead=args.look_ahead,
+                            test_iteration=args.test_iteration, kcap=kcap, max_speakers=mx, min_speakers=mn,
+                            return_speakers=bounded)
+      labels, speakers = out if bounded else (out, None)
+      labels = labels if as_arrays else [lab.tolist() for lab in labels]
+      return (labels, speakers) if bounded else labels
+    except native.NativeError as err:
+      if err.code != native.UIS_ERR_OVERFLOW or kcap >= 1024:
+        raise
+      kcap = 32 if kcap == 0 else kcap * 2  # a hypothesis opened more clusters than the device tables hold: grow and retry
+
+
+def _predict_shard(model, args, device_index, sequences, out, position, bounds):
+  out[position] = model._predict_cuda(sequences, args, device_index, bounds=bounds)  # pylint: disable=protected-access
+
+
+def _take(bound, indices):
+  return bound[indices] if bound is not None else None
+
+
+def _decode_cpu_bounded(model, args, sequence, max_speakers, min_speakers):
+  """One pool task of the CPU parallel_predict with speaker bounds (module level: the pool pickles it)."""
+  return model._decode_cpu(sequence, args, max_speakers, min_speakers)  # pylint: disable=protected-access
+
+
+def parallel_predict(model, test_sequences, args, num_processes=4, *, max_speakers=None, min_speakers=None):
   """Parallel prediction over a list of sequences (uisrnn.py:593-623).
 
   CPU model: a forkserver process pool, as the reference.  CUDA model: `num_processes` is the
   number of GPUs to use (capped by the visible devices); the list is split by total frame count
   and each shard is decoded by one native call on its own device, from its own host thread
   (the C ABI releases the GIL).  Utterances are independent, so there is no collective.
+  Speaker bounds as in `UISRNN.predict`; per-utterance values travel with their shards.
   """
   if not isinstance(test_sequences, list):
     raise TypeError('test_sequences must be a list.')
+  bounded = max_speakers is not None or min_speakers is not None
+  bounds = _speaker_bounds(len(test_sequences), max_speakers, min_speakers) if bounded else (None, None)
   if model.device.type == 'cuda':
     for sequence in test_sequences:
       _check_test_sequence(sequence, model.observation_dim)
     n_dev = max(1, min(int(num_processes), torch.cuda.device_count()))
     if n_dev == 1 or len(test_sequences) < 2:
+      if bounded:
+        return model.predict(test_sequences, args, max_speakers=bounds[0], min_speakers=bounds[1])
       return model._predict_cuda(test_sequences, args)  # pylint: disable=protected-access
     shards = shard_by_frames([len(s) for s in test_sequences], n_dev)
     twins = [model] + [_clone_for_device(model, d) for d in range(1, n_dev)]
     results, threads = [None] * n_dev, []
     for d, shard in enumerate(shards):
       thread = threading.Thread(target=_predict_shard, args=(
-          twins[d], args, d, [test_sequences[i] for i in shard], results, d))
+          twins[d], args, d, [test_sequences[i] for i in shard], results, d,
+          (_take(bounds[0], shard), _take(bounds[1], shard))))
       thread.start()
       threads.append(thread)
     for thread in threads:
       thread.join()
     merged = [None] * len(test_sequences)
-    for shard, labels in zip(shards, results):
-      if labels is None:
+    speakers = np.zeros(len(test_sequences), np.int32)
+    for shard, result in zip(shards, results):
+      if result is None:
         raise RuntimeError('parallel_predict: a device shard failed')
-      for i, lab in zip(shard, labels):
+      labels = result[0] if bounded else result
+      for j, (i, lab) in enumerate(zip(shard, labels)):
         merged[i] = lab
+        if bounded:
+          speakers[i] = result[1][j]
+    if bounded:
+      _warn_min_speakers(range(len(test_sequences)), [len(s) for s in test_sequences], speakers, bounds[1])
     return merged
   ctx = multiprocessing.get_context('forkserver')
   model.rnn_model.share_memory()
   with ctx.Pool(num_processes) as pool:
-    return pool.map(functools.partial(model.predict_single, args=args), test_sequences)
+    if not bounded:
+      return pool.map(functools.partial(model.predict_single, args=args), test_sequences)
+    for sequence in test_sequences:
+      _check_test_sequence(sequence, model.observation_dim)
+    n = len(test_sequences)
+    out = pool.starmap(functools.partial(_decode_cpu_bounded, model, args), zip(
+        test_sequences, bounds[0] if bounds[0] is not None else [0] * n,
+        bounds[1] if bounds[1] is not None else [0] * n))
+  _warn_min_speakers(range(n), [len(s) for s in test_sequences], [o[1] for o in out], bounds[1])
+  return [o[0] for o in out]
 
 
 class _DeviceTwin:
@@ -500,23 +597,13 @@ class _DeviceTwin:
     self._models = {}
     self._lock = threading.Lock()
 
-  def _predict_cuda(self, sequences, args, device_index):
+  def _predict_cuda(self, sequences, args, device_index, bounds=(None, None)):
     from . import native
     with self._lock:
       if device_index not in self._models:
         self._models[device_index] = native.NativeModel(self._weights, device=device_index)
       model = self._models[device_index]
-    kcap = _DEFAULT_KCAP
-    while True:
-      try:
-        with model.lock:
-          labels = model.predict(sequences, beam_size=args.beam_size, look_ahead=args.look_ahead,
-                                 test_iteration=args.test_iteration, kcap=kcap)
-        return [lab.tolist() for lab in labels]
-      except native.NativeError as err:
-        if err.code != native.UIS_ERR_OVERFLOW or kcap >= 1024:
-          raise
-        kcap = 32 if kcap == 0 else kcap * 2
+    return _native_predict(model, sequences, args, False, bounds)
 
 
 def _clone_for_device(model, device_index):
