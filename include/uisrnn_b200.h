@@ -66,7 +66,9 @@ typedef struct uis_predict_opts {
 } uis_predict_opts;
 
 /* Optional per-call debug / parity taps.  Any pointer may be NULL.  All are HOST buffers
- * the library fills before uis_predict*() returns (it synchronises the stream if any tap is set). */
+ * the library fills before uis_predict*() returns (it synchronises the stream if any tap is set).
+ * Taps do not change the plan: a traced call runs the kernel the same call without taps runs (engine,
+ * lanes, cluster or stationary-weights mode) and returns the same labels. */
 typedef struct uis_debug_taps {
   int32_t trace_utt;       /* utterance index to trace step by step, -1 = none                 */
   int32_t trace_capacity;  /* rows available in step_winners / step_scores                     */

@@ -2,7 +2,8 @@
 utterance, every weight matrix split by k-tiles, partial sums exchanged through distributed shared memory.
 Stationary-weights mode (cluster=32): 32 CTAs per utterance keep their rows of the weights in shared memory and
 exchange results through the shared slot pool with group barriers.  The labels must be those of the reference
-(golden) and of the one-CTA-per-utterance path."""
+(golden) and of the one-CTA-per-utterance path.  Scores, hidden states and running means of both modes are pinned
+through the debug taps in test_gpu_latency_modes.py."""
 import numpy as np
 import pytest
 

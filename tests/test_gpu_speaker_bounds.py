@@ -21,7 +21,6 @@ pytestmark = pytest.mark.gpu
 LA1 = {'ffma1': dict(engine=1, lanes=1, cluster=-1), 'ffma2': dict(engine=1, lanes=2, cluster=-1)}
 LA1_TOY = {'tc': dict(engine=2), 'cluster2': dict(engine=1, cluster=2), 'cluster4': dict(engine=1, cluster=4),
            'stat': dict(cluster=32)}
-TRACED = ('ffma1', 'ffma2', 'tc', 'tree', 'spill')  # the cluster modes run without debug taps
 
 
 def variants(case):
@@ -61,11 +60,8 @@ def test_fixture_case_through_kernel_variant(native, monkeypatch, case, variant)
     monkeypatch.setenv('UISRNN_B200_TREE_SPILL', 'force')
   opts = dict(LA1, **LA1_TOY).get(variant, {})
   kw = dict(bound_kw(case), return_speakers=True, **opts)
-  if variant in TRACED:
-    (labels, speakers), dbg = model.predict([case['x']], trace_utt=0, **kw)
-    compare_trace(dbg['win'], dbg['score'], dbg['off'], case['win'], case['score'], case['off'])
-  else:
-    labels, speakers = model.predict([case['x']], **kw)
+  (labels, speakers), dbg = model.predict([case['x']], trace_utt=0, **kw)  # traced in every variant
+  compare_trace(dbg['win'], dbg['score'], dbg['off'], case['win'], case['score'], case['off'])
   st = model.stats()
   if variant == 'tc':
     assert st['engine'] == 2

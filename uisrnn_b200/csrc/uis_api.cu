@@ -436,7 +436,7 @@ void plan_tree_spill(uis_model* m, Plan* pl) {
   pl->spill_budget = budget;
 }
 
-int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o, Plan* pl, bool has_taps = false) {
+int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o, Plan* pl) {
   if (!m || !o || (U > 0 && !off)) return fail(UIS_ERR_INVALID, "null argument");
   if (U < 0) return fail(UIS_ERR_INVALID, "U < 0");
   if (o->beam_size < 1 || o->look_ahead < 1 || o->test_iteration < 1)
@@ -536,7 +536,7 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
   // Stationary-weights mode (uis_beam_stat.cuh): 32 CTAs per utterance keep the weights in shared memory.  The fastest
   // way to decode up to #SMs / 32 utterances at a time; opts->cluster = 32 forces it, 0 picks it automatically,
   // UISRNN_B200_STAT=0 disables the automatic choice.
-  if (!tree && U >= 1 && (o->cluster == 0 || o->cluster == uis::kStatGroup) && !has_taps && m->depth == 1 &&
+  if (!tree && U >= 1 && (o->cluster == 0 || o->cluster == uis::kStatGroup) && m->depth == 1 &&
       o->lanes <= 1 && o->engine != 2) {
     const char* env = std::getenv("UISRNN_B200_STAT");
     const bool want = o->cluster == uis::kStatGroup ||
@@ -557,7 +557,7 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
     if (o->cluster == uis::kStatGroup)
       return fail(UIS_ERR_UNSUPPORTED, "stationary-weights mode needs hidden=512 dim=256 depth=1, >= 32 CTAs and beam_size/kcap that fit in shared memory");
   }
-  if (!tree && !pl->tcn && U >= 1 && o->cluster >= 0 && !has_taps && m->depth == 1 && o->lanes <= 1) {
+  if (!tree && !pl->tcn && U >= 1 && o->cluster >= 0 && m->depth == 1 && o->lanes <= 1) {
     int cs = 0;
     if (o->cluster == 2 || o->cluster == 4 || o->cluster == 8) {
       cs = o->cluster;
@@ -1097,7 +1097,7 @@ int uis_predict_device_bounded(uis_model* m, const float* x_dev, const int64_t* 
                                const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
                                const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev) {
   Plan pl;
-  if (int rc = make_plan(m, frame_offsets, U, opts, &pl, taps != nullptr)) return rc;
+  if (int rc = make_plan(m, frame_offsets, U, opts, &pl)) return rc;
   if (int rc = check_bounds(U, max_speakers, min_speakers)) return rc;
   if (U > 0 && pl.rows > 0 && (!x_dev || !labels_dev)) return fail(UIS_ERR_INVALID, "null device buffer");
   uis::DeviceGuard device_guard_(m->device);
@@ -1336,7 +1336,7 @@ int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* 
     off[u + 1] = off[u] + n_frames[u];
   }
   Plan pl;
-  if (int rc = make_plan(m, off.data(), U, opts, &pl, taps != nullptr)) return rc;
+  if (int rc = make_plan(m, off.data(), U, opts, &pl)) return rc;
   uis::DeviceGuard device_guard_(m->device);
   CU(device_guard_.status);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1370,7 +1370,7 @@ int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* 
       std::vector<int64_t> goff(u1 - u0 + 1);
       for (int q = u0; q <= u1; ++q) goff[q - u0] = off[q] - off[u0];
       Plan gp;
-      if (int rc = make_plan(m, goff.data(), u1 - u0, opts, &gp, false)) return rc;
+      if (int rc = make_plan(m, goff.data(), u1 - u0, opts, &gp)) return rc;
       if (int rc = predict_host_group(m, seqs + u0, n_frames + u0, u1 - u0, goff.data(), gp, labels_out + u0, nullptr, st,
                                       SpeakerBounds{max_speakers, min_speakers}.at(u0),
                                       speakers_out ? speakers_out + u0 : nullptr))

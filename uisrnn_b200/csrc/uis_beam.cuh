@@ -1056,6 +1056,8 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
   XchCtx xc{reinterpret_cast<float*>(smem + L.xch), reinterpret_cast<uint64_t*>(smem + L.xbar),
             XCL ? cluster_ctarank() : 0u, XCL ? cluster_nctarank() : 1u, 0u};
   const int xsize = (int)xc.size;
+  // Debug taps: the CTAs of a cluster / group decode the same utterance in lock step, and one of them writes the taps
+  const bool tap_leader = (!XCL || xc.rank == 0) && (!STAT || sq == 0);
 
   unsigned it = 0;  // weight-ring tile counter (identical in every consumer thread)
   // Statistics are thread 0's alone and live in shared memory: as locals they would hold ~30 registers in
@@ -1100,21 +1102,21 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
       if (N == 0) {
         p.status[u] = 0;
         if (p.spk_out) p.spk_out[u] = 0;
-        if (p.dbg_final_scores) {
+        if (p.dbg_final_scores && tap_leader) {
           for (int b = 0; b < B; ++b) p.dbg_final_scores[(size_t)u * B + b] = INF;
           if (p.dbg_final_k) p.dbg_final_k[u] = 0;
         }
         continue;
       }
       ls[LS_U] = u; ls[LS_N] = N; ls[LS_TN] = p.T * N; ls[LS_T] = 0; ls[LS_NB] = 1; ls[LS_GEN] = 0;
-      ls[LS_ACTIVE] = 1; ls[LS_FAILED] = 0; ls[LS_TRACED] = (u == p.trace_utt); ls[LS_ERR] = 0;
+      ls[LS_ACTIVE] = 1; ls[LS_FAILED] = 0; ls[LS_TRACED] = (u == p.trace_utt) && tap_leader; ls[LS_ERR] = 0;
       ls[LS_ROW0_LO] = (int)(row0 & 0xffffffffll); ls[LS_ROW0_HI] = (int)(row0 >> 32);
       ls[LS_DBGROWS_LO] = 0; ls[LS_DBGROWS_HI] = 0; ls[LS_FRESH] = 1;
       ls[LS_KHI] = spk_max(p, u); ls[LS_KLO] = spk_min(p, u);
       for (unsigned w = 0; w < PW; ++w) reinterpret_cast<unsigned*>(lane_base(g) + L.l_scored)[w] = 0;
       int* meta = reinterpret_cast<int*>(lane_base(g) + L.l_meta);  // [gen][field][B]: K,last,tot,nl
       meta[0] = 0; meta[B] = -1; meta[2 * B] = 0; reinterpret_cast<float*>(meta)[3 * B] = 0.f;
-      if (u == p.trace_utt && p.dbg_off) p.dbg_off[0] = 0;
+      if (u == p.trace_utt && tap_leader && p.dbg_off) p.dbg_off[0] = 0;
       return;
     }
   };
@@ -1669,20 +1671,29 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
         ls[LS_PICK] = r;
         if (p.spk_out && !(STAT && sq != 0)) p.spk_out[u] = ok ? fK[r] : 0;
       }
-      if (p.dbg_final_scores) {
+      if (p.dbg_final_scores && tap_leader) {
         if (tid < B) p.dbg_final_scores[(size_t)u * B + tid] = (ok && tid < nwin) ? fNl[tid] : INF;
         if (tid == 0 && p.dbg_final_k) p.dbg_final_k[u] = ok ? fK[0] : 0;
       }
       if (ls[LS_TRACED] && ok && p.dbg_best_mean) {
+        // (stationary-weights mode: the slots are in the group's pool, published by the group barrier that ended the
+        //  last weight pass; other CTAs wrote most of them, so the reads bypass L1)
         const TabEntry* ftab = reinterpret_cast<const TabEntry*>(lane_base(g) + L.l_tabs) + (size_t)ngen * B * Kcap;
         for (int c = 0; c < fK[0]; ++c) {  // best hypothesis = rank 0
           const TabEntry en = ftab[c];
-          if (tid < D) p.dbg_best_mean[(size_t)c * D + tid] = pool_mean_cta[g * pool_m_stride + (size_t)en.slot * D + tid];
-          for (int q = tid; q < DH; q += NT)
-            p.dbg_best_hidden[(size_t)c * DH + q] = pool_hidden_cta[g * pool_h_stride + (size_t)en.slot * DH + q];
+          const float* mp = pool_mean_cta + g * pool_m_stride + (size_t)en.slot * D;
+          const float* hp = pool_hidden_cta + g * pool_h_stride + (size_t)en.slot * DH;
+          if (tid < D) p.dbg_best_mean[(size_t)c * D + tid] = STAT ? __ldcg(mp + tid) : mp[tid];
+          for (int q = tid; q < DH; q += NT) p.dbg_best_hidden[(size_t)c * DH + q] = STAT ? __ldcg(hp + q) : hp[q];
           if (tid == 0) p.dbg_best_blocks[c] = en.blocks;
         }
       }
+    }
+    if constexpr (STAT) {
+      // The traced utterance's state is read from the group's pool above; the other CTAs may only write the slots of
+      // their next utterance (its first weight pass, before any group barrier) once the leader has read it.
+      if (fin[0] && LSp(0)[LS_U] == p.trace_utt && p.dbg_best_mean)
+        stat_group_sync<NT>(p.stat_bar + (size_t)sgroup * kStatGroup, stat_epoch, tid);
     }
     named_bar_sync(1, NT);
     if (tid < G) {
