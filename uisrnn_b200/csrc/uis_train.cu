@@ -759,9 +759,11 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
     const float coef = fminf(max_norm / (sqrtf(tot) + 1e-6f), 1.0f);
     gi *= coef;
   }
-  const float b1 = 0.9f, b2 = 0.999f, eps = 1e-8f;
-  const float mi = b1 * m[i] + (1.f - b1) * gi;
-  const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
+  // 1 - beta is rounded from its exact value, as torch does with the Python doubles (1.f - 0.999f would be
+  // 1.3e-5 relative off 0.001, and every update 6e-6 relative off torch's)
+  const float b1 = 0.9f, b2 = 0.999f, one_m_b1 = 0.1f, one_m_b2 = 0.001f, eps = 1e-8f;
+  const float mi = b1 * m[i] + one_m_b1 * gi;
+  const float vi = b2 * v[i] + one_m_b2 * gi * gi;
   m[i] = mi; v[i] = vi;
   const float denom = sqrtf(vi) / bc2_sqrt + eps;
   float pi = p[i] - step_size * (mi / denom);
