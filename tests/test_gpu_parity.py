@@ -5,6 +5,7 @@ running means within 1e-5 absolute (BASELINE.md section 3.4)."""
 import numpy as np
 import pytest
 
+import beam_replay
 from helpers import (GOLDEN, compare_trace, depth2_cases, load_weights, oracle_model, rel_err, small_cases,
                      toy_utterances, uis_oracle)
 
@@ -291,7 +292,8 @@ def test_depth3_untrained_matches_oracle(native):
 @pytest.mark.parametrize('H,D,depth', [(100, 40, 1), (8, 2, 2), (300, 200, 1), (129, 65, 1), (512, 100, 1), (24, 16, 3)])
 def test_any_shape_up_to_512x256_runs_zero_padded(native, H, D, depth):
   """A model whose (hidden, dim) is not a kernel shape runs zero-padded in the next larger one (uis_model_create):
-  labels, per-step scores and the un-padded states of the best hypothesis against the oracle at the ORIGINAL shape.
+  labels against the oracle at the ORIGINAL shape, and the traced utterance's per-step scores and selection and the
+  un-padded states of its best hypothesis against the float64 replay (tests/beam_replay.py) at that shape.
   (8, 2, depth 2) is the model of the reference's own integration test; observation_dim 16 / 100 are its other shapes."""
   rng = np.random.default_rng(1000 * H + D)
   u = lambda *s: (rng.uniform(-1, 1, size=s) / np.sqrt(H)).astype(np.float32)
@@ -314,6 +316,12 @@ def test_any_shape_up_to_512x256_runs_zero_padded(native, H, D, depth):
   for x, o in zip(xs, got):
     assert o.tolist() == uis_oracle.predict_single(om, x, beam_size=5, look_ahead=1, test_iteration=2)
   assert dbg['best_mean'].shape[1] == D and dbg['best_hidden'].shape[1:] == (depth, H)
+  # the taps: every step's increments and selection and the final state against the float64 replay at this shape
+  final = dict(best_mean=dbg['best_mean'], best_hidden=dbg['best_hidden'], best_blocks=dbg['best_blocks'],
+               final_k=dbg['final_k'][0], final_scores=dbg['final_scores'][0])
+  replay = beam_replay.Replay(w, xs[0], 5, 1, 2, dbg['win'], dbg['score'], dbg['off'], mean0=mean0)
+  beam_replay.check(replay, beam_replay.INC_RTOL, labels=got[0].tolist(), final=final,
+                    state_tol=beam_replay.STATE_TOL)
   la2 = model.predict(xs[:1], beam_size=3, look_ahead=2, test_iteration=1, kcap=32)[0]
   assert la2.tolist() == uis_oracle.predict_single(om, xs[0], beam_size=3, look_ahead=2, test_iteration=1)
 
