@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define UIS_ABI_VERSION 5
+#define UIS_ABI_VERSION 6
 
 typedef enum uis_status {
   UIS_OK = 0,
@@ -191,6 +191,40 @@ int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* 
 int uis_predict_device_bounded(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
                                const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
                                const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev);
+
+/*
+ * ABI 6: the N best hypotheses of every utterance, with their scores.  Not in the reference, which returns rank 0's
+ * labels only.  Each call takes the bounded call's arguments (speaker bounds as above; the cluster counts come in
+ * `out`) plus
+ *   n_best       1 <= n_best <= beam_size, else UIS_ERR_INVALID.
+ *   out          where the hypotheses go (HOST buffers for uis_predict_nbest, DEVICE buffers for
+ *                uis_predict_device_nbest; the label member the other entry point uses is ignored).
+ * Hypothesis j < n_best of an utterance is the j-th final rank (in rank order) with at least min_speakers clusters;
+ * when no final rank has that many, it is rank 0 alone.  So hypothesis 0 is what uis_predict_bounded returns.  Its
+ * score is the neg_likelihood accumulated over the whole tiled decode (BeamState.neg_likelihood, the value
+ * uis_debug_taps.final_scores shows).  Entries past count[u] hold labels -1, score +inf and 0 clusters; an empty or
+ * failed utterance returns no hypothesis.  With test_iteration > 1 two hypotheses may differ only in an earlier
+ * copy and so carry the same labels (the last copy's); they are not merged.
+ * uis_predict_bounded / uis_predict_device_bounded are n_best = 1 calls of the same search.
+ * Workspace: beyond uis_predict_workspace_bytes(), uis_predict_nbest holds 4 * (n_best - 1) * rows more label bytes
+ * and 4 * (2 * n_best + 1) * U bytes for the outputs (its group planner counts both).
+ */
+typedef struct uis_nbest_out {
+  int32_t* const* labels_out;  /* host entry: labels_out[u] -> int32 [n_best][n_frames[u]]                        */
+  int32_t* labels_dev;         /* device entry: int32 [n_best][frame_offsets[U]], plane 0 = uis_predict_device's labels */
+  float* scores;               /* [U][n_best]  neg_likelihood, +inf where absent                                   */
+  int32_t* speakers;           /* [U][n_best]  clusters, 0 where absent (may be NULL)                              */
+  int32_t* count;              /* [U]          hypotheses returned (may be NULL)                                   */
+} uis_nbest_out;
+
+int uis_predict_nbest(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                      const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                      const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                      const uis_nbest_out* out);
+int uis_predict_device_nbest(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                             const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                             const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                             const uis_nbest_out* out);
 
 /* Device bytes uis_predict_device() will hold for this problem (workspace is cached in the handle). */
 size_t uis_predict_workspace_bytes(uis_model* m, const int64_t* frame_offsets, int U,

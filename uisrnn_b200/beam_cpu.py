@@ -14,6 +14,12 @@ import torch
 from . import loss_func
 
 
+def nbest_ranks(clusters, min_speakers, n_best):
+  """Final ranks an N-best decode returns, given the cluster count of every final rank: the first `n_best` ranks
+  with at least `min_speakers` clusters, or rank 0 alone when there is none."""
+  return [r for r, k in enumerate(clusters) if k >= min_speakers][:n_best] or [0]
+
+
 class _Hypothesis:
   """One beam entry: per-cluster running means / hidden states / visit and block counts."""
   __slots__ = ('means', 'hiddens', 'visits', 'blocks', 'trace', 'score')
@@ -41,6 +47,7 @@ class CpuBeamSearch:
     self.log_1mp0 = np.log(1 - model.transition_bias)
     self.alpha = model.crp_alpha
     self.log_alpha = np.log(model.crp_alpha)
+    self.rnn.eval()  # (mean0 / hidden0 below: no dropout between stacked layers, as in decode)
     with torch.no_grad():
       self.weight = (1 / (2 * model.sigma2)).detach()
       zeros = torch.zeros(1, 1, model.observation_dim, device=self.device)
@@ -116,9 +123,13 @@ class CpuBeamSearch:
 
   @torch.no_grad()
   def decode(self, sequence, beam_size, look_ahead, test_iteration, max_speakers=0, min_speakers=0,
-             return_speakers=False):
+             return_speakers=False, n_best=None):
     """`sequence`: float64 [N, D] ndarray.  Returns the N labels of the last tiled copy (and, with
     return_speakers, the cluster count of the returned hypothesis).
+
+    n_best=k: returns (labels, scores, clusters) of up to k final hypotheses instead (`nbest_ranks`): their
+    labels of the last tiled copy, their neg_likelihood over the whole decode and their cluster counts.  An empty
+    sequence returns no hypothesis.
 
     Speaker bounds (0 = none): an index tuple that would take its hypothesis past `max_speakers` clusters
     scores +inf; the returned hypothesis is the best-ranked final one with at least `min_speakers` clusters,
@@ -145,6 +156,12 @@ class CpuBeamSearch:
         index = np.unravel_index(order[rank], scores.shape)
         survivors.append(self._expand(beam[int(index[0])], frames, index[1:]))
       beam = survivors
+    if n_best is not None:
+      if length == 0:
+        return [], [], []
+      chosen = [beam[r] for r in nbest_ranks([len(h.means) for h in beam], min_speakers, n_best)]
+      return ([[int(c) for c in h.trace[-length:]] for h in chosen], [float(h.score) for h in chosen],
+              [len(h.means) for h in chosen])
     best = next((h for h in beam if len(h.means) >= min_speakers), beam[0])
     labels = [int(c) for c in best.trace[-length:]]
     return (labels, len(best.means)) if return_speakers else labels

@@ -16,6 +16,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 #include <numeric>
 #include <string>
 #include <vector>
@@ -160,6 +161,7 @@ struct uis_model {
   // workspace
   DevBuf x64, x32, gi, row_off, order, pool_mean, pool_hidden, pool_mse, bp, queue_stats, labels, status;
   DevBuf spk_bound, spk_out;  // bounded calls only: [U][2] speaker bounds; [U] speaker counts (host-buffer entry point)
+  DevBuf nb_scores, nb_speakers, nb_count;  // N-best calls, host-buffer entry point: [U][n_best], [U][n_best], [U]
   DevBuf tree_arena;  // look-ahead spill kernel: [spill CTAs][make_tree_arena(..).total]
   DevBuf dbg_win, dbg_score, dbg_off, dbg_final_scores, dbg_final_k, dbg_best_mean, dbg_best_hidden,
       dbg_best_blocks;
@@ -603,6 +605,18 @@ struct SpeakerBounds {
   }
 };
 
+// N-best outputs of a call (n_best = 1 with NULL pointers: a plain call).  Labels are n_best planes of the call's rows.
+struct NBestOut {
+  int k = 1;
+  float* scores = nullptr;     // [U][k]
+  int32_t* speakers = nullptr; // [U][k]
+  int32_t* count = nullptr;    // [U]
+  NBestOut at(int u0) const {
+    return NBestOut{k, scores ? scores + (size_t)u0 * k : nullptr, speakers ? speakers + (size_t)u0 * k : nullptr,
+                    count ? count + u0 : nullptr};
+  }
+};
+
 int check_bounds(int U, const int32_t* mx, const int32_t* mn) {
   for (int u = 0; u < U; ++u) {
     const int a = mx ? mx[u] : 0, b = mn ? mn[u] : 0;
@@ -613,10 +627,37 @@ int check_bounds(int U, const int32_t* mx, const int32_t* mn) {
   return 0;
 }
 
+// n_best in [1, beam_size]; an N-best call needs its label and score buffers.
+int check_nbest(int n_best, const uis_predict_opts* opts, const uis_nbest_out* out) {
+  if (n_best < 1 || n_best > opts->beam_size)
+    return fail(UIS_ERR_INVALID, "n_best=%d (need 1 <= n_best <= beam_size=%d)", n_best, opts->beam_size);
+  if (!out->scores) return fail(UIS_ERR_INVALID, "n_best: null scores buffer");
+  return 0;
+}
+
+int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                        const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
+                        const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev,
+                        const NBestOut& nb);
+int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                      const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
+                      const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out,
+                      const NBestOut& nb);
+
 int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, const Plan& pl, int32_t* labels_dev,
-               const uis_debug_taps* taps, cudaStream_t st, const SpeakerBounds& sb, bool gi_ready = false) {
+               const uis_debug_taps* taps, cudaStream_t st, const SpeakerBounds& sb, const NBestOut& nb,
+               bool gi_ready = false) {
   const int H = m->H, D = m->D;
   if (sb.out_dev && U > 0) CU(cudaMemsetAsync(sb.out_dev, 0, (size_t)U * sizeof(int32_t), st));  // empty inputs: 0
+  if (U > 0 && pl.rows == 0) {  // no kernel runs: every utterance is empty and returns no hypothesis
+    if (nb.count) CU(cudaMemsetAsync(nb.count, 0, (size_t)U * sizeof(int32_t), st));
+    if (nb.speakers) CU(cudaMemsetAsync(nb.speakers, 0, (size_t)U * nb.k * sizeof(int32_t), st));
+    if (nb.scores) {
+      const std::vector<float> inf((size_t)U * nb.k, std::numeric_limits<float>::infinity());
+      CU(cudaMemcpyAsync(nb.scores, inf.data(), inf.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+      CU(cudaStreamSynchronize(st));  // (inf is about to go out of scope)
+    }
+  }
   m->stats = uis_stats{};
   m->stats.utterances = U;
   m->stats.frames = pl.rows;
@@ -702,6 +743,8 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
     p.spk_bound = m->spk_bound.as<int>();
   }
   p.spk_out = sb.out_dev;
+  p.n_best = nb.k; p.label_plane = pl.rows;
+  p.nbest_scores = nb.scores; p.nbest_speakers = nb.speakers; p.nbest_count = nb.count;
   p.trace_utt = -1;
   if (pl.stat) {
     p.stat_bar = m->stat_bar.as<unsigned>();
@@ -1050,7 +1093,7 @@ int uis_model_destroy(uis_model* m) {
                     &m->pool_mean, &m->pool_hidden, &m->bp, &m->queue_stats, &m->labels, &m->status, &m->dbg_win,
                     &m->dbg_score, &m->dbg_off, &m->dbg_final_scores, &m->dbg_final_k, &m->dbg_best_mean,
                     &m->dbg_best_hidden, &m->dbg_best_blocks, &m->tc_planes, &m->tc_scratch, &m->pool_mse, &m->stat_bar, &m->stat_scratch,
-                    &m->tree_arena};
+                    &m->tree_arena, &m->nb_scores, &m->nb_speakers, &m->nb_count};
   for (DevBuf* b : bufs) b->release();
   for (auto& e : m->ev)
     if (e) cudaEventDestroy(e);
@@ -1096,6 +1139,28 @@ int uis_predict_device(uis_model* m, const float* x_dev, const int64_t* frame_of
 int uis_predict_device_bounded(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
                                const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
                                const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev) {
+  return predict_device_impl(m, x_dev, frame_offsets, U, opts, labels_dev, taps, stream, max_speakers, min_speakers,
+                             speakers_dev, NBestOut{});
+}
+
+int uis_predict_device_nbest(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                             const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                             const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                             const uis_nbest_out* out) {
+  if (!opts || !out) return fail(UIS_ERR_INVALID, "null argument");
+  if (int rc = check_nbest(n_best, opts, out)) return rc;
+  return predict_device_impl(m, x_dev, frame_offsets, U, opts, out->labels_dev, taps, stream, max_speakers, min_speakers,
+                             nullptr, NBestOut{n_best, out->scores, out->speakers, out->count});
+}
+
+}  // extern "C"
+
+namespace {
+
+int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                        const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
+                        const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev,
+                        const NBestOut& nb) {
   Plan pl;
   if (int rc = make_plan(m, frame_offsets, U, opts, &pl)) return rc;
   if (int rc = check_bounds(U, max_speakers, min_speakers)) return rc;
@@ -1112,12 +1177,8 @@ int uis_predict_device_bounded(uis_model* m, const float* x_dev, const int64_t* 
     x_dev = m->x32.as<float>();
   }
   return run_device(m, x_dev, frame_offsets, U, pl, labels_dev, taps, st,
-                    SpeakerBounds{max_speakers, min_speakers, speakers_dev});
+                    SpeakerBounds{max_speakers, min_speakers, speakers_dev}, nb);
 }
-
-}  // extern "C"
-
-namespace {
 
 int ensure_host_path(uis_model* m) {
   if (!m->copy_stream) CU(cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
@@ -1145,12 +1206,12 @@ size_t staging_chunk_rows(int d_user) {
 // projection on `st`, then the beam kernel, then one D2H copy of all labels.
 int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
                             const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
-                            const SpeakerBounds& sb, int32_t* speakers_out);
+                            const SpeakerBounds& sb, int32_t* speakers_out, const NBestOut& nb);
 
 int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
                        const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
-                       const SpeakerBounds& sb, int32_t* speakers_out) {
-  const int rc = predict_host_group_impl(m, seqs, n_frames, U, off, pl, labels_out, taps, st, sb, speakers_out);
+                       const SpeakerBounds& sb, int32_t* speakers_out, const NBestOut& nb) {
+  const int rc = predict_host_group_impl(m, seqs, n_frames, U, off, pl, labels_out, taps, st, sb, speakers_out, nb);
   if (rc != 0 && rc != UIS_ERR_OVERFLOW && rc != UIS_ERR_CAPACITY) {
     // a failed call may leave copies / kernels in flight on either stream: drain them (the error already recorded in
     // uis_last_error() is the one reported) so that the staging ring and the workspace are quiescent for the next call
@@ -1165,7 +1226,7 @@ int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n
 
 int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
                             const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
-                            const SpeakerBounds& sb_host, int32_t* speakers_out) {
+                            const SpeakerBounds& sb_host, int32_t* speakers_out, const NBestOut& nb_host) {
   const int D = m->D_user, H = m->H;  // the caller's rows; the device rows are padded to m->D floats
   const size_t rows = (size_t)pl.rows;
   if (rows == 0) {
@@ -1180,17 +1241,31 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
   if (int rc = m->x64.ensure((size_t)slots * chunk * D * 8)) return rc;
   if (int rc = m->x32.ensure(rows * m->D * 4)) return rc;
   if (int rc = m->gi.ensure(rows * 3 * H * sizeof(float))) return rc;
-  if (int rc = m->labels.ensure(rows * 4)) return rc;
+  const int K = nb_host.k;  // label planes
+  if (int rc = m->labels.ensure(rows * 4 * K)) return rc;
   SpeakerBounds sb = sb_host;  // speaker counts land in the handle's device buffer, then in `speakers_out`
   if (speakers_out) {
     if (int rc = m->spk_out.ensure((size_t)U * 4)) return rc;
     sb.out_dev = m->spk_out.as<int32_t>();
   }
-  if (rows * 4 > m->labels_pin_cap) {
+  NBestOut nb{K};  // likewise the N-best scores, cluster counts and hypothesis counts
+  if (nb_host.scores) {
+    if (int rc = m->nb_scores.ensure((size_t)U * K * 4)) return rc;
+    nb.scores = m->nb_scores.as<float>();
+  }
+  if (nb_host.speakers) {
+    if (int rc = m->nb_speakers.ensure((size_t)U * K * 4)) return rc;
+    nb.speakers = m->nb_speakers.as<int32_t>();
+  }
+  if (nb_host.count) {
+    if (int rc = m->nb_count.ensure((size_t)U * 4)) return rc;
+    nb.count = m->nb_count.as<int32_t>();
+  }
+  if (rows * 4 * K > m->labels_pin_cap) {
     if (m->labels_pin) cudaFreeHost(m->labels_pin);
     m->labels_pin = nullptr;
     m->labels_pin_cap = 0;
-    const size_t want = rows * 4 + rows / 2 + 4096;
+    const size_t want = rows * 4 * K + rows / 2 + 4096;
     if (cudaMallocHost(&m->labels_pin, want) != cudaSuccess) {
       (void)cudaGetLastError();
       return fail(UIS_ERR_NOMEM, "cudaMallocHost(%zu) for the label staging buffer failed", want);
@@ -1284,16 +1359,21 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
     r0 = r1;
   }
   CU(cudaEventRecord(m->ev_h2d[1], cs));
-  if (int rc = run_device(m, m->x32.as<float>(), off, U, pl, m->labels.as<int32_t>(), taps, st, sb, /*gi_ready=*/true))
+  if (int rc = run_device(m, m->x32.as<float>(), off, U, pl, m->labels.as<int32_t>(), taps, st, sb, nb, /*gi_ready=*/true))
     return rc;
   m->stats.kernel_launches = 1 + 2 * (int64_t)n_chunks + (pl.L > 1 && pl.spill == 1 ? 1 : 0);
   m->stats.chunks = n_chunks;
   m->stats.staged = staged ? 1 : 0;
-  CU(cudaMemcpyAsync(m->labels_pin, m->labels.p, rows * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(m->labels_pin, m->labels.p, rows * 4 * K, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  for (int q = 0; q < U; ++q)
-    if (n_frames[q] > 0) std::memcpy(labels_out[q], m->labels_pin + off[q], (size_t)n_frames[q] * 4);
+  for (int j = 0; j < K; ++j)  // plane j of the device rows -> rows j of the caller's [K][n_frames[q]] buffers
+    for (int q = 0; q < U; ++q)
+      if (n_frames[q] > 0)
+        std::memcpy(labels_out[q] + (size_t)j * n_frames[q], m->labels_pin + (size_t)j * rows + off[q], (size_t)n_frames[q] * 4);
   if (speakers_out) CU(cudaMemcpy(speakers_out, sb.out_dev, (size_t)U * 4, cudaMemcpyDeviceToHost));
+  if (nb.scores) CU(cudaMemcpy(nb_host.scores, nb.scores, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
+  if (nb.speakers) CU(cudaMemcpy(nb_host.speakers, nb.speakers, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
+  if (nb.count) CU(cudaMemcpy(nb_host.count, nb.count, (size_t)U * 4, cudaMemcpyDeviceToHost));
   if (int rc = collect(m)) return rc;
   CU(cudaEventElapsedTime(&m->stats.h2d_ms, m->ev_h2d[0], m->ev_h2d[1]));
   CU(cudaEventElapsedTime(&m->stats.pipeline_ms, m->ev_pipe, m->ev[1]));  // first cast -> beam kernel start
@@ -1324,10 +1404,37 @@ int uis_predict(uis_model* m, const double* const* seqs, const int64_t* n_frames
 int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
                         const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
                         const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out) {
+  return predict_host_impl(m, seqs, n_frames, U, opts, labels_out, taps, stream, max_speakers, min_speakers,
+                           speakers_out, NBestOut{});
+}
+
+int uis_predict_nbest(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                      const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                      const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                      const uis_nbest_out* out) {
+  if (!opts || !out) return fail(UIS_ERR_INVALID, "null argument");
+  if (int rc = check_nbest(n_best, opts, out)) return rc;
+  return predict_host_impl(m, seqs, n_frames, U, opts, out->labels_out, taps, stream, max_speakers, min_speakers,
+                           nullptr, NBestOut{n_best, out->scores, out->speakers, out->count});
+}
+
+}  // extern "C"
+
+namespace {
+
+int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                      const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
+                      const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out,
+                      const NBestOut& nb) {
   if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
   if (U < 0 || (U > 0 && (!seqs || !n_frames || !labels_out))) return fail(UIS_ERR_INVALID, "null argument");
   if (int rc = check_bounds(U, max_speakers, min_speakers)) return rc;
   if (speakers_out && U > 0) std::memset(speakers_out, 0, (size_t)U * sizeof(int32_t));  // empty inputs: 0
+  if (U > 0) {  // empty inputs return no N-best hypothesis
+    if (nb.scores) std::fill(nb.scores, nb.scores + (size_t)U * nb.k, std::numeric_limits<float>::infinity());
+    if (nb.speakers) std::memset(nb.speakers, 0, (size_t)U * nb.k * sizeof(int32_t));
+    if (nb.count) std::memset(nb.count, 0, (size_t)U * sizeof(int32_t));
+  }
   const auto t_begin = std::chrono::steady_clock::now();
   std::vector<int64_t> off(U + 1, 0);
   for (int u = 0; u < U; ++u) {
@@ -1344,7 +1451,7 @@ int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* 
   // Memory: the per-frame workspace (gi 12H B + fp32 rows 4D B + labels) is the part that grows with the input.
   // A list that does not fit the device at once is decoded in groups of whole utterances, one after the other
   // (utterances are independent, uisrnn.py:587-589); UISRNN_B200_MAX_ROWS forces a limit (tests).
-  const size_t per_row = (size_t)3 * m->H * 4 + (size_t)m->D * 4 + 4;
+  const size_t per_row = (size_t)3 * m->H * 4 + (size_t)m->D * 4 + (size_t)4 * nb.k;  // (+ one label per plane)
   size_t max_rows = 0;
   if (const char* env = std::getenv("UISRNN_B200_MAX_ROWS")) max_rows = (size_t)std::max(1ll, std::atoll(env));
   if (!max_rows) {
@@ -1352,13 +1459,13 @@ int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* 
     CU(cudaMemGetInfo(&free_b, &total_b));
     const size_t held = m->gi.cap + m->x32.cap + m->labels.cap + m->x64.cap;  // re-used by this call
     const size_t fixed = workspace_bytes(m, pl, U) - (size_t)pl.rows * 3 * m->H * 4 +
-                         (size_t)uis_model::kSlots * staging_chunk_rows(m->D_user) * m->D_user * 8;
+                         (size_t)uis_model::kSlots * staging_chunk_rows(m->D_user) * m->D_user * 8 + (size_t)U * (2 * nb.k + 1) * 4;
     const double budget = 0.9 * (double)(free_b + held) - (double)fixed;
     max_rows = budget > (double)per_row ? (size_t)(budget / (double)per_row) : 1;
   }
   if ((size_t)pl.rows <= max_rows || taps || U <= 1) {
     if (int rc = predict_host_group(m, seqs, n_frames, U, off.data(), pl, labels_out, taps, st,
-                                    SpeakerBounds{max_speakers, min_speakers}, speakers_out))
+                                    SpeakerBounds{max_speakers, min_speakers}, speakers_out, nb))
       return rc;
     m->stats.groups = 1;
   } else {
@@ -1373,7 +1480,7 @@ int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* 
       if (int rc = make_plan(m, goff.data(), u1 - u0, opts, &gp)) return rc;
       if (int rc = predict_host_group(m, seqs + u0, n_frames + u0, u1 - u0, goff.data(), gp, labels_out + u0, nullptr, st,
                                       SpeakerBounds{max_speakers, min_speakers}.at(u0),
-                                      speakers_out ? speakers_out + u0 : nullptr))
+                                      speakers_out ? speakers_out + u0 : nullptr, nb.at(u0)))
         return rc;
       m->stats.groups = 1;
       add_stats(&total, m->stats);
@@ -1384,6 +1491,10 @@ int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* 
   m->stats.host_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
   return 0;
 }
+
+}  // namespace
+
+extern "C" {
 
 int uis_get_stats(uis_model* m, uis_stats* out) {
   if (!m || !out) return fail(UIS_ERR_INVALID, "null argument");

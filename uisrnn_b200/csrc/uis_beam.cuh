@@ -133,6 +133,13 @@ struct BeamParams {
   // speaker bounds (uis_predict*_bounded), indexed by utterance id; null = unbounded
   const int* spk_bound;  // [U][2]: max_speakers (0 = none), min_speakers
   int* spk_out;          // [U]    clusters of the returned hypothesis, 0 for a failed utterance
+  // N-best output (uis_predict*_nbest): hypothesis j of utterance u is the j-th final rank with at least
+  // min_speakers clusters (nbest_rank); its labels are plane j of `labels` (plane stride label_plane rows)
+  int n_best;              // >= 1; 1 = labels plane 0 only
+  long long label_plane;   // rows per label plane (n_best > 1)
+  float* nbest_scores;     // [U][n_best]  neg_likelihood, +inf where absent (may be null)
+  int* nbest_speakers;     // [U][n_best]  clusters, 0 where absent (may be null)
+  int* nbest_count;        // [U]          hypotheses returned (may be null)
 };
 
 // Per-utterance speaker bounds: a hypothesis may hold at most spk_max clusters; the returned one is the best-ranked
@@ -148,6 +155,28 @@ __device__ inline int spk_pick(const int* K, int n, int kmin) {
   for (int r = 0; r < n; ++r)
     if (K[r] >= kmin) return r;
   return 0;
+}
+// Rank of N-best hypothesis j < n_best among n final ranks: the j-th rank with K[r] >= kmin; rank 0 for j = 0 when
+// none qualifies (spk_pick); -1 when absent.
+__device__ inline int nbest_rank(const int* K, int n, int kmin, int j) {
+  int seen = 0;
+#pragma unroll 1
+  for (int r = 0; r < n; ++r)
+    if (K[r] >= kmin && seen++ == j) return r;
+  return (j == 0) ? 0 : -1;
+}
+// Hypotheses an N-best call returns: the qualifying ranks up to n_best, or 1 (the rank-0 fall-back).
+__device__ inline int nbest_n(const int* K, int n, int kmin, int n_best) {
+  int c = 0;
+#pragma unroll 1
+  for (int r = 0; r < n && c < n_best; ++r) c += K[r] >= kmin;
+  return c > 0 ? c : 1;
+}
+// Per-hypothesis outputs of hypothesis j (rank r, -1 = absent) of a finished utterance u.
+__device__ inline void nbest_store(const BeamParams& p, int u, int j, int r, const int* K, const float* Nl) {
+  const float INF = __int_as_float(0x7f800000);
+  if (p.nbest_scores) p.nbest_scores[(size_t)u * p.n_best + j] = r >= 0 ? Nl[r] : INF;
+  if (p.nbest_speakers) p.nbest_speakers[(size_t)u * p.n_best + j] = r >= 0 ? K[r] : 0;
 }
 
 template <int V> struct Pow2Floor { static constexpr int value = (V >= 2) ? 2 * Pow2Floor<V / 2>::value : 1; };
@@ -189,7 +218,7 @@ __host__ __device__ inline unsigned align_up(unsigned v, unsigned a) { return (v
 // lane scalars (ints) ------------------------------------------------------------------------
 enum { LS_U = 0, LS_N, LS_TN, LS_T, LS_NB, LS_GEN, LS_ACTIVE, LS_FAILED, LS_TRACED, LS_NFINITE, LS_KMAX,
        LS_NWIN, LS_ERR, LS_M, LS_COLBASE, LS_NE, LS_ROW0_LO, LS_ROW0_HI, LS_DBGROWS_LO, LS_DBGROWS_HI,
-       LS_FRESH, LS_PICK, LS_KHI, LS_KLO, LS_COUNT = 24 };  // LS_KHI / LS_KLO: speaker bounds
+       LS_FRESH, LS_KHI, LS_KLO, LS_COUNT = 24 };  // LS_KHI / LS_KLO: speaker bounds
 // CTA scalars
 enum { MI_PUBLISHED = 0, MI_DONE, MI_MTOT, MI_QNEXT, MI_NLIST, MI_MAXK };
 
@@ -1102,6 +1131,8 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
       if (N == 0) {
         p.status[u] = 0;
         if (p.spk_out) p.spk_out[u] = 0;
+        if (p.nbest_count) p.nbest_count[u] = 0;
+        for (int j = 0; j < p.n_best; ++j) nbest_store(p, u, j, -1, nullptr, nullptr);
         if (p.dbg_final_scores && tap_leader) {
           for (int b = 0; b < B; ++b) p.dbg_final_scores[(size_t)u * B + b] = INF;
           if (p.dbg_final_k) p.dbg_final_k[u] = 0;
@@ -1666,10 +1697,30 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
       const bool ok = !ls[LS_ERR] && nwin > 0;
       const int* fK = reinterpret_cast<const int*>(lane_base(g) + L.l_meta) + ngen * 4 * B;
       const float* fNl = reinterpret_cast<const float*>(fK + 3 * B);
-      if (tid == 0) {  // the returned hypothesis: the first final rank with min_speakers clusters (else rank 0)
-        const int r = ok ? spk_pick(fK, nwin, ls[LS_KLO]) : 0;
-        ls[LS_PICK] = r;
-        if (p.spk_out && !(STAT && sq != 0)) p.spk_out[u] = ok ? fK[r] : 0;
+      // utterance epilogue: back-track the returned hypotheses (uisrnn.py:561), one per thread.  Hypothesis j is the
+      // j-th final rank with min_speakers clusters (rank 0 when none has them, j = 0); it walks its own column chain
+      // into label plane j.  (Stationary-weights mode: the replicas of a group decode the same utterance, and CTA 0
+      // of the group reports it.)
+      for (int j = tid; j < p.n_best && !(STAT && sq != 0); j += NT) {
+        const int r0 = ok ? nbest_rank(fK, nwin, ls[LS_KLO], j) : -1;
+        const int N = ls[LS_N];
+        int* lab = p.labels + (size_t)j * p.label_plane + (((long long)ls[LS_ROW0_HI] << 32) | (unsigned)ls[LS_ROW0_LO]);
+        if (r0 < 0) {
+          for (int i = 0; i < N; ++i) lab[i] = -1;
+        } else {
+          const unsigned* bp = bp_cta + (size_t)g * p.maxN * B;
+          int r = r0;
+          for (int i = N - 1; i >= 0; --i) {
+            const unsigned e = bp[(size_t)i * B + r];
+            lab[i] = (int)(e & 0xffffu);
+            r = (int)(e >> 16);
+          }
+        }
+        if (j == 0) {
+          if (p.spk_out) p.spk_out[u] = ok ? fK[r0] : 0;
+          if (p.nbest_count) p.nbest_count[u] = ok ? nbest_n(fK, nwin, ls[LS_KLO], p.n_best) : 0;
+        }
+        nbest_store(p, u, j, r0, fK, fNl);
       }
       if (p.dbg_final_scores && tap_leader) {
         if (tid < B) p.dbg_final_scores[(size_t)u * B + tid] = (ok && tid < nwin) ? fNl[tid] : INF;
@@ -1700,24 +1751,8 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
       const int g = tid;
       volatile int* ls = LSp(g);
       if (ls[LS_ACTIVE]) {
-        if (fin[g]) {  // utterance epilogue: back-track the best hypothesis (uisrnn.py:561)
-          const int u = ls[LS_U], N = ls[LS_N];
-          const long long row0 = ((long long)ls[LS_ROW0_HI] << 32) | (unsigned)ls[LS_ROW0_LO];
-          if (STAT && sq != 0) {
-            // (the replicas of a group decode the same utterance: CTA 0 of the group reports it)
-          } else if (ls[LS_ERR] || ls[LS_NWIN] == 0) {
-            p.status[u] = ls[LS_ERR] ? -4 : -1;
-            for (int i = 0; i < N; ++i) p.labels[row0 + i] = -1;
-          } else {
-            p.status[u] = 0;
-            const unsigned* bp = bp_cta + (size_t)g * p.maxN * B;
-            int r = ls[LS_PICK];
-            for (int i = N - 1; i >= 0; --i) {
-              const unsigned e = bp[(size_t)i * B + r];
-              p.labels[row0 + i] = (int)(e & 0xffffu);
-              r = (int)(e >> 16);
-            }
-          }
+        if (fin[g]) {
+          if (!(STAT && sq != 0)) p.status[ls[LS_U]] = ls[LS_ERR] ? -4 : ls[LS_NWIN] == 0 ? -1 : 0;
           lane_fetch(g);
         } else {
           const long long rows = (((long long)ls[LS_DBGROWS_HI] << 32) | (unsigned)ls[LS_DBGROWS_LO]) + ls[LS_NWIN];

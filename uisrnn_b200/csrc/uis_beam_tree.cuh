@@ -627,35 +627,35 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
     }  // beam steps
 
     named_bar_sync(1, NT);
+    const bool ok = !(failed || misc[TM_ERR]);
     if (tid == 0) {
-      if (failed || misc[TM_ERR]) {
-        const int e = misc[TM_ERR];
-        p.status[u] = (e == 1) ? -4 : (e == 2 || e == 3) ? -5 : -1;
-        for (int i = 0; i < N; ++i) p.labels[row0 + i] = -1;
+      const int e = misc[TM_ERR];
+      p.status[u] = ok ? 0 : (e == 1) ? -4 : (e == 2 || e == 3) ? -5 : -1;
+    }
+    // back-track the returned hypotheses, one per thread: hypothesis j is the j-th final rank with min_speakers
+    // clusters (rank 0 when none has them, j = 0) and walks its own column chain into label plane j
+    for (int j = tid; j < p.n_best; j += NT) {
+      const int* fK = meta + gen * 4 * B;
+      const int r0 = ok ? nbest_rank(fK, nb, spk_min(p, u), j) : -1;
+      int* lab = p.labels + (size_t)j * p.label_plane + row0;
+      if (r0 < 0) {
+        for (int i = 0; i < N; ++i) lab[i] = -1;
       } else {
-        p.status[u] = 0;
-        const int nsteps = (TN + L - 1) / L;
-        const int pick = spk_pick(meta + gen * 4 * B, nb, spk_min(p, u));
-        if (pick != 0) {  // back-track from rank `pick`: its last-step back-pointers move to column 0
-          const int t0 = (nsteps - 1) * L, Lc = min(L, TN - t0);
-          for (int i = 0; i < Lc; ++i) bp_lab[(size_t)(t0 + i) * B] = bp_lab[(size_t)(t0 + i) * B + pick];
-          bp_par[(size_t)(nsteps - 1) * B] = bp_par[(size_t)(nsteps - 1) * B + pick];
-        }
-        int r = 0;
-        for (int s = nsteps - 1; s >= 0 && (long long)s * L + L > TN - N; --s) {
+        int r = r0;
+        for (int s = (TN + L - 1) / L - 1; s >= 0 && (long long)s * L + L > TN - N; --s) {
           const int t0 = s * L, Lc = min(L, TN - t0);
           for (int i = Lc - 1; i >= 0; --i) {
             const int f = t0 + i;
-            if (f >= TN - N) p.labels[row0 + (f - (TN - N))] = (int)bp_lab[(size_t)f * B + r];
+            if (f >= TN - N) lab[f - (TN - N)] = (int)bp_lab[(size_t)f * B + r];
           }
           r = (int)bp_par[(size_t)s * B + r];
         }
       }
+      // clusters of hypothesis 0, 0 for a failed utterance; an empty utterance returns no N-best hypothesis
+      if (j == 0 && p.spk_out) p.spk_out[u] = ok ? fK[r0] : 0;
+      if (j == 0 && p.nbest_count) p.nbest_count[u] = (ok && N > 0) ? nbest_n(fK, nb, spk_min(p, u), p.n_best) : 0;
+      nbest_store(p, u, j, N > 0 ? r0 : -1, fK, reinterpret_cast<const float*>(fK + 3 * B));
     }
-    const bool ok = !(failed || misc[TM_ERR]);
-    // clusters of the returned hypothesis, 0 for a failed utterance (stored apart from the back-track: there it
-    // costs the (1024, 512) kernels spill)
-    if (tid == 0 && p.spk_out) p.spk_out[u] = ok ? meta[gen * 4 * B + spk_pick(meta + gen * 4 * B, nb, spk_min(p, u))] : 0;
     if (p.dbg_final_scores) {
       const float* fNl = reinterpret_cast<const float*>(meta + gen * 4 * B + 3 * B);
       if (tid < B) p.dbg_final_scores[(size_t)u * B + tid] = (ok && tid < nb) ? fNl[tid] : INF;

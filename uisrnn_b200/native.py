@@ -20,7 +20,7 @@ UIS_ERR_CUDA = -3
 UIS_ERR_OVERFLOW = -4
 UIS_ERR_NOMEM = -5
 UIS_ERR_CAPACITY = -6
-UIS_ABI_VERSION = 5  # include/uisrnn_b200.h
+UIS_ABI_VERSION = 6  # include/uisrnn_b200.h
 
 
 class NativeError(RuntimeError):
@@ -43,6 +43,11 @@ class DebugTaps(C.Structure):
               ('best_hidden', C.POINTER(C.c_float)), ('best_blocks', C.POINTER(C.c_int32))]
 
 
+class NBestOut(C.Structure):
+  _fields_ = [('labels_out', C.POINTER(C.c_void_p)), ('labels_dev', C.c_void_p), ('scores', C.POINTER(C.c_float)),
+              ('speakers', C.POINTER(C.c_int32)), ('count', C.POINTER(C.c_int32))]
+
+
 class Stats(C.Structure):
   _fields_ = [('utterances', C.c_int64), ('frames', C.c_int64), ('beam_steps', C.c_int64),
               ('gru_columns', C.c_int64), ('weight_passes', C.c_int64), ('candidates', C.c_int64),
@@ -63,7 +68,7 @@ class Stats(C.Structure):
 # Every symbol include/uisrnn_b200.h declares (tests check the .so exports all of them).
 EXPORTS = ('uis_version', 'uis_last_error', 'uis_model_create', 'uis_model_destroy',
            'uis_model_constants', 'uis_predict', 'uis_predict_device', 'uis_predict_bounded',
-           'uis_predict_device_bounded',
+           'uis_predict_device_bounded', 'uis_predict_nbest', 'uis_predict_device_nbest',
            'uis_predict_workspace_bytes', 'uis_get_stats', 'uis_trainer_create',
            'uis_trainer_destroy', 'uis_trainer_step', 'uis_trainer_get', 'uis_trainer_losses',
            'uis_trainer_comm_size', 'uis_trainer_comm_export', 'uis_trainer_comm_apply',
@@ -151,6 +156,14 @@ def load_library():
   lib.uis_predict_bounded.argtypes = lib.uis_predict.argtypes + [ip, ip, ip]
   lib.uis_predict_device_bounded.restype = C.c_int
   lib.uis_predict_device_bounded.argtypes = lib.uis_predict_device.argtypes + [ip, ip, C.c_void_p]
+  lib.uis_predict_nbest.restype = C.c_int
+  lib.uis_predict_nbest.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int,
+                                    C.POINTER(PredictOpts), C.POINTER(DebugTaps), C.c_void_p, ip, ip, C.c_int32,
+                                    C.POINTER(NBestOut)]
+  lib.uis_predict_device_nbest.restype = C.c_int
+  lib.uis_predict_device_nbest.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int,
+                                           C.POINTER(PredictOpts), C.POINTER(DebugTaps), C.c_void_p, ip, ip,
+                                           C.c_int32, C.POINTER(NBestOut)]
   lib.uis_predict_workspace_bytes.restype = C.c_size_t
   lib.uis_predict_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.c_int,
                                               C.POINTER(PredictOpts)]
@@ -214,6 +227,15 @@ def speaker_bounds(n, max_speakers=None, min_speakers=None):
   if mx is not None and mn is not None and ((mx > 0) & (mn > mx)).any():
     raise ValueError('min_speakers must not exceed max_speakers')
   return mx, mn
+
+
+def check_n_best(n_best, beam_size):
+  """Raises ValueError unless n_best is an int in [1, beam_size]."""
+  if isinstance(n_best, (bool, np.bool_)) or not isinstance(n_best, (int, np.integer)):
+    raise ValueError('n_best must be an int, got {!r}'.format(n_best))
+  if not 1 <= n_best <= beam_size:
+    raise ValueError('n_best must be in [1, beam_size={}], got {}'.format(beam_size, n_best))
+  return int(n_best)
 
 
 class NativeModel:
@@ -297,15 +319,20 @@ class NativeModel:
 
   def predict(self, seqs, beam_size=10, look_ahead=1, test_iteration=2, kcap=0, n_ctas=0,
               trace_utt=None, stream=0, lanes=0, cluster=0, engine=0, max_speakers=None, min_speakers=None,
-              return_speakers=False):
+              return_speakers=False, n_best=None):
     """seqs: list of C-contiguous float64 [N_u, D] arrays (host).  Returns a list of int32
     label arrays (and a dict of debug arrays when trace_utt is not None).
+
+    n_best=k (1 <= k <= beam_size, uis_predict_nbest): returns (labels, scores, speakers, count) instead, where
+    labels[u] is int32 [k][N_u] (row 0 = the labels of the same call without n_best), scores float32 [U][k]
+    (neg_likelihood, +inf where absent), speakers int32 [U][k] and count int32 [U]; return_speakers is ignored.
 
     max_speakers / min_speakers: an int for every utterance or one value per utterance, 0 = no bound
     (uis_predict_bounded in include/uisrnn_b200.h).  return_speakers=True appends an int32 array with the
     cluster count of every returned hypothesis to the result."""
     n = len(seqs)
     mx, mn = speaker_bounds(n, max_speakers, min_speakers)
+    k = 1 if n_best is None else check_n_best(n_best, beam_size)
     keep = [s if (type(s) is np.ndarray and s.dtype == np.float64 and s.flags.c_contiguous)
             else np.ascontiguousarray(s, dtype=np.float64) for s in seqs]
     for s in keep:
@@ -315,9 +342,9 @@ class NativeModel:
     lens = np.fromiter((s.shape[0] for s in keep), dtype=np.int64, count=n) if n else np.zeros(1, np.int64)
     offs = np.zeros(n + 1, np.int64)
     np.cumsum(lens[:n], out=offs[1:])
-    flat = np.empty(max(int(offs[-1]), 1), np.int32)
-    outs = [flat[offs[i]:offs[i + 1]] for i in range(n)]
-    out_addr = (flat.ctypes.data + 4 * offs[:max(n, 1)]).astype(np.uint64)
+    flat = np.empty(max(k * int(offs[-1]), 1), np.int32)
+    outs = [flat[k * offs[i]:k * offs[i + 1]] for i in range(n)]
+    out_addr = (flat.ctypes.data + 4 * k * offs[:max(n, 1)]).astype(np.uint64)
     in_addr = np.fromiter((s.ctypes.data for s in keep), dtype=np.uint64, count=n) if n else np.zeros(1, np.uint64)
     lengths = lens.ctypes.data_as(C.POINTER(C.c_int64))
     in_ptrs = in_addr.ctypes.data_as(C.POINTER(C.c_void_p))
@@ -331,10 +358,21 @@ class NativeModel:
     ip = C.POINTER(C.c_int32)
     spk = np.zeros(max(n, 1), np.int32) if return_speakers else None
     arg = lambda a: a.ctypes.data_as(ip) if a is not None else None
-    rc = self._lib.uis_predict_bounded(self._h, in_ptrs, lengths, n, C.byref(opts), out_ptrs, tp,
-                                       C.c_void_p(stream), arg(mx), arg(mn), arg(spk))
+    if n_best is None:
+      rc = self._lib.uis_predict_bounded(self._h, in_ptrs, lengths, n, C.byref(opts), out_ptrs, tp,
+                                         C.c_void_p(stream), arg(mx), arg(mn), arg(spk))
+    else:
+      scores = np.empty((max(n, 1), k), np.float32)
+      nb_spk = np.empty((max(n, 1), k), np.int32)
+      count = np.empty(max(n, 1), np.int32)
+      nb = NBestOut(out_ptrs, None, scores.ctypes.data_as(C.POINTER(C.c_float)), nb_spk.ctypes.data_as(ip),
+                    count.ctypes.data_as(ip))
+      rc = self._lib.uis_predict_nbest(self._h, in_ptrs, lengths, n, C.byref(opts), tp, C.c_void_p(stream),
+                                       arg(mx), arg(mn), k, C.byref(nb))
     _check(self._lib, rc)
-    if return_speakers:
+    if n_best is not None:
+      outs = ([o.reshape(k, int(lens[i])) for i, o in enumerate(outs)], scores[:n], nb_spk[:n], count[:n])
+    elif return_speakers:
       outs = (outs, spk[:n])
     if bufs is not None:
       nrows = int(bufs['off'][-1]) if len(bufs['off']) else 0
@@ -349,14 +387,27 @@ class NativeModel:
 
   def predict_device(self, x_ptr, frame_offsets, labels_ptr, beam_size=10, look_ahead=1,
                      test_iteration=2, kcap=0, n_ctas=0, stream=0, lanes=0, cluster=0, engine=0,
-                     max_speakers=None, min_speakers=None, speakers_ptr=0):
+                     max_speakers=None, min_speakers=None, speakers_ptr=0, n_best=None, scores_ptr=0,
+                     nbest_speakers_ptr=0, count_ptr=0):
     """Device-resident variant: x_ptr -> fp32 [rows, D], labels_ptr -> int32 [rows] (raw
     device addresses, e.g. torch.Tensor.data_ptr()).  Asynchronous on `stream`.  Speaker bounds as in
-    predict(); speakers_ptr (device int32 [U], 0 = none) receives the cluster counts."""
+    predict(); speakers_ptr (device int32 [U], 0 = none) receives the cluster counts.
+
+    n_best=k (uis_predict_device_nbest): labels_ptr -> int32 [k][rows]; scores_ptr -> float32 [U][k] (required),
+    nbest_speakers_ptr -> int32 [U][k] and count_ptr -> int32 [U] (0 = none); speakers_ptr is ignored."""
     off = np.ascontiguousarray(frame_offsets, dtype=np.int64)
     mx, mn = speaker_bounds(len(off) - 1, max_speakers, min_speakers)
     ip = C.POINTER(C.c_int32)
     opts = self._opts(beam_size, look_ahead, test_iteration, kcap, n_ctas, lanes, cluster, engine)
+    if n_best is not None:
+      k = check_n_best(n_best, beam_size)
+      nb = NBestOut(None, C.c_void_p(labels_ptr), C.cast(C.c_void_p(scores_ptr), C.POINTER(C.c_float)),
+                    C.cast(C.c_void_p(nbest_speakers_ptr), ip), C.cast(C.c_void_p(count_ptr), ip))
+      _check(self._lib, self._lib.uis_predict_device_nbest(
+          self._h, C.c_void_p(x_ptr), off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1, C.byref(opts), None,
+          C.c_void_p(stream), mx.ctypes.data_as(ip) if mx is not None else None,
+          mn.ctypes.data_as(ip) if mn is not None else None, k, C.byref(nb)))
+      return
     rc = self._lib.uis_predict_device_bounded(self._h, C.c_void_p(x_ptr),
                                               off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1,
                                               C.byref(opts), C.c_void_p(labels_ptr), None,

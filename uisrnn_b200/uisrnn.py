@@ -9,6 +9,7 @@ There is no silent fallback: on a CUDA device an unsupported configuration raise
 device (explicit `--enable_cuda=False`, the reference's own device rule) the decoder in
 `beam_cpu.py` is used.  Training uses PyTorch autograd on the model's device.
 """
+import collections
 import functools
 import threading
 import warnings
@@ -26,6 +27,10 @@ from . import loss_func
 from . import utils
 
 _INITIAL_SIGMA2_VALUE = 0.1
+# One utterance's N-best result (predict(..., n_best=k)): up to k hypotheses in rank order -- their label lists (the
+# last tiled copy), their neg_likelihood over the whole decode and their cluster counts.
+NBest = collections.namedtuple('NBest', ['labels', 'scores', 'speakers'])
+
 _DEFAULT_KCAP = 0  # clusters per hypothesis held in device tables: 0 = the library's default (16 or 32, by kernel); grown on overflow
 
 
@@ -413,10 +418,11 @@ class UISRNN:
         self._native = (key, native.NativeModel(self.export_weights(), device=index))
       return self._native[1]
 
-  def _predict_cuda(self, sequences, args, device_index=None, as_arrays=False, bounds=(None, None)):
+  def _predict_cuda(self, sequences, args, device_index=None, as_arrays=False, bounds=(None, None), n_best=None):
     """Labels of `sequences` from the native library; with speaker bounds (int32 arrays from
-    native.speaker_bounds, None = absent) returns (labels, cluster counts)."""
-    return _native_predict(self._native_model(device_index), sequences, args, as_arrays, bounds)
+    native.speaker_bounds, None = absent) returns (labels, cluster counts); with n_best, (NBest list, cluster
+    counts of hypothesis 0)."""
+    return _native_predict(self._native_model(device_index), sequences, args, as_arrays, bounds, n_best)
 
   def _decode_cpu(self, sequence, args, max_speakers=0, min_speakers=0):
     """(labels, cluster count) of one sequence on the CPU device."""
@@ -434,11 +440,29 @@ class UISRNN:
     labels = [np.asarray(o[0], np.int32) if as_arrays else o[0] for o in out]
     return labels, np.array([o[1] for o in out], np.int32)
 
-  def predict_single(self, test_sequence, args, *, max_speakers=None, min_speakers=None):
+  def _predict_nbest(self, sequences, args, bounds, n_best):
+    """(NBest list, cluster counts of hypothesis 0) of a checked list of sequences."""
+    if self.device.type == 'cuda':
+      return self._predict_cuda(sequences, args, bounds=bounds, n_best=n_best)
+    mx, mn = bounds
+    out = [_decode_cpu_nbest(self, args, n_best, s, mx[i] if mx is not None else 0, mn[i] if mn is not None else 0)
+           for i, s in enumerate(sequences)]
+    return out, np.array([o.speakers[0] if o.speakers else 0 for o in out], np.int32)
+
+  def predict_single(self, test_sequence, args, *, max_speakers=None, min_speakers=None, n_best=None):
     """Labels (list of N ints) for one test sequence [N, D] float64 (uisrnn.py:479-562).
 
-    max_speakers / min_speakers (ints, 0 or None = no bound) bound the number of speakers: see `predict`."""
+    max_speakers / min_speakers (ints, 0 or None = no bound) bound the number of speakers, and n_best returns
+    an NBest instead: see `predict`."""
     _check_test_sequence(test_sequence, self.observation_dim)
+    if n_best is not None:
+      if np.ndim(max_speakers) or np.ndim(min_speakers):
+        raise ValueError('predict_single takes one int per bound')
+      k = _check_n_best(n_best, args)
+      bounds = _speaker_bounds(1, max_speakers, min_speakers)
+      out, speakers = self._predict_nbest([test_sequence], args, bounds, k)
+      _warn_min_speakers([0], [len(test_sequence)], speakers, bounds[1])
+      return out[0]
     if max_speakers is None and min_speakers is None:
       if self.device.type == 'cuda':
         return self._predict_cuda([test_sequence], args)[0]
@@ -450,7 +474,7 @@ class UISRNN:
     _warn_min_speakers([0], [len(test_sequence)], speakers, bounds[1])
     return labels[0]
 
-  def predict(self, test_sequences, args, *, max_speakers=None, min_speakers=None):
+  def predict(self, test_sequences, args, *, max_speakers=None, min_speakers=None, n_best=None):
     """Labels for one sequence (ndarray -> list of ints) or many (list -> list of lists)
     (uisrnn.py:564-590).  On CUDA a list is decoded by a single native call.
 
@@ -459,9 +483,26 @@ class UISRNN:
     label is < max_speakers.  The labels come from the best-ranked final hypothesis with at least min_speakers
     clusters; when the final beam holds none, rank 0's labels are returned and one warning names those utterances.
     Clusters are counted over the whole decode (test_iteration tiled copies), so with test_iteration > 1 the
-    returned labels may use fewer distinct ids than min_speakers."""
+    returned labels may use fewer distinct ids than min_speakers.
+
+    N-best (not in the reference): with `n_best` = k (1 <= k <= beam_size) every utterance gives an `NBest`
+    (labels, scores, speakers) instead of a label list: one NBest for an ndarray, a list of them for a list.  It holds
+    up to k final hypotheses in rank order -- the first k final ranks with at least min_speakers clusters, or rank 0
+    alone when none has them -- so hypothesis 0 is what the call returns without n_best.  `scores` are the
+    hypotheses' neg_likelihood accumulated over the whole decode (lower is better; the gap between the first two is
+    a confidence), `speakers` their cluster counts.  An empty sequence gives no hypothesis.  With test_iteration > 1
+    two hypotheses can differ only in an earlier tiled copy and so carry the same labels; they are kept apart."""
     if isinstance(test_sequences, np.ndarray):
-      return self.predict_single(test_sequences, args, max_speakers=max_speakers, min_speakers=min_speakers)
+      return self.predict_single(test_sequences, args, max_speakers=max_speakers, min_speakers=min_speakers,
+                                 n_best=n_best)
+    if isinstance(test_sequences, list) and n_best is not None:
+      k = _check_n_best(n_best, args)
+      for sequence in test_sequences:
+        _check_test_sequence(sequence, self.observation_dim)
+      bounds = _speaker_bounds(len(test_sequences), max_speakers, min_speakers)
+      out, speakers = self._predict_nbest(test_sequences, args, bounds, k)
+      _warn_min_speakers(range(len(test_sequences)), [len(s) for s in test_sequences], speakers, bounds[1])
+      return out
     if isinstance(test_sequences, list):
       if max_speakers is not None or min_speakers is not None:
         for sequence in test_sequences:
@@ -494,9 +535,21 @@ def _warn_min_speakers(indices, lengths, speakers, min_speakers):
                   'the best hypothesis was returned instead'.format(short), RuntimeWarning, stacklevel=3)
 
 
-def _native_predict(model, sequences, args, as_arrays, bounds):
+def _check_n_best(n_best, args):
+  from . import native  # validation only: the library is not loaded
+  return native.check_n_best(n_best, args.beam_size)
+
+
+def _nbest_result(labels, scores, speakers, count):
+  """NBest list of a native N-best call (entries truncated to each utterance's count)."""
+  return [NBest([row.tolist() for row in lab[:c]], [float(v) for v in sc[:c]], [int(v) for v in sp[:c]])
+          for lab, sc, sp, c in zip(labels, scores, speakers, count)]
+
+
+def _native_predict(model, sequences, args, as_arrays, bounds, n_best=None):
   """NativeModel.predict with the kcap retry: a hypothesis that opened more clusters than the device tables hold
-  fails with UIS_ERR_OVERFLOW, and the call is repeated with larger tables."""
+  fails with UIS_ERR_OVERFLOW, and the call is repeated with larger tables.  With n_best: (NBest list, cluster
+  counts of hypothesis 0)."""
   from . import native
   mx, mn = bounds
   bounded = mx is not None or mn is not None
@@ -506,7 +559,9 @@ def _native_predict(model, sequences, args, as_arrays, bounds):
       with model.lock:  # a uis_model handle (one workspace) is not re-entrant
         out = model.predict(sequences, beam_size=args.beam_size, look_ahead=args.look_ahead,
                             test_iteration=args.test_iteration, kcap=kcap, max_speakers=mx, min_speakers=mn,
-                            return_speakers=bounded)
+                            return_speakers=bounded, n_best=n_best)
+      if n_best is not None:
+        return _nbest_result(*out), out[2][:, 0].copy()
       labels, speakers = out if bounded else (out, None)
       labels = labels if as_arrays else [lab.tolist() for lab in labels]
       return (labels, speakers) if bounded else labels
@@ -516,8 +571,8 @@ def _native_predict(model, sequences, args, as_arrays, bounds):
       kcap = 32 if kcap == 0 else kcap * 2  # a hypothesis opened more clusters than the device tables hold: grow and retry
 
 
-def _predict_shard(model, args, device_index, sequences, out, position, bounds):
-  out[position] = model._predict_cuda(sequences, args, device_index, bounds=bounds)  # pylint: disable=protected-access
+def _predict_shard(model, args, device_index, sequences, out, position, bounds, n_best=None):
+  out[position] = model._predict_cuda(sequences, args, device_index, bounds=bounds, n_best=n_best)  # pylint: disable=protected-access
 
 
 def _take(bound, indices):
@@ -529,18 +584,28 @@ def _decode_cpu_bounded(model, args, sequence, max_speakers, min_speakers):
   return model._decode_cpu(sequence, args, max_speakers, min_speakers)  # pylint: disable=protected-access
 
 
-def parallel_predict(model, test_sequences, args, num_processes=4, *, max_speakers=None, min_speakers=None):
+def _decode_cpu_nbest(model, args, n_best, sequence, max_speakers, min_speakers):
+  """NBest of one sequence on the CPU device (module level: the CPU parallel_predict's pool pickles it)."""
+  decoder = beam_cpu.CpuBeamSearch(model)
+  return NBest(*decoder.decode(sequence, args.beam_size, args.look_ahead, args.test_iteration, int(max_speakers),
+                               int(min_speakers), n_best=n_best))
+
+
+def parallel_predict(model, test_sequences, args, num_processes=4, *, max_speakers=None, min_speakers=None,
+                     n_best=None):
   """Parallel prediction over a list of sequences (uisrnn.py:593-623).
 
   CPU model: a forkserver process pool, as the reference.  CUDA model: `num_processes` is the
   number of GPUs to use (capped by the visible devices); the list is split by total frame count
   and each shard is decoded by one native call on its own device, from its own host thread
   (the C ABI releases the GIL).  Utterances are independent, so there is no collective.
-  Speaker bounds as in `UISRNN.predict`; per-utterance values travel with their shards.
+  Speaker bounds and n_best as in `UISRNN.predict`; per-utterance values travel with their shards.
   """
   if not isinstance(test_sequences, list):
     raise TypeError('test_sequences must be a list.')
-  bounded = max_speakers is not None or min_speakers is not None
+  if n_best is not None:
+    n_best = _check_n_best(n_best, args)
+  bounded = max_speakers is not None or min_speakers is not None or n_best is not None
   bounds = _speaker_bounds(len(test_sequences), max_speakers, min_speakers) if bounded else (None, None)
   if model.device.type == 'cuda':
     for sequence in test_sequences:
@@ -548,7 +613,7 @@ def parallel_predict(model, test_sequences, args, num_processes=4, *, max_speake
     n_dev = max(1, min(int(num_processes), torch.cuda.device_count()))
     if n_dev == 1 or len(test_sequences) < 2:
       if bounded:
-        return model.predict(test_sequences, args, max_speakers=bounds[0], min_speakers=bounds[1])
+        return model.predict(test_sequences, args, max_speakers=bounds[0], min_speakers=bounds[1], n_best=n_best)
       return model._predict_cuda(test_sequences, args)  # pylint: disable=protected-access
     shards = shard_by_frames([len(s) for s in test_sequences], n_dev)
     twins = [model] + [_clone_for_device(model, d) for d in range(1, n_dev)]
@@ -556,7 +621,7 @@ def parallel_predict(model, test_sequences, args, num_processes=4, *, max_speake
     for d, shard in enumerate(shards):
       thread = threading.Thread(target=_predict_shard, args=(
           twins[d], args, d, [test_sequences[i] for i in shard], results, d,
-          (_take(bounds[0], shard), _take(bounds[1], shard))))
+          (_take(bounds[0], shard), _take(bounds[1], shard)), n_best))
       thread.start()
       threads.append(thread)
     for thread in threads:
@@ -582,9 +647,15 @@ def parallel_predict(model, test_sequences, args, num_processes=4, *, max_speake
     for sequence in test_sequences:
       _check_test_sequence(sequence, model.observation_dim)
     n = len(test_sequences)
-    out = pool.starmap(functools.partial(_decode_cpu_bounded, model, args), zip(
+    task = functools.partial(_decode_cpu_bounded, model, args) if n_best is None else \
+        functools.partial(_decode_cpu_nbest, model, args, n_best)
+    out = pool.starmap(task, zip(
         test_sequences, bounds[0] if bounds[0] is not None else [0] * n,
         bounds[1] if bounds[1] is not None else [0] * n))
+  if n_best is not None:
+    _warn_min_speakers(range(n), [len(s) for s in test_sequences], [o.speakers[0] if o.speakers else 0 for o in out],
+                       bounds[1])
+    return out
   _warn_min_speakers(range(n), [len(s) for s in test_sequences], [o[1] for o in out], bounds[1])
   return [o[0] for o in out]
 
@@ -597,13 +668,13 @@ class _DeviceTwin:
     self._models = {}
     self._lock = threading.Lock()
 
-  def _predict_cuda(self, sequences, args, device_index, bounds=(None, None)):
+  def _predict_cuda(self, sequences, args, device_index, bounds=(None, None), n_best=None):
     from . import native
     with self._lock:
       if device_index not in self._models:
         self._models[device_index] = native.NativeModel(self._weights, device=device_index)
       model = self._models[device_index]
-    return _native_predict(model, sequences, args, False, bounds)
+    return _native_predict(model, sequences, args, False, bounds, n_best)
 
 
 def _clone_for_device(model, device_index):
