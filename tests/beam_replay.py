@@ -19,6 +19,7 @@ Whether d2[0] is an exact fp32 zero cannot be decided from a float64 state: a ca
 within ZERO_BAND is marked ambiguous (its +inf status is the kernel's to decide), except new-cluster candidates when
 the kernel's own mean0 (uis_model_constants) is given, which decide it exactly."""
 import contextlib
+import types
 
 import numpy as np
 
@@ -66,18 +67,32 @@ class Model:
     self.mean0, self.hidden0 = m[0], h[0]
 
   def core(self, x, h):
-    """CoreRNN on a batch of columns: x [n, D], h [n, depth, H] -> mean [n, D], hidden [n, depth, H]."""
+    """CoreRNN on a batch of columns: x [n, D], h [n, depth, H] -> mean [n, D], hidden [n, depth, H].  numpy arrays,
+    or float64 torch tensors (on any device: the weights follow them there)."""
     H = self.H
-    inp, out = x, np.empty_like(h)
+    w, xp = self._weights_like(x)
+    inp, out = x, xp.empty_like(h)
     for l in range(self.depth):
-      gi = inp @ self.w_ih[l].T + self.b_ih[l]
-      gh = h[:, l] @ self.w_hh[l].T + self.b_hh[l]
-      r = 1 / (1 + np.exp(-(gi[:, :H] + gh[:, :H])))
-      z = 1 / (1 + np.exp(-(gi[:, H:2 * H] + gh[:, H:2 * H])))
-      n = np.tanh(gi[:, 2 * H:] + r * gh[:, 2 * H:])
+      gi = inp @ w.w_ih[l].T + w.b_ih[l]
+      gh = h[:, l] @ w.w_hh[l].T + w.b_hh[l]
+      r = 1 / (1 + xp.exp(-(gi[:, :H] + gh[:, :H])))
+      z = 1 / (1 + xp.exp(-(gi[:, H:2 * H] + gh[:, H:2 * H])))
+      n = xp.tanh(gi[:, 2 * H:] + r * gh[:, 2 * H:])
       out[:, l] = (h[:, l] - n) * z + n
       inp = out[:, l]
-    return np.maximum(inp @ self.w1.T + self.b1, 0) @ self.w2.T + self.b2, out
+    return (inp @ w.w1.T + w.b1).clip(min=0) @ w.w2.T + w.b2, out
+
+  def _weights_like(self, x):
+    if isinstance(x, np.ndarray):
+      return self, np
+    import torch
+    cache = self.__dict__.setdefault('_on_device', {})
+    if x.device not in cache:
+      t = lambda a: torch.as_tensor(a, dtype=torch.float64, device=x.device)
+      cache[x.device] = types.SimpleNamespace(
+          w_ih=[t(a) for a in self.w_ih], w_hh=[t(a) for a in self.w_hh], b_ih=[t(a) for a in self.b_ih],
+          b_hh=[t(a) for a in self.b_hh], w1=t(self.w1), b1=t(self.b1), w2=t(self.w2), b2=t(self.b2))
+    return cache[x.device], torch
 
 
 class Hyp:
@@ -375,3 +390,148 @@ def _check(replay, inc_rtol, labels, final, state_tol, worst, visit):
     lastsc = np.asarray(replay.score[replay.off[-2]:replay.off[-1]], np.float64)
     assert np.array_equal(fs[:len(lastsc)], lastsc) and np.all(np.isinf(fs[len(lastsc):]))
   return labs
+
+
+class PathScores:
+  """What path_score returns, per path: `score`, the float64 neg_likelihood; and the two parts of the allowance an
+  fp32 accumulation of the same path may differ by, as check() bounds each step: `ulps`, one fp32 ulp of the running
+  score per sub-step, and `mass`, the sum of |increment| (the part INC_RTOL scales).  Absent paths are nan."""
+
+  def __init__(self, score, ulps, mass):
+    self.score, self.ulps, self.mass = score, ulps, mass
+
+  def allowance(self, inc_rtol=INC_RTOL):
+    return self.ulps + inc_rtol * self.mass
+
+  def share(self, got, inc_rtol=INC_RTOL):
+    """|got - score| / allowance: how much of its allowance each fp32 score in `got` uses (<= 1 within it; +inf for
+    a path the float64 search scores +inf, 0 for an empty one)."""
+    err = np.abs(np.asarray(got, np.float64) - self.score)
+    with np.errstate(invalid='ignore', divide='ignore'):
+      return np.where(err == 0, 0.0, err / self.allowance(inc_rtol))
+
+
+def path_score(model, xs, labels, mean0=None, device='cpu', max_slots=1 << 17):
+  """Float64 rescoring of given label paths: the neg_likelihood the search assigns to a hypothesis whose cluster at
+  frame t is labels[t], summed over the frames with the score terms of Replay (running-mean off-by-one, log-term
+  association, first-column rule; `mean0`, the kernel's fp32 mean0, decides that rule exactly for new clusters).
+
+    xs      list of [N_u, D] inputs, already tiled (np.tile(x, (test_iteration, 1))) when the path covers the tiling
+    labels  list of int [R_u, N_u]: R_u paths over utterance u; a row of -1 is an absent rank (nan scores)
+
+  Returns a PathScores of arrays [sum R_u] in (utterance, row) order.  A path is its labels only at look_ahead 1 or
+  any look_ahead (the sub-steps of a tree step add the same per-frame increments), but only over the whole tiled
+  decode: predict() returns the last tiled copy, which at test_iteration > 1 leaves the earlier copies' labels, and so
+  every cluster's state, undetermined.  Rescore those from the back-track of a trace instead.
+
+  Batched in torch float64 on `device`: one GRU product per frame over every path of every utterance, each cluster
+  state evaluated once however many paths share it (a cluster's state depends only on the frames it holds so far, so
+  paths that agree on those share a node).  Utterances are taken in groups of at most `max_slots` cluster slots."""
+  import torch
+  m = model if isinstance(model, Model) else Model(model)
+  dev = torch.device(device)
+  f64 = dict(dtype=torch.float64, device=dev)
+  rows = [np.atleast_2d(np.asarray(lab, np.int64)) for lab in labels]
+  assert all(r.shape[1] == len(x) for x, r in zip(xs, rows)), 'labels and inputs of different lengths'
+  first = np.concatenate([[0], np.cumsum([len(r) for r in rows])]).astype(np.int64)
+  out = [np.full(int(first[-1]), np.nan) for _ in range(3)]
+  w = torch.as_tensor(m.w, **f64)
+  mean0_64 = torch.as_tensor(m.mean0, **f64)
+  hidden0 = torch.as_tensor(m.hidden0, **f64)
+  new0 = None if mean0 is None else float(np.asarray(mean0, F32)[0])
+  inf = torch.tensor(np.inf, dtype=torch.float32, device=dev)
+  # groups of utterances: a path of K clusters holds K slots
+  groups, cur, slots = [], [], 0
+  for u, r in enumerate(rows):
+    k = int(np.maximum(r.max(axis=1, initial=-1), -1).sum() + len(r)) if r.size else 0
+    if cur and slots + k > max_slots:
+      groups.append(cur)
+      cur, slots = [], 0
+    cur.append(u)
+    slots += k
+  groups.append(cur)
+  with torch.no_grad():
+    for us in groups:
+      paths = [(u, j) for u in us for j in range(len(rows[u])) if rows[u].shape[1] == 0 or rows[u][j, 0] >= 0]
+      if not paths:
+        continue
+      n_p = np.array([rows[u].shape[1] for u, _ in paths], np.int64)
+      lab = np.full((len(paths), max(1, int(n_p.max()))), -1, np.int64)
+      for p, (u, j) in enumerate(paths):
+        lab[p, :n_p[p]] = rows[u][j]
+      if (lab[np.arange(lab.shape[1]) < n_p[:, None]] < 0).any():
+        raise ValueError('a path has a -1 label inside its frames')
+      kp = lab.max(axis=1) + 1
+      base = np.concatenate([[0], np.cumsum(kp)[:-1]]).astype(np.int64)
+      S = int(kp.sum())
+      xg = [np.asarray(xs[u], np.float64).astype(F32) for u in us]
+      xoff = np.concatenate([[0], np.cumsum([len(x) for x in xg])]).astype(np.int64)
+      pos = {u: i for i, u in enumerate(us)}
+      X = torch.as_tensor(np.concatenate(xg).reshape(-1, m.D), device=dev)
+      utt = torch.as_tensor(np.array([pos[u] for u, _ in paths], np.int64), device=dev)
+      xrow = torch.as_tensor(xoff[[pos[u] for u, _ in paths]], device=dev)
+      lab_t, n_t, base_t = (torch.as_tensor(a, device=dev) for a in (lab, n_p, base))
+      mean = torch.zeros((S, m.D), **f64)
+      hid = torch.zeros((S, m.depth, m.H), **f64)
+      visits = torch.zeros(S, **f64)
+      blocks = torch.zeros(S, **f64)
+      nid = torch.full((S,), -1, dtype=torch.int64, device=dev)
+      P = len(paths)
+      K = torch.zeros(P, dtype=torch.int64, device=dev)
+      last = torch.full((P,), -1, dtype=torch.int64, device=dev)
+      tot = torch.zeros(P, **f64)
+      score, ulps, mass = torch.zeros(P, **f64), torch.zeros(P, **f64), torch.zeros(P, **f64)
+      next_id = 0
+      for t in range(int(n_p.max())):
+        live = torch.nonzero(n_t > t).squeeze(1)
+        c = lab_t[live, t]
+        Kl = K[live]
+        if bool((c > Kl).any()):
+          raise ValueError('frame %d: a label skips a cluster (labels open clusters in order 0, 1, ..)' % t)
+        new = c == Kl
+        slot = base_t[live] + c
+        x32 = X[xrow[live] + t]
+        x = x32.double()
+        # score terms (Replay._scores)
+        mu = torch.where(new[:, None], mean0_64[None], mean[slot])
+        d = mu - x
+        mse = (d * d) @ w
+        if new0 is None:
+          zero = d[:, 0] == 0
+        else:
+          zero = torch.where(new, x32[:, 0] == new0, d[:, 0] == 0)
+        mse = torch.where(zero, inf.double(), mse)
+        lt = torch.log(tot[live] + m.alpha)
+        pen = torch.where(new, m.pen_new_head - lt,
+                          torch.where(c == last[live], torch.full_like(lt, m.pen_last),
+                                      (m.log_p0 + torch.log(blocks[slot])) - lt))
+        inc = mse - pen
+        s = score[live] + inc
+        score[live] = s
+        a = s.abs().float()
+        ulps[live] += (torch.nextafter(a, inf) - a).double()
+        mass[live] += inc.abs()
+        # hypothesis bookkeeping (Replay._moved)
+        turn = new | (c != last[live])
+        blocks[slot] = blocks[slot] + turn.double()
+        tot[live] = tot[live] + turn.double()
+        K[live] = Kl + new.long()
+        last[live] = c
+        # advance the visited cluster: one core per distinct source state (Replay._advance)
+        key = torch.where(new, -1 - utt[live], nid[slot])
+        uniq, inv = torch.unique(key, return_inverse=True)
+        rep = torch.empty(len(uniq), dtype=torch.int64, device=dev).scatter_(
+            0, inv, torch.arange(len(inv), device=dev))
+        rs, rn = slot[rep], new[rep]
+        mo, ho = m.core(x[rep], torch.where(rn[:, None, None], hidden0[None], hid[rs]))
+        v = visits[rs]
+        mo = torch.where(rn[:, None], mo, (mean[rs] * (v - 1)[:, None] + mo) / v.clamp(min=1)[:, None])
+        mean[slot] = mo[inv]
+        hid[slot] = ho[inv]
+        visits[slot] = torch.where(new, torch.ones_like(v[inv]), visits[slot] + 1)
+        nid[slot] = next_id + inv
+        next_id += len(uniq)
+      idx = np.array([first[u] + j for u, j in paths], np.int64)
+      for o, v in zip(out, (score, ulps, mass)):
+        o[idx] = v.cpu().numpy()
+  return PathScores(*out)

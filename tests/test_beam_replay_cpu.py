@@ -1,6 +1,8 @@
 """The float64 step replay (tests/beam_replay.py) pinned without a GPU: every traced golden the unmodified reference
 produced, and oracle records on fresh inputs, pass its step, selection, state and label checks at the bounds below;
-and traces perturbed in the ways a kernel could go wrong fail them.
+and traces perturbed in the ways a kernel could go wrong fail them.  The path rescorer (beam_replay.path_score) is
+pinned the same way: every final rank of every traced golden, rescored from its labels alone, lies within the allowance
+of the reference's fp32 score (worst: 0.17 of it), and a relabelled frame or a score moved past the allowance fails.
 
 The reference's own fp32 search is what the replay is measured against here.  Its worst deviation over this file
 (printed by test_report_worst with `pytest -s`) is beside each bound; the bounds are about 10x that."""
@@ -157,10 +159,99 @@ def test_replay_keeps_first_column_rule():
     assert R.check(R.Replay(w, x, 10, 1, 1, rec['win'], rec['score'], rec['off'], mean0=mean0), REF_INC_RTOL) == labels
 
 
+def final_paths(case):
+  """Every final rank of a traced golden as (tiled x, labels [R, N * test_iteration], the reference's fp32 final
+  scores [R]): the back-track of the trace from each rank, over the whole tiled decode."""
+  off, T = case['off'], case['test_iteration']
+  tn = len(case['x']) * T
+  finals = int(off[-1] - off[-2])
+  labels = np.array([R.backtrack(case['win'], off, tn, r) for r in range(finals)], np.int64).reshape(finals, tn)
+  return np.tile(case['x'], (T, 1)), labels, case['score'][int(off[-2]):int(off[-1])].astype(np.float64)
+
+
+def rescore(case, worst=None):
+  x, labels, ref = final_paths(case)
+  res = R.path_score(load_weights(case['model']), [x], [labels])
+  used = res.share(ref, REF_INC_RTOL)
+  if worst is not None:
+    worst['path'] = max(worst.get('path', 0.0), float(used.max()))
+  return labels, ref, res, used
+
+
+@pytest.mark.parametrize('case', GOLDEN_CASES, ids=[c['name'] for c in GOLDEN_CASES])
+def test_rescored_final_ranks_match_reference(case):
+  """Every final rank of every traced golden (toy trace, small_cases, depth2_cases, speaker_bounds_cases: look_ahead
+  1-3, test_iteration 1-3, with and without bounds) rescored from its labels alone lies within the allowance of the
+  reference's own fp32 score; the recorded final traces and golden labels are the last tiled copy of those paths."""
+  labels, ref, res, used = rescore(case, WORST)
+  r = int(np.argmax(used))
+  assert used[r] <= 1, 'rank %d: score %.9g, float64 %.12g, allowed %.3g' % (r, ref[r], res.score[r],
+                                                                             res.allowance(REF_INC_RTOL)[r])
+  last = labels[:, labels.shape[1] - len(case['x']):]
+  if 'final_traces' in case:
+    assert np.array_equal(last, case['final_traces'][:len(labels)])
+  assert last[int(case.get('chosen', 0))].tolist() == case['labels'].tolist()
+
+
+def test_relabelled_frame_fails_the_rescore():
+  """Rank 0 of a 60-frame decode with every single frame moved to another cluster it could have joined: each of these
+  paths scores outside the allowance of the reference's rank-0 score."""
+  case = next(c for c in GOLDEN_CASES if c['name'] == 'bounds_s_min_pick')
+  x, labels, ref = final_paths(case)
+  path = labels[0]
+  moved = []
+  for t in range(1, len(path)):
+    opened = int(path[:t].max()) + 1
+    if path[t] < opened and opened > 1:  # (not the frame that opens its cluster: the clusters still open in order)
+      q = path.copy()
+      q[t] = (path[t] + 1) % opened
+      moved.append(q)
+  assert len(moved) > 25
+  res = R.path_score(load_weights(case['model']), [x], [np.array(moved)])
+  assert np.all(np.abs(res.score - ref[0]) > res.allowance(REF_INC_RTOL))
+
+
+def test_final_score_moved_past_the_allowance_fails():
+  """The final score of the longest traced decode (180 sub-steps) moved by 4 fp32 ulps beyond its allowance: still
+  inside a 1e-5 relative score check, outside the rescore.  (The allowance itself holds one ulp of the running score
+  per sub-step, about half the decode's length in ulps of the final score.)"""
+  case = next(c for c in GOLDEN_CASES if c['name'] == 'b10')
+  x, labels, ref = final_paths(case)
+  res = R.path_score(load_weights(case['model']), [x], [labels[:1]])
+  s = np.float32(ref[0])
+  assert res.share(ref[:1], REF_INC_RTOL)[0] <= 1
+  moved = np.float32(res.score[0] + np.sign(s - res.score[0]) * res.allowance(REF_INC_RTOL)[0])
+  for _ in range(4):
+    moved = np.nextafter(moved, np.float32(np.inf) if moved > res.score[0] else np.float32(-np.inf))
+  assert rel_err([moved], [s]) < 1e-5
+  assert res.share([float(moved)], REF_INC_RTOL)[0] > 1
+  assert res.allowance(REF_INC_RTOL)[0] < 200 * float(R.ulp32(s))
+
+
+def test_rescore_batches_and_shares_states():
+  """Paths rescored together, with duplicates, absent ranks and an empty utterance, score as they do alone."""
+  a = next(c for c in GOLDEN_CASES if c['name'] == 'b10')
+  b = next(c for c in GOLDEN_CASES if c['name'] == 'la3')
+  xa, la, _ = final_paths(a)
+  xb, lb, _ = final_paths(b)
+  w = load_weights('model_small.npz')
+  alone = [R.path_score(w, [xa], [la]), R.path_score(w, [xb], [lb])]
+  lb_absent = np.concatenate([lb, np.full((2, lb.shape[1]), -1)])
+  together = R.path_score(w, [xb, np.zeros((0, 64)), xa], [lb_absent, np.zeros((1, 0), np.int64), np.concatenate([la, la])],
+                          max_slots=20)
+  nb = len(lb)
+  for got, want in ((together.score[:nb], alone[1].score), (together.score[nb + 3:nb + 3 + len(la)], alone[0].score),
+                    (together.score[nb + 3 + len(la):], alone[0].score), (together.ulps[:nb], alone[1].ulps)):
+    assert np.array_equal(got, want)
+  assert np.isnan(together.score[nb:nb + 2]).all() and together.score[nb + 2] == 0
+
+
 def test_report_worst():
   """The replay's measured deviation from the reference's fp32 search (run with -s to see it)."""
   worst = {}
   for case in GOLDEN_CASES:
     run(case, worst=worst)
+    rescore(case, worst)
   print('\nreference vs float64 replay, worst: ' + ', '.join('%s %.2e' % kv for kv in sorted(worst.items())))
   assert worst['inc'] <= REF_INC_RTOL and worst['mean'] <= REF_STATE_TOL and worst['hidden'] <= REF_STATE_TOL
+  assert worst['path'] <= 1

@@ -13,7 +13,8 @@ another kernel fails.
 The matrix traces every lane of CTAs that hold several, both engines, the cluster and stationary-weights modes, depth
 1-4, zero-padded shapes, the look-ahead tree kernel in shared memory and spilled, speaker bounds, host staging chunks,
 edge inputs and 4200-step decodes (beyond the 4094 steps the default log tables hold).  What stays unchecked here:
-predict_device (it takes no taps) and utterances that are not traced in a call (their labels only)."""
+predict_device (it takes no taps), utterances that are not traced in a call (their labels only) and calls on every SM;
+tests/test_gpu_full_occupancy.py covers those."""
 
 import numpy as np
 import pytest
