@@ -523,7 +523,7 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
     }
     if (!pl->tcn)
       while (G > 1 && smem_bytes(m->H, m->D, pl->B, pl->Kcap, G) > 227u * 1024u) --G;
-    while (G > 1 && G * pl->B > 256) --G;  // phase P4 gives one consumer thread to every (lane, winner)
+    while (G > 1 && G * pl->B > 256) --G;  // at most 256 (lane, winner) pairs per CTA step
   }
   if (tree && o->engine == 2) return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: look_ahead must be 1");
   pl->G = G;

@@ -218,9 +218,9 @@ __host__ __device__ inline unsigned align_up(unsigned v, unsigned a) { return (v
 // lane scalars (ints) ------------------------------------------------------------------------
 enum { LS_U = 0, LS_N, LS_TN, LS_T, LS_NB, LS_GEN, LS_ACTIVE, LS_FAILED, LS_TRACED, LS_NFINITE, LS_KMAX,
        LS_NWIN, LS_ERR, LS_M, LS_COLBASE, LS_NE, LS_ROW0_LO, LS_ROW0_HI, LS_DBGROWS_LO, LS_DBGROWS_HI,
-       LS_FRESH, LS_KHI, LS_KLO, LS_COUNT = 24 };  // LS_KHI / LS_KLO: speaker bounds
+       LS_FRESH, LS_KHI, LS_KLO, LS_NLIST, LS_COUNT = 24 };  // LS_KHI / LS_KLO: speaker bounds; LS_NLIST: slots listed for scoring
 // CTA scalars
-enum { MI_PUBLISHED = 0, MI_DONE, MI_MTOT, MI_QNEXT, MI_NLIST, MI_MAXK };
+enum { MI_PUBLISHED = 0, MI_DONE, MI_MTOT, MI_QNEXT, MI_MAXK };
 
 template <int H, int D, int kCP = kCPBeam, bool XCL = false, int TCN = 0, bool STAT = false>
 __host__ __device__ inline SmemLayout make_layout(int B, int Kcap, int G) {
@@ -260,7 +260,7 @@ __host__ __device__ inline SmemLayout make_layout(int B, int Kcap, int G) {
   if constexpr (TCN > 0) o += 2 * TcCfg<H, D, TCN>::STAGES * 8;  // full, empty
   else o += 2 * kStages * 8;
   L.misc = o;      o += 64;
-  L.slist = o;     o += 4u * 64u * G;  // (lane, slot) work list of the per-slot scoring
+  L.slist = o;     o += 4u * 64u * G;  // per lane: 64-entry slot list of the per-slot scoring
   L.phase = o;     o += 128 + 32;  // thread 0's statistics: 10 phase cycle counters, phase mark, 5 counters, 4 tensor-core pass counters
   L.xch = o; L.xbar = o;
   if (XCL) {  // cluster K-split: two exchange buffers of kXchVals floats per consumer thread + 2 mbarriers
@@ -1151,64 +1151,88 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
       return;
     }
   };
-  // All consumer threads: start the cp.async of frame `t` of lane g into buffer (t & 1).
-  auto lane_prefetch = [&](int g, int t) {
+  // Lane teams.  The lanes are independent outside the weight pass, so the consumer warps split into G teams of
+  // TW = NW / G warps and team t runs every selection phase of lane t (P0-P4, the Gaussian terms of its slots, P6) on
+  // its own: a one-warp team synchronises with __syncwarp, a larger one on named barrier 2 + t (barrier 1 is the
+  // consumers').  Warps past G * TW own no lane.  The lanes meet only around the pass: after every team has published
+  // its lane's column count M, after the CTA column list is written, and at the pass's own barriers.  (team, ttid,
+  // twarp) are recomputed from `warp` and p.G where needed, so they hold no registers across the pass.
+  if (G > NW) __trap();  // the launcher runs at most one lane per consumer warp
+  auto team_of = [&]() { return warp / (NW / G); };
+  auto team_sync = [&]() {
+    const int TW = NW / G;
+    if (TW == 1) __syncwarp();
+    else named_bar_sync(2 + warp / TW, TW * 32);
+  };
+
+  // Team threads of lane g: start the cp.async of frame `t` of lane g into buffer (t & 1).  The team waits for its
+  // own copies (cp.async completion is per thread).
+  auto lane_prefetch = [&](int g, int t, int ttid, int TT) {
     volatile int* ls = LSp(g);
     const long long row0 = ((long long)ls[LS_ROW0_HI] << 32) | (unsigned)ls[LS_ROW0_LO];
     const long long r = row0 + (t % ls[LS_N]);
     float* xts = reinterpret_cast<float*>(lane_base(g) + L.l_xt) + (t & 1) * D;
-    for (int q = tid; q < D / 4; q += NT) cp_async16(xts + q * 4, p.x + (size_t)r * D + q * 4);
+    for (int q = ttid; q < D / 4; q += TT) cp_async16(xts + q * 4, p.x + (size_t)r * D + q * 4);
   };
 
-  // Gaussian terms per live slot.  Every consumer thread calls this (it synchronises on named barrier 1).
+  // Gaussian terms of lane g's slots, by the team of lane g (it synchronises on the team barrier).
   //   next == false (phase P1): slots of `used` without a bit in `scored`, against the current frame x_t;
   //   next == true  (tensor-core engine, while the first tiles of the weight pass are multiplied): every slot the
   //   caller marked in `scored` (the next generation's live slots, new slots excluded), against x_{t+1}.
   // weighted_mse_loss for one row (loss_func.py:33-41): sum_d fl(fl(diff^2) * w_d), divided by the count of rows
   // whose first squared difference is non-zero (0 -> inf / nan); stored per slot in pool_mse.
   float* pool_mse_cta = p.pool_mse + (size_t)blockIdx.x * G * p.P;
-  unsigned* slist = reinterpret_cast<unsigned*>(smem + L.slist);
-  const int slist_cap = 64 * G;
-  auto score_live_slots = [&](bool next) {
+  constexpr int kSlotList = 64;  // slots per listing round and lane
+  auto score_lane_slots = [&](int g, bool next, int ttid, int twarp, int TW) {
+    unsigned* used = reinterpret_cast<unsigned*>(lane_base(g) + L.l_used);
+    unsigned* scored = reinterpret_cast<unsigned*>(lane_base(g) + L.l_scored);
+    unsigned* slist = reinterpret_cast<unsigned*>(smem + L.slist) + kSlotList * g;
+    volatile int* ls = LSp(g);
+    const float* xs = reinterpret_cast<const float*>(lane_base(g) + L.l_xt) + ((ls[LS_T] + (next ? 1 : 0)) & 1) * D;
+    const float* mu_g = pool_mean_cta + g * pool_m_stride;
+    float* mse_g = pool_mse_cta + (size_t)g * p.P;
     for (;;) {
-      if (tid == 0) misc[MI_NLIST] = 0;
-      named_bar_sync(1, NT);
-      for (int f = tid; f < G * (int)PW; f += NT) {  // one thread per bitmap word: append its slots to the list
-        const int g = f / (int)PW, w = f % (int)PW;
-        unsigned* used = reinterpret_cast<unsigned*>(lane_base(g) + L.l_used);
-        unsigned* scored = reinterpret_cast<unsigned*>(lane_base(g) + L.l_scored);
-        unsigned bits = next ? (scored[w] & ~used[w]) : (used[w] & ~scored[w]);  // (next: `used` holds the slots already listed)
-        if (!LSp(g)[LS_ACTIVE]) bits = 0;
-        const int n = __popc(bits);
-        if (n) {
-          int pos = atomicAdd((int*)&misc[MI_NLIST], n);
+      if (twarp == 0) {  // the team's first warp lists the slots: a prefix over the bitmap words, 32 words per round
+        int ntot = 0;
+        for (int w0 = 0; w0 < (int)PW; w0 += 32) {
+          const int w = w0 + lane;
+          unsigned bits = 0;
+          if (w < (int)PW) bits = next ? (scored[w] & ~used[w]) : (used[w] & ~scored[w]);  // (next: `used` = listed)
+          const int n = __popc(bits);
+          int incl = n;
+#pragma unroll
+          for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += v;
+          }
+          int pos = ntot + incl - n;
           unsigned done = 0;
-          while (bits && pos < slist_cap) {
+          while (bits && pos < kSlotList) {
             const int bit = __ffs(bits) - 1;
             bits &= bits - 1;
             done |= 1u << bit;
-            slist[pos++] = ((unsigned)g << 16) | (unsigned)(w * 32 + bit);
+            slist[pos++] = (unsigned)(w * 32 + bit);
           }
-          if (next) used[w] |= done; else scored[w] |= done;
+          if (done) { if (next) used[w] |= done; else scored[w] |= done; }
+          ntot += __shfl_sync(0xffffffffu, incl, 31);
         }
+        if (lane == 0) ls[LS_NLIST] = ntot;
       }
-      named_bar_sync(1, NT);
-      const int ntot = misc[MI_NLIST], nlist = min(ntot, slist_cap);
+      team_sync();
+      const int ntot = ls[LS_NLIST], nlist = min(ntot, kSlotList);
       // one warp per slot; each warp takes kBatch slots per trip and issues all their slot-pool loads (L2) before
       // reducing any of them, so the L2 round trips overlap instead of serialising
       constexpr int kBatch = 4;
-      for (int f0 = warp * kBatch; f0 < nlist; f0 += NW * kBatch) {
-        int cg[kBatch];
-        unsigned cslot[kBatch];
+      for (int f0 = twarp * kBatch; f0 < nlist; f0 += TW * kBatch) {
+        int cslot[kBatch];
         float4 m4[kBatch][(D + 127) / 128];
 #pragma unroll
         for (int q = 0; q < kBatch; ++q) {
           const int f = f0 + q;
-          cg[q] = -1; cslot[q] = 0;
+          cslot[q] = -1;
           if (f < nlist) {
-            const unsigned ent = slist[f];
-            cg[q] = (int)(ent >> 16); cslot[q] = ent & 0xffffu;
-            const float* mu = pool_mean_cta + cg[q] * pool_m_stride + (size_t)cslot[q] * D;
+            cslot[q] = (int)slist[f];
+            const float* mu = mu_g + (size_t)cslot[q] * D;
 #pragma unroll
             for (int i = 0; i < (D + 127) / 128; ++i)
               if (lane * 4 + i * 128 < D)
@@ -1220,12 +1244,10 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
 #pragma unroll
         for (int q = 0; q < kBatch; ++q) {
           acc[q] = 0.f; d0sq[q] = 1.f;
-          const int g = cg[q] < 0 ? 0 : cg[q];
-          const float* xs = reinterpret_cast<const float*>(lane_base(g) + L.l_xt) + ((LSp(g)[LS_T] + (next ? 1 : 0)) & 1) * D;
 #pragma unroll
           for (int i = 0; i < (D + 127) / 128; ++i) {
             const int d = lane * 4 + i * 128;
-            if (d < D && cg[q] >= 0) {
+            if (d < D && cslot[q] >= 0) {
               const float4 x4 = *reinterpret_cast<const float4*>(xs + d);
               const float4 w4 = *reinterpret_cast<const float4*>(wv + d);
               const float e0 = __fsub_rn(m4[q][i].x, x4.x), e1 = __fsub_rn(m4[q][i].y, x4.y);
@@ -1246,344 +1268,310 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
         }
         // lane q finishes slot q (the tails run side by side)
         float my_acc = acc[0], my_d0 = __shfl_sync(0xffffffffu, d0sq[0], 0);
-        int my_g = cg[0];
-        unsigned my_slot = cslot[0];
+        int my_slot = cslot[0];
 #pragma unroll
         for (int q = 1; q < kBatch; ++q) {
           const float dq = __shfl_sync(0xffffffffu, d0sq[q], 0);
-          if (lane == q) { my_acc = acc[q]; my_d0 = dq; my_g = cg[q]; my_slot = cslot[q]; }
+          if (lane == q) { my_acc = acc[q]; my_d0 = dq; my_slot = cslot[q]; }
         }
-        if (lane < kBatch && my_g >= 0) {
+        if (lane < kBatch && my_slot >= 0) {
           if (my_d0 == 0.f) my_acc = __fdiv_rn(my_acc, 0.f);  // zero "non-zero rows" (loss_func.py:36)
-          pool_mse_cta[(size_t)my_g * p.P + my_slot] = my_acc;
+          mse_g[my_slot] = my_acc;
         }
       }
-      named_bar_sync(1, NT);  // the terms are visible to every consumer thread (CTA-scope ordering of global memory)
-      if (ntot <= slist_cap) break;  // (more slots than the list holds: another round over the unlisted ones)
+      team_sync();  // the terms are visible to the whole team (ordering of global memory among the team's threads)
+      if (ntot <= kSlotList) break;  // (more slots than the list holds: another round over the unlisted ones)
     }
   };
 
-  if (tid < G) lane_fetch(tid);
-  named_bar_sync(1, NT);
-  for (int g = 0; g < G; ++g)
-    if (LSp(g)[LS_ACTIVE]) lane_prefetch(g, 0);
-  cp_async_commit();
+  if (team_of() < G) {
+    const int g = team_of(), TT = (NW / G) * 32, ttid = tid - g * TT;
+    if (ttid == 0) lane_fetch(g);
+    team_sync();
+    if (LSp(g)[LS_ACTIVE]) lane_prefetch(g, 0, ttid, TT);
+    cp_async_commit();
+  }
+  named_bar_sync(1, NT);  // slot 0 of every lane's pool and the MSE weights are written
 
   for (;;) {
-    int nact = 0;
-    for (int g = 0; g < G; ++g) nact += LSp(g)[LS_ACTIVE];
-    if (nact == 0) break;
-
-    // ---- P0: publish this step's weight pass; per-lane candidate offsets; land x_t / gi_t
-    if (tid == 0 && !TC) {
-      __threadfence_block();
-      misc[MI_PUBLISHED] = misc[MI_PUBLISHED] + 1;
-    }
-    if (tid < G) {
-      const int g = tid;
+    if (team_of() < G) {
+      const int g = team_of(), TW = NW / G, TT = TW * 32, ttid = tid - g * TT, twarp = warp - g * TW;
       volatile int* ls = LSp(g);
-      ls[LS_M] = 0; ls[LS_NWIN] = 0; ls[LS_NE] = 0;
-      if (ls[LS_ACTIVE]) {
-        const int* mK = reinterpret_cast<const int*>(lane_base(g) + L.l_meta) + ls[LS_GEN] * 4 * B;
-        int* candoff = reinterpret_cast<int*>(lane_base(g) + L.l_candoff);
-        int off = 0, kmax = 0;
-        const int nb = ls[LS_NB], khi = ls[LS_KHI];
-        // a hypothesis at max_speakers clusters has no new-cluster candidate (its score would be +inf); the flat
-        // tie-break index below keeps the unbounded (kmax + 1) stride
-        for (int b = 0; b < nb; ++b) { candoff[b] = off; off += mK[b] + (mK[b] < khi ? 1 : 0); kmax = max(kmax, mK[b]); }
-        candoff[nb] = off;
-        ls[LS_NFINITE] = 0; ls[LS_KMAX] = kmax; ls[LS_NE] = off;
+      unsigned char* lb = lane_base(g);
+      const bool active = ls[LS_ACTIVE] != 0;
+      const int gen = ls[LS_GEN], t = ls[LS_T];
+      const int* mK = reinterpret_cast<const int*>(lb + L.l_meta) + gen * 4 * B;
+      const int* mLast = mK + B; const int* mTot = mK + 2 * B;
+      const float* mNl = reinterpret_cast<const float*>(mK + 3 * B);
+      int* candoff = reinterpret_cast<int*>(lb + L.l_candoff);
+      const TabEntry* tab = reinterpret_cast<const TabEntry*>(lb + L.l_tabs) + (size_t)gen * B * Kcap;
+      unsigned* used = reinterpret_cast<unsigned*>(lb + L.l_used);
+      unsigned* scored = reinterpret_cast<unsigned*>(lb + L.l_scored);
+      int* wins = reinterpret_cast<int*>(lb + L.l_wins);
+      int* wcol = reinterpret_cast<int*>(lb + L.l_wcol);
+      int* lcolsrc = reinterpret_cast<int*>(lb + L.l_lcol);
+      int* lcolnew = lcolsrc + B;
+
+      // ---- P0: candidate offsets of the lane; land x_t
+      if (ttid == 0) {
+        ls[LS_M] = 0; ls[LS_NWIN] = 0; ls[LS_NE] = 0;
+        if (active) {
+          int off = 0, kmax = 0;
+          const int nb = ls[LS_NB], khi = ls[LS_KHI];
+          // a hypothesis at max_speakers clusters has no new-cluster candidate (its score would be +inf); the flat
+          // tie-break index below keeps the unbounded (kmax + 1) stride
+          for (int b = 0; b < nb; ++b) { candoff[b] = off; off += mK[b] + (mK[b] < khi ? 1 : 0); kmax = max(kmax, mK[b]); }
+          candoff[nb] = off;
+          ls[LS_NFINITE] = 0; ls[LS_KMAX] = kmax; ls[LS_NE] = off;
+        }
       }
-    }
-    for (int g = 0; g < G; ++g) {
-      unsigned* used = reinterpret_cast<unsigned*>(lane_base(g) + L.l_used);
-      unsigned* scored = reinterpret_cast<unsigned*>(lane_base(g) + L.l_scored);
-      for (unsigned w = tid; w < PW; w += NT) {
+      for (unsigned w = ttid; w < PW; w += TT) {
         used[w] = (w == 0) ? 1u : 0u;  // slot 0 = INIT, always live
         if (!TC) scored[w] = 0;        // (tensor-core engine: set by the pre-scoring of the previous step's pass)
       }
-    }
-    cp_async_wait_all();
-    named_bar_sync(1, NT);
-    UIS_PHASE(6);
-    for (int g = 0; g < G; ++g) {  // prefetch the next frame of every running lane
-      volatile int* ls = LSp(g);
-      if (ls[LS_ACTIVE] && ls[LS_T] + 1 < ls[LS_TN]) lane_prefetch(g, ls[LS_T] + 1);
-    }
-    cp_async_commit();
+      cp_async_wait_all();
+      team_sync();
+      UIS_PHASE(6);
+      if (active && t + 1 < ls[LS_TN]) lane_prefetch(g, t + 1, ttid, TT);  // the lane's next frame
+      cp_async_commit();
 
-    // ---- P1: score every candidate (b, c <= K_b) of every lane  (uisrnn.py:409-420 existing cluster, :434-446 new
-    //          cluster).  The Gaussian term depends only on (slot, x_t) -- hypotheses share most of their clusters'
-    //          states -- so it is evaluated once per LIVE SLOT (one warp each), not once per candidate; slots whose
-    //          term against x_t was already computed during the previous weight pass (tensor-core engine: the
-    //          consumer warps idle while the first tiles are multiplied) are skipped.
-    {
-      int ne_g[kMaxLanes], ne_tot = 0;
-      for (int g = 0; g < G; ++g) { ne_g[g] = LSp(g)[LS_NE]; ne_tot += ne_g[g]; }
-      // P1a: one thread per candidate resolves (hypothesis, cluster) -> slot, marks the slot
-      // live, and evaluates the transition / ddCRP term in fp64 from the host-built log tables
-      // (the np.log values of uisrnn.py:415-420, 444-446).  Parked in keys[] / svals[].
-      for (int f = tid; f < ne_tot; f += NT) {
-        int g = 0, e = f;
-        while (e >= ne_g[g]) { e -= ne_g[g]; ++g; }
-        volatile int* ls = LSp(g);
-        const int gen = ls[LS_GEN];
-        const int* mK = reinterpret_cast<const int*>(lane_base(g) + L.l_meta) + gen * 4 * B;
-        const int* mLast = mK + B; const int* mTot = mK + 2 * B;
-        const int* candoff = reinterpret_cast<const int*>(lane_base(g) + L.l_candoff);
-        const TabEntry* tab = reinterpret_cast<const TabEntry*>(lane_base(g) + L.l_tabs) + (size_t)gen * B * Kcap;
+      if (active) {
+        // ---- P1: score every candidate (b, c <= K_b) of the lane  (uisrnn.py:409-420 existing cluster, :434-446 new
+        //          cluster).  The Gaussian term depends only on (slot, x_t) -- hypotheses share most of their
+        //          clusters' states -- so it is evaluated once per LIVE SLOT (one warp each), not once per candidate;
+        //          slots whose term against x_t was already computed during the previous weight pass (tensor-core
+        //          engine: the consumer warps idle while the first tiles are multiplied) are skipped.
+        const int ne = ls[LS_NE], kmax = ls[LS_KMAX];
+        double* pens = reinterpret_cast<double*>(lb + L.l_keys);
+        unsigned long long* keys = reinterpret_cast<unsigned long long*>(lb + L.l_keys);
+        unsigned* svals = reinterpret_cast<unsigned*>(lb + L.l_svals);
+        // P1a: one thread per candidate resolves (hypothesis, cluster) -> slot, marks the slot live, and evaluates the
+        // transition / ddCRP term in fp64 from the host-built log tables (the np.log values of uisrnn.py:415-420,
+        // 444-446).  Parked in keys[] / svals[].  A thread's candidates grow, so its hypothesis index only moves on.
         int b = 0;
-        while (candoff[b + 1] <= e) ++b;
-        const int c = e - candoff[b];
-        int slot = kInitSlot;
-        double pen;
-        if (c < mK[b]) {
-          const TabEntry en = tab[(size_t)b * Kcap + c];
-          slot = en.slot;
-          atomicOr(reinterpret_cast<unsigned*>(lane_base(g) + L.l_used) + (slot >> 5), 1u << (slot & 31));
-          pen = (c == mLast[b]) ? p.log_1mp0 : (p.log_p0 + __ldg(p.logn + en.blocks)) - __ldg(p.logtot + mTot[b]);
-        } else {
-          pen = (p.log_p0 + p.log_alpha) - __ldg(p.logtot + mTot[b]);
-        }
-        reinterpret_cast<double*>(lane_base(g) + L.l_keys)[e] = pen;
-        // slot (16 bits) | hypothesis (5 bits, or 7 when beam_size > 32: the host then caps kcap at 511) | cluster
-        reinterpret_cast<unsigned*>(lane_base(g) + L.l_svals)[e] = (unsigned)slot | ((unsigned)b << 16) | ((unsigned)c << (16 + bbits));
-      }
-      named_bar_sync(1, NT);
-      // P1s: the live slots that still lack their term against x_t
-      score_live_slots(/*against the next frame=*/false);
-      // P1c: one thread per candidate: loss = fl32(f64(mse) - log terms); neg_likelihood accumulates in fp32
-      //      (uisrnn.py:452); ranking key
-      for (int f = tid; f < ne_tot; f += NT) {
-        int g = 0, e = f;
-        while (e >= ne_g[g]) { e -= ne_g[g]; ++g; }
-        volatile int* ls = LSp(g);
-        const unsigned info = reinterpret_cast<const unsigned*>(lane_base(g) + L.l_svals)[e];
-        const int b = (int)((info >> 16) & ((1u << bbits) - 1u)), c = (int)(info >> (16 + bbits));
-        const float mse = pool_mse_cta[(size_t)g * p.P + (info & 0xffffu)];
-        const float* mNl = reinterpret_cast<const float*>(lane_base(g) + L.l_meta) + ls[LS_GEN] * 4 * B + 3 * B;
-        const double pen = reinterpret_cast<const double*>(lane_base(g) + L.l_keys)[e];
-        const float loss = __double2float_rn((double)mse - pen);
-        const float S = __fadd_rn(mNl[b], loss);
-        reinterpret_cast<float*>(lane_base(g) + L.l_svals)[e] = S;
-        const unsigned flat = (unsigned)(b * (ls[LS_KMAX] + 1) + c);
-        reinterpret_cast<unsigned long long*>(lane_base(g) + L.l_keys)[e] =
-            ((unsigned long long)float_order_key(S) << 32) | flat;
-        if (S < INF) atomicAdd((int*)&ls[LS_NFINITE], 1);
-      }
-      named_bar_sync(1, NT);
-      UIS_PHASE(7);
-
-      // ---- P2: rank by counting; the best min(#finite, B) become the new hypotheses (:546-552)
-      for (int f = tid; f < ne_tot; f += NT) {
-        int g = 0, e = f;
-        while (e >= ne_g[g]) { e -= ne_g[g]; ++g; }
-        volatile int* ls = LSp(g);
-        const int nwin = min((int)ls[LS_NFINITE], B);
-        const unsigned long long* keys = reinterpret_cast<const unsigned long long*>(lane_base(g) + L.l_keys);
-        const unsigned long long k = keys[e];
-        int rank = 0;
-        for (int q = 0; q < ne_g[g]; ++q) rank += (keys[q] < k) ? 1 : 0;
-        if (rank < nwin) {
-          const int* candoff = reinterpret_cast<const int*>(lane_base(g) + L.l_candoff);
-          int b = 0;
+        for (int e = ttid; e < ne; e += TT) {
           while (candoff[b + 1] <= e) ++b;
-          int* wins = reinterpret_cast<int*>(lane_base(g) + L.l_wins);
-          wins[rank] = b;
-          wins[B + rank] = e - candoff[b];
-          reinterpret_cast<float*>(wins)[2 * B + rank] = reinterpret_cast<const float*>(lane_base(g) + L.l_svals)[e];
+          const int c = e - candoff[b];
+          int slot = kInitSlot;
+          double pen;
+          if (c < mK[b]) {
+            const TabEntry en = tab[(size_t)b * Kcap + c];
+            slot = en.slot;
+            atomicOr(used + (slot >> 5), 1u << (slot & 31));
+            pen = (c == mLast[b]) ? p.log_1mp0 : (p.log_p0 + __ldg(p.logn + en.blocks)) - __ldg(p.logtot + mTot[b]);
+          } else {
+            pen = (p.log_p0 + p.log_alpha) - __ldg(p.logtot + mTot[b]);
+          }
+          pens[e] = pen;
+          // slot (16 bits) | hypothesis (5 bits, or 7 when beam_size > 32: the host then caps kcap at 511) | cluster
+          svals[e] = (unsigned)slot | ((unsigned)b << 16) | ((unsigned)c << (16 + bbits));
         }
-        if (e == 0) ls[LS_NWIN] = nwin;
-      }
-      named_bar_sync(1, NT);
-      UIS_PHASE(8);
-    }
+        team_sync();
+        // P1s: the live slots that still lack their term against x_t
+        score_lane_slots(g, /*against the next frame=*/false, ttid, twarp, TW);
+        // P1c: one thread per candidate: loss = fl32(f64(mse) - log terms); neg_likelihood accumulates in fp32
+        //      (uisrnn.py:452); ranking key; the finite scores are counted per warp
+        const float* mse_g = pool_mse_cta + (size_t)g * p.P;
+        int nfin = 0;
+        for (int e0 = 0; e0 < ne; e0 += TT) {
+          const int e = e0 + ttid;
+          bool finite = false;
+          if (e < ne) {
+            const unsigned info = svals[e];
+            const int bb = (int)((info >> 16) & ((1u << bbits) - 1u)), c = (int)(info >> (16 + bbits));
+            const float mse = mse_g[info & 0xffffu];
+            const float loss = __double2float_rn((double)mse - pens[e]);
+            const float S = __fadd_rn(mNl[bb], loss);
+            reinterpret_cast<float*>(svals)[e] = S;
+            const unsigned flat = (unsigned)(bb * (kmax + 1) + c);
+            keys[e] = ((unsigned long long)float_order_key(S) << 32) | flat;
+            finite = S < INF;
+          }
+          nfin += __popc(__ballot_sync(0xffffffffu, finite));
+        }
+        if (lane == 0 && nfin) atomicAdd((int*)&ls[LS_NFINITE], nfin);
+        team_sync();
+        UIS_PHASE(7);
 
-    // ---- P3: warp g assigns lane g's GRU columns (distinct source slots) and allocates new
-    //          slots; the remaining warps copy the parents' tables into the next generation
-    if (warp < G) {
-      const int g = warp;
-      volatile int* ls = LSp(g);
-      const int nwin = ls[LS_NWIN];
-      if (ls[LS_ACTIVE] && nwin > 0) {
-        const int gen = ls[LS_GEN];
-        const int* mK = reinterpret_cast<const int*>(lane_base(g) + L.l_meta) + gen * 4 * B;
-        const TabEntry* tab = reinterpret_cast<const TabEntry*>(lane_base(g) + L.l_tabs) + (size_t)gen * B * Kcap;
-        const int* wins = reinterpret_cast<const int*>(lane_base(g) + L.l_wins);
-        int* wcol = reinterpret_cast<int*>(lane_base(g) + L.l_wcol);
-        int* lcolsrc = reinterpret_cast<int*>(lane_base(g) + L.l_lcol);
-        int* lcolnew = lcolsrc + B;
-        const unsigned* used = reinterpret_cast<const unsigned*>(lane_base(g) + L.l_used);
-        int M = 0;
-        if (nwin <= 32) {  // one winner per lane (beam_size <= 32, or fewer finite candidates)
-          const int r = lane;
-          int src = -1;
-          if (r < nwin) {
-            const int b = wins[r], c = wins[B + r];
-            src = (c < mK[b]) ? tab[(size_t)b * Kcap + c].slot : kInitSlot;
+        // ---- P2: rank by counting; the best min(#finite, B) become the new hypotheses (:546-552)
+        const int nwin = min((int)ls[LS_NFINITE], B);
+        b = 0;
+        for (int e = ttid; e < ne; e += TT) {
+          const unsigned long long k = keys[e];
+          int rank = 0;
+          for (int q = 0; q < ne; ++q) rank += (keys[q] < k) ? 1 : 0;
+          if (rank < nwin) {
+            while (candoff[b + 1] <= e) ++b;
+            wins[rank] = b;
+            wins[B + rank] = e - candoff[b];
+            reinterpret_cast<float*>(wins)[2 * B + rank] = reinterpret_cast<const float*>(svals)[e];
           }
-          int first = r;
-          for (int q = 0; q < nwin; ++q) {
-            const int sq = __shfl_sync(0xffffffffu, src, q);
-            if (q < first && sq == src) first = q;
-          }
-          const bool isfirst = (r < nwin) && (first == r);
-          const unsigned fm = __ballot_sync(0xffffffffu, isfirst);
-          const int mycol = __popc(fm & ((1u << lane) - 1));
-          M = __popc(fm);
-          const int c_of_first = __shfl_sync(0xffffffffu, mycol, first);
-          if (r < nwin) wcol[r] = c_of_first;
-          if (isfirst) lcolsrc[mycol] = src;
-        } else {
-          // beam_size > 32: the winners are walked in chunks of 32; their source slots are parked in lcolnew (rewritten
-          // by the slot allocation below) so that every winner can look for an earlier winner with the same source
-          for (int r = lane; r < nwin; r += 32) {
-            const int b = wins[r], c = wins[B + r];
-            lcolnew[r] = (c < mK[b]) ? tab[(size_t)b * Kcap + c].slot : kInitSlot;
-          }
-          __syncwarp();
-          for (int r0 = 0; r0 < nwin; r0 += 32) {  // columns are numbered in winner order, as in the one-chunk case
-            const int r = r0 + lane;
-            int first = r, src = -1;
-            if (r < nwin) {
-              src = lcolnew[r];
-              for (int q = 0; q < r; ++q)
-                if (lcolnew[q] == src) { first = q; break; }
-            }
-            const bool isfirst = (r < nwin) && (first == r);
-            const unsigned fm = __ballot_sync(0xffffffffu, isfirst);
-            if (isfirst) {
-              const int mycol = M + __popc(fm & ((1u << lane) - 1));
-              wcol[r] = mycol;
-              lcolsrc[mycol] = src;
-            }
-            M += __popc(fm);
-            __syncwarp();
-            if (r < nwin && !isfirst) wcol[r] = wcol[first];  // `first` is an earlier winner: its column is already there
-            __syncwarp();
-          }
-          __syncwarp();
         }
-        // allocate M free slots from the bitmap (any free slot will do)
-        int cnt = 0;
-        for (unsigned w = lane; w < PW; w += 32) {
-          unsigned fr = ~used[w];
-          if (w == PW - 1 && (p.P & 31)) fr &= (1u << (p.P & 31)) - 1;
-          cnt += __popc(fr);
-        }
-        int incl = cnt;
+        if (ttid == 0) ls[LS_NWIN] = nwin;
+        team_sync();
+        UIS_PHASE(8);
+
+        // ---- P3: the team's first warp assigns the lane's GRU columns (distinct source slots) and allocates new
+        //          slots; every warp of the team copies its share of the parents' tables into the next generation
+        if (nwin > 0) {
+          if (twarp == 0) {
+            int M = 0;
+            if (nwin <= 32) {  // one winner per lane (beam_size <= 32, or fewer finite candidates)
+              const int r = lane;
+              int src = -1;
+              if (r < nwin) {
+                const int wb = wins[r], c = wins[B + r];
+                src = (c < mK[wb]) ? tab[(size_t)wb * Kcap + c].slot : kInitSlot;
+              }
+              int first = r;
+              for (int q = 0; q < nwin; ++q) {
+                const int sq_ = __shfl_sync(0xffffffffu, src, q);
+                if (q < first && sq_ == src) first = q;
+              }
+              const bool isfirst = (r < nwin) && (first == r);
+              const unsigned fm = __ballot_sync(0xffffffffu, isfirst);
+              const int mycol = __popc(fm & ((1u << lane) - 1));
+              M = __popc(fm);
+              const int c_of_first = __shfl_sync(0xffffffffu, mycol, first);
+              if (r < nwin) wcol[r] = c_of_first;
+              if (isfirst) lcolsrc[mycol] = src;
+            } else {
+              // beam_size > 32: the winners are walked in chunks of 32; their source slots are parked in lcolnew
+              // (rewritten by the slot allocation below) so that every winner can look for an earlier winner with the
+              // same source
+              for (int r = lane; r < nwin; r += 32) {
+                const int wb = wins[r], c = wins[B + r];
+                lcolnew[r] = (c < mK[wb]) ? tab[(size_t)wb * Kcap + c].slot : kInitSlot;
+              }
+              __syncwarp();
+              for (int r0 = 0; r0 < nwin; r0 += 32) {  // columns are numbered in winner order, as in the one-chunk case
+                const int r = r0 + lane;
+                int first = r, src = -1;
+                if (r < nwin) {
+                  src = lcolnew[r];
+                  for (int q = 0; q < r; ++q)
+                    if (lcolnew[q] == src) { first = q; break; }
+                }
+                const bool isfirst = (r < nwin) && (first == r);
+                const unsigned fm = __ballot_sync(0xffffffffu, isfirst);
+                if (isfirst) {
+                  const int mycol = M + __popc(fm & ((1u << lane) - 1));
+                  wcol[r] = mycol;
+                  lcolsrc[mycol] = src;
+                }
+                M += __popc(fm);
+                __syncwarp();
+                if (r < nwin && !isfirst) wcol[r] = wcol[first];  // `first` is an earlier winner: its column is already there
+                __syncwarp();
+              }
+              __syncwarp();
+            }
+            // allocate M free slots from the bitmap (any free slot will do)
+            int cnt = 0;
+            for (unsigned w = lane; w < PW; w += 32) {
+              unsigned fr = ~used[w];
+              if (w == PW - 1 && (p.P & 31)) fr &= (1u << (p.P & 31)) - 1;
+              cnt += __popc(fr);
+            }
+            int incl = cnt;
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const int v = __shfl_up_sync(0xffffffffu, incl, o);
-          if (lane >= o) incl += v;
-        }
-        int idx = incl - cnt;
-        for (unsigned w = lane; w < PW && idx < M; w += 32) {
-          unsigned fr = ~used[w];
-          if (w == PW - 1 && (p.P & 31)) fr &= (1u << (p.P & 31)) - 1;
-          while (fr && idx < M) {
-            const int bit = __ffs(fr) - 1;
-            fr &= fr - 1;
-            lcolnew[idx++] = (int)(w * 32 + bit);
+            for (int o = 1; o < 32; o <<= 1) {
+              const int v = __shfl_up_sync(0xffffffffu, incl, o);
+              if (lane >= o) incl += v;
+            }
+            int idx = incl - cnt;
+            for (unsigned w = lane; w < PW && idx < M; w += 32) {
+              unsigned fr = ~used[w];
+              if (w == PW - 1 && (p.P & 31)) fr &= (1u << (p.P & 31)) - 1;
+              while (fr && idx < M) {
+                const int bit = __ffs(fr) - 1;
+                fr &= fr - 1;
+                lcolnew[idx++] = (int)(w * 32 + bit);
+              }
+            }
+            if (lane == 0) ls[LS_M] = M;
           }
-        }
-        if (lane == 0) ls[LS_M] = M;
-      }
-    }
-    if (TC || warp >= G) {
-      // parents' tables -> next generation: the warps without a lane of their own (FFMA kernels: G <= 4 of 8 warps);
-      // with up to 8 lanes per CTA (tensor-core pass) every warp takes its share after its lane job
-      const int cw = TC ? NW : NW - G, cme = TC ? warp : warp - G;
-      int done = 0;
-      for (int g = 0; g < G; ++g) {
-        volatile int* ls = LSp(g);
-        const int nwin = ls[LS_NWIN];
-        if (!ls[LS_ACTIVE]) continue;
-        const int gen = ls[LS_GEN];
-        const int* mK = reinterpret_cast<const int*>(lane_base(g) + L.l_meta) + gen * 4 * B;
-        const TabEntry* tab = reinterpret_cast<const TabEntry*>(lane_base(g) + L.l_tabs) + (size_t)gen * B * Kcap;
-        TabEntry* ntab = reinterpret_cast<TabEntry*>(lane_base(g) + L.l_tabs) + (size_t)(gen ^ 1) * B * Kcap;
-        const int* wins = reinterpret_cast<const int*>(lane_base(g) + L.l_wins);
-        for (int r = 0; r < nwin; ++r, ++done) {
-          if (done % cw != cme) continue;
-          const int b = wins[r];
-          const int Kb = mK[b];
-          for (int c = lane; c < Kb; c += 32) ntab[(size_t)r * Kcap + c] = tab[(size_t)b * Kcap + c];
-        }
-      }
-    }
-    named_bar_sync(1, NT);
-    UIS_PHASE(9);
+          // parents' tables -> next generation: winner r goes to warp r % TW of the team
+          TabEntry* ntab = reinterpret_cast<TabEntry*>(lb + L.l_tabs) + (size_t)(gen ^ 1) * B * Kcap;
+          for (int r = twarp; r < nwin; r += TW) {
+            const int wb = wins[r];
+            const int Kb = mK[wb];
+            for (int c = lane; c < Kb; c += 32) ntab[(size_t)r * Kcap + c] = tab[(size_t)wb * Kcap + c];
+          }
+          team_sync();
+          UIS_PHASE(9);
 
-    // ---- P4: patch the one changed table entry per child; back-pointers; hypothesis meta;
-    //          build the CTA-wide column list
-    int colbase[kMaxLanes], Mtot = 0;
-    for (int g = 0; g < G; ++g) { colbase[g] = Mtot; Mtot += LSp(g)[LS_M]; }
-    if (tid < G * B) {
-      const int g = tid / B, r = tid % B;
-      volatile int* ls = LSp(g);
-      const int nwin = ls[LS_NWIN];
-      if (ls[LS_ACTIVE] && r < nwin) {
-        const int gen = ls[LS_GEN];
-        int* meta = reinterpret_cast<int*>(lane_base(g) + L.l_meta);
-        const int* mK = meta + gen * 4 * B; const int* mLast = mK + B; const int* mTot = mK + 2 * B;
-        int* nK = meta + (gen ^ 1) * 4 * B; int* nLast = nK + B; int* nTot = nK + 2 * B;
-        float* nNl = reinterpret_cast<float*>(nK + 3 * B);
-        const TabEntry* tab = reinterpret_cast<const TabEntry*>(lane_base(g) + L.l_tabs) + (size_t)gen * B * Kcap;
-        TabEntry* ntab = reinterpret_cast<TabEntry*>(lane_base(g) + L.l_tabs) + (size_t)(gen ^ 1) * B * Kcap;
-        const int* wins = reinterpret_cast<const int*>(lane_base(g) + L.l_wins);
-        const int* wcol = reinterpret_cast<const int*>(lane_base(g) + L.l_wcol);
-        const int* lcolsrc = reinterpret_cast<const int*>(lane_base(g) + L.l_lcol);
-        const int* lcolnew = lcolsrc + B;
-        const int b = wins[r], c = wins[B + r];
-        const float S = reinterpret_cast<const float*>(wins)[2 * B + r];
-        const int Kb = mK[b];
-        const bool isnew = (c == Kb);
-        const int t = ls[LS_T], TN = ls[LS_TN], N = ls[LS_N];
-        if (isnew && Kb >= Kcap) {
-          ls[LS_ERR] = 1;  // more clusters than the device tables hold
-        } else {
-          const TabEntry old = isnew ? TabEntry{kInitSlot, 0, 0, 0} : tab[(size_t)b * Kcap + c];
-          const bool moved = isnew || (c != mLast[b]);
-          const int lc = wcol[r];
-          TabEntry ne;
-          ne.slot = lcolnew[lc];
-          ne.blocks = old.blocks + (moved ? 1 : 0);  // uisrnn.py:431-432; a new cluster starts at 1 (:76)
-          ne.visits = old.visits + 1;
-          ne.pad = 0;
-          ntab[(size_t)r * Kcap + c] = ne;
-          nK[r] = Kb + (isnew ? 1 : 0);
-          atomicMax((int*)&misc[MI_MAXK], Kb + (isnew ? 1 : 0));
-          nLast[r] = c;
-          nTot[r] = mTot[b] + (moved ? 1 : 0);
-          nNl[r] = S;
-          const int m = colbase[g] + lc;
-          if (lcolsrc[lc] == old.slot) colvis[m] = old.visits;  // same slot => same visit count
-        }
-        if (t >= TN - N) bp_cta[((size_t)g * p.maxN + (t - (TN - N))) * B + r] = ((unsigned)b << 16) | (unsigned)c;
-        if (ls[LS_TRACED]) {
-          const long long rows = ((long long)ls[LS_DBGROWS_HI] << 32) | (unsigned)ls[LS_DBGROWS_LO];
-          if (p.dbg_win && rows + r < p.trace_capacity) {
-            p.dbg_win[(rows + r) * 2 + 0] = b;
-            p.dbg_win[(rows + r) * 2 + 1] = c;
-            p.dbg_score[rows + r] = S;
+          // ---- P4: patch the one changed table entry per child; back-pointers; hypothesis meta.  The visit count of
+          //          each lane-local column goes to lvis (the ranking keys are dead from here on) until the CTA
+          //          column list is built.
+          int* meta = reinterpret_cast<int*>(lb + L.l_meta);
+          int* nK = meta + (gen ^ 1) * 4 * B; int* nLast = nK + B; int* nTot = nK + 2 * B;
+          float* nNl = reinterpret_cast<float*>(nK + 3 * B);
+          int* lvis = reinterpret_cast<int*>(lb + L.l_keys);
+          const int TN = ls[LS_TN], N = ls[LS_N];
+          const bool traced = ls[LS_TRACED] != 0;
+          for (int r = ttid; r < nwin; r += TT) {
+            const int wb = wins[r], c = wins[B + r];
+            const float S = reinterpret_cast<const float*>(wins)[2 * B + r];
+            const int Kb = mK[wb];
+            const bool isnew = (c == Kb);
+            if (isnew && Kb >= Kcap) {
+              ls[LS_ERR] = 1;  // more clusters than the device tables hold
+            } else {
+              const TabEntry old = isnew ? TabEntry{kInitSlot, 0, 0, 0} : tab[(size_t)wb * Kcap + c];
+              const bool moved = isnew || (c != mLast[wb]);
+              const int lc = wcol[r];
+              TabEntry nen;
+              nen.slot = lcolnew[lc];
+              nen.blocks = old.blocks + (moved ? 1 : 0);  // uisrnn.py:431-432; a new cluster starts at 1 (:76)
+              nen.visits = old.visits + 1;
+              nen.pad = 0;
+              ntab[(size_t)r * Kcap + c] = nen;
+              nK[r] = Kb + (isnew ? 1 : 0);
+              atomicMax((int*)&misc[MI_MAXK], Kb + (isnew ? 1 : 0));
+              nLast[r] = c;
+              nTot[r] = mTot[wb] + (moved ? 1 : 0);
+              nNl[r] = S;
+              if (lcolsrc[lc] == old.slot) lvis[lc] = old.visits;  // same slot => same visit count
+            }
+            if (t >= TN - N) bp_cta[((size_t)g * p.maxN + (t - (TN - N))) * B + r] = ((unsigned)wb << 16) | (unsigned)c;
+            if (traced) {
+              const long long rows = ((long long)ls[LS_DBGROWS_HI] << 32) | (unsigned)ls[LS_DBGROWS_LO];
+              if (p.dbg_win && rows + r < p.trace_capacity) {
+                p.dbg_win[(rows + r) * 2 + 0] = wb;
+                p.dbg_win[(rows + r) * 2 + 1] = c;
+                p.dbg_score[rows + r] = S;
+              }
+              if (r == 0 && p.dbg_off) p.dbg_off[t + 1] = rows + nwin;
+            }
           }
-          if (r == 0 && p.dbg_off) p.dbg_off[t + 1] = rows + nwin;
         }
       }
     }
-    for (int f = tid; f < Mtot; f += NT) {  // column list: lane-local -> CTA-wide
-      int g = 0;
-      while (g + 1 < G && f >= colbase[g + 1]) ++g;
-      const int lc = f - colbase[g];
+    named_bar_sync(1, NT);  // every lane's M, winners and tables are published
+
+    int nact = 0, Mtot = 0, colbase = 0;  // colbase: first CTA column of this thread's lane
+    for (int g = 0; g < G; ++g) {
+      nact += LSp(g)[LS_ACTIVE];
+      if (g == team_of()) colbase = Mtot;
+      Mtot += LSp(g)[LS_M];
+    }
+    if (nact == 0) break;
+    // column list: lane-local -> CTA-wide, each team its own lane's columns
+    if (team_of() < G) {
+      const int g = team_of(), TT = (NW / G) * 32, ttid = tid - g * TT;
+      volatile int* ls = LSp(g);
+      const int M = ls[LS_M];
+      const long long row = (((long long)ls[LS_ROW0_HI] << 32) | (unsigned)ls[LS_ROW0_LO]) + (ls[LS_T] % ls[LS_N]);
       const int* lcolsrc = reinterpret_cast<const int*>(lane_base(g) + L.l_lcol);
-      collane[f] = g;
-      colsrc[f] = lcolsrc[lc];
-      colnew[f] = lcolsrc[B + lc];
-      {
-        volatile int* lsg = LSp(g);
-        const long long row0g = ((long long)lsg[LS_ROW0_HI] << 32) | (unsigned)lsg[LS_ROW0_LO];
-        colrow[f] = row0g + (lsg[LS_T] % lsg[LS_N]);
+      const int* lvis = reinterpret_cast<const int*>(lane_base(g) + L.l_keys);
+      for (int lc = ttid; lc < M; lc += TT) {
+        const int f = colbase + lc;
+        collane[f] = g;
+        colsrc[f] = lcolsrc[lc];
+        colnew[f] = lcolsrc[B + lc];
+        colvis[f] = lvis[lc];
+        colrow[f] = row;
       }
     }
     constexpr int kColsPerPass = TC ? TCN : C::CP;
@@ -1595,49 +1583,54 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
       }
       st_cols += Mtot;
       st_pass += npass;
-      if (npass > 1 && !TC) { __threadfence_block(); misc[MI_PUBLISHED] = misc[MI_PUBLISHED] + (npass - 1); }
+      if (!TC) { __threadfence_block(); misc[MI_PUBLISHED] = misc[MI_PUBLISHED] + npass; }  // the producer streams
     }
     named_bar_sync(1, NT);
 
     UIS_PHASE(0);
     // ---- P5: GRU + MLP for the Mtot distinct source states, C::CP columns per weight pass
     if constexpr (TC) {
-      // Gaussian terms of the NEXT step, computed while the tensor pipe works on the first tiles of this pass: every
-      // slot of the next generation's tables except the ones this pass is about to write, against x_{t+1}
-      // (uisrnn.py:411-414 reads the pre-update mean; slots are immutable once written).
+      // Gaussian terms of the NEXT step, computed by every team for its lane while the tensor pipe works on the first
+      // tiles of this pass: every slot of the next generation's tables except the ones this pass is about to write,
+      // against x_{t+1} (uisrnn.py:411-414 reads the pre-update mean; slots are immutable once written).
       auto prescore = [&]() {
-        cp_async_wait_all();  // x_{t+1} was requested in P0
-        for (int f = tid; f < G * (int)PW; f += NT) {
-          const int g = f / (int)PW, w = f % (int)PW;
-          reinterpret_cast<unsigned*>(lane_base(g) + L.l_used)[w] = 0;    // (list marker of score_live_slots)
-          reinterpret_cast<unsigned*>(lane_base(g) + L.l_scored)[w] = 0;
-        }
-        named_bar_sync(1, NT);
-        for (int f = tid; f < G * B * Kcap; f += NT) {
-          const int g = f / (B * Kcap), r = (f / Kcap) % B, c = f % Kcap;
+        if (team_of() < G) {
+          const int g = team_of(), TW = NW / G, TT = TW * 32, ttid = tid - g * TT, twarp = warp - g * TW;
           volatile int* ls = LSp(g);
-          const bool go_on = ls[LS_ACTIVE] && !ls[LS_ERR] && ls[LS_NWIN] > 0 && ls[LS_T] + 1 < ls[LS_TN];
-          if (!go_on || r >= ls[LS_NWIN]) continue;
-          const int ngen = ls[LS_GEN] ^ 1;
-          const int* nK = reinterpret_cast<const int*>(lane_base(g) + L.l_meta) + ngen * 4 * B;
+          unsigned* used = reinterpret_cast<unsigned*>(lane_base(g) + L.l_used);
           unsigned* scored = reinterpret_cast<unsigned*>(lane_base(g) + L.l_scored);
-          if (r == 0 && c == 0) atomicOr(scored, 1u);  // slot 0 = INIT (the new-cluster candidate)
-          if (c < nK[r]) {
-            const int slot = (reinterpret_cast<const TabEntry*>(lane_base(g) + L.l_tabs) + (size_t)ngen * B * Kcap)[(size_t)r * Kcap + c].slot;
-            atomicOr(scored + (slot >> 5), 1u << (slot & 31));
+          cp_async_wait_all();  // x_{t+1} was requested in P0 by this team
+          for (unsigned w = ttid; w < PW; w += TT) { used[w] = 0; scored[w] = 0; }  // (used: list marker)
+          team_sync();
+          const int nwin = ls[LS_NWIN];
+          if (ls[LS_ACTIVE] && !ls[LS_ERR] && nwin > 0 && ls[LS_T] + 1 < ls[LS_TN]) {
+            const int ngen = ls[LS_GEN] ^ 1;
+            const int* nK = reinterpret_cast<const int*>(lane_base(g) + L.l_meta) + ngen * 4 * B;
+            const TabEntry* ntab = reinterpret_cast<const TabEntry*>(lane_base(g) + L.l_tabs) + (size_t)ngen * B * Kcap;
+            if (ttid == 0) atomicOr(scored, 1u);  // slot 0 = INIT (the new-cluster candidate)
+            for (int f = ttid; f < nwin * Kcap; f += TT) {
+              const int r = f / Kcap, c = f % Kcap;
+              if (c < nK[r]) {
+                const int slot = ntab[(size_t)r * Kcap + c].slot;
+                atomicOr(scored + (slot >> 5), 1u << (slot & 31));
+              }
+            }
+            team_sync();
+            const int M = ls[LS_M];
+            const int* lcolnew = reinterpret_cast<const int*>(lane_base(g) + L.l_lcol) + B;
+            for (int lc = ttid; lc < M; lc += TT)  // the slots this step's passes write: scored in P1 of the next step
+              atomicAnd(scored + (lcolnew[lc] >> 5), ~(1u << (lcolnew[lc] & 31)));
+            team_sync();
+            score_lane_slots(g, /*against the next frame=*/true, ttid, twarp, TW);
           }
         }
-        named_bar_sync(1, NT);
-        for (int f = tid; f < Mtot; f += NT) {  // the slots this step's passes write: scored in P1 of the next step
-          unsigned* scored = reinterpret_cast<unsigned*>(lane_base(collane[f]) + L.l_scored);
-          atomicAnd(scored + (colnew[f] >> 5), ~(1u << (colnew[f] & 31)));
-        }
-        score_live_slots(/*against the next frame=*/true);  // (starts with a barrier)
+        named_bar_sync(1, NT);  // the warpgroups enter the pass's tiles together
       };
       auto nothing = []() {};
-      if (Mtot == 0)
-        for (int f = tid; f < G * (int)PW; f += NT)
-          reinterpret_cast<unsigned*>(lane_base(f / (int)PW) + L.l_scored)[f % (int)PW] = 0;
+      if (Mtot == 0 && team_of() < G) {  // no pass, no pre-scoring: every team clears its own lane's marks
+        const int g = team_of(), TT = (NW / G) * 32;
+        for (unsigned w = tid - g * TT; w < PW; w += TT) reinterpret_cast<unsigned*>(lane_base(g) + L.l_scored)[w] = 0;
+      }
       for (int m0 = 0; m0 < Mtot; m0 += TCN) {
         if (m0 == 0)
           tc_run_pass<H, D, TC ? TCN : 16>(p, reinterpret_cast<const unsigned char*>(ring), reinterpret_cast<unsigned char*>(XA),
@@ -1682,76 +1675,70 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
     }
     }  // !TC
 
-    // ---- P6: advance every lane; finished utterances are back-tracked and replaced
-    int fin[kMaxLanes];
-    for (int g = 0; g < G; ++g) {
+    // ---- P6: every team advances its lane; a finished utterance is back-tracked and replaced
+    if (team_of() < G) {
+      const int g = team_of(), TT = (NW / G) * 32, ttid = tid - g * TT;
       volatile int* ls = LSp(g);
       const bool act = ls[LS_ACTIVE] != 0;
-      const bool failed = act && ls[LS_ERR] != 0;
-      fin[g] = act && (failed || ls[LS_NWIN] == 0 || ls[LS_T] + 1 >= ls[LS_TN]);
-    }
-    for (int g = 0; g < G; ++g) {  // debug taps of finishing lanes (all threads)
-      if (!fin[g]) continue;
-      volatile int* ls = LSp(g);
-      const int u = ls[LS_U], nwin = ls[LS_NWIN], ngen = ls[LS_GEN] ^ 1;
-      const bool ok = !ls[LS_ERR] && nwin > 0;
-      const int* fK = reinterpret_cast<const int*>(lane_base(g) + L.l_meta) + ngen * 4 * B;
-      const float* fNl = reinterpret_cast<const float*>(fK + 3 * B);
-      // utterance epilogue: back-track the returned hypotheses (uisrnn.py:561), one per thread.  Hypothesis j is the
-      // j-th final rank with min_speakers clusters (rank 0 when none has them, j = 0); it walks its own column chain
-      // into label plane j.  (Stationary-weights mode: the replicas of a group decode the same utterance, and CTA 0
-      // of the group reports it.)
-      for (int j = tid; j < p.n_best && !(STAT && sq != 0); j += NT) {
-        const int r0 = ok ? nbest_rank(fK, nwin, ls[LS_KLO], j) : -1;
-        const int N = ls[LS_N];
-        int* lab = p.labels + (size_t)j * p.label_plane + (((long long)ls[LS_ROW0_HI] << 32) | (unsigned)ls[LS_ROW0_LO]);
-        if (r0 < 0) {
-          for (int i = 0; i < N; ++i) lab[i] = -1;
-        } else {
-          const unsigned* bp = bp_cta + (size_t)g * p.maxN * B;
-          int r = r0;
-          for (int i = N - 1; i >= 0; --i) {
-            const unsigned e = bp[(size_t)i * B + r];
-            lab[i] = (int)(e & 0xffffu);
-            r = (int)(e >> 16);
+      const bool fin = act && (ls[LS_ERR] != 0 || ls[LS_NWIN] == 0 || ls[LS_T] + 1 >= ls[LS_TN]);
+      if (fin) {  // debug taps and outputs of the finishing utterance (the team)
+        const int u = ls[LS_U], nwin = ls[LS_NWIN], ngen = ls[LS_GEN] ^ 1;
+        const bool ok = !ls[LS_ERR] && nwin > 0;
+        const int* fK = reinterpret_cast<const int*>(lane_base(g) + L.l_meta) + ngen * 4 * B;
+        const float* fNl = reinterpret_cast<const float*>(fK + 3 * B);
+        // utterance epilogue: back-track the returned hypotheses (uisrnn.py:561), one per thread.  Hypothesis j is the
+        // j-th final rank with min_speakers clusters (rank 0 when none has them, j = 0); it walks its own column chain
+        // into label plane j.  (Stationary-weights mode: the replicas of a group decode the same utterance, and CTA 0
+        // of the group reports it.)
+        for (int j = ttid; j < p.n_best && !(STAT && sq != 0); j += TT) {
+          const int r0 = ok ? nbest_rank(fK, nwin, ls[LS_KLO], j) : -1;
+          const int N = ls[LS_N];
+          int* lab = p.labels + (size_t)j * p.label_plane + (((long long)ls[LS_ROW0_HI] << 32) | (unsigned)ls[LS_ROW0_LO]);
+          if (r0 < 0) {
+            for (int i = 0; i < N; ++i) lab[i] = -1;
+          } else {
+            const unsigned* bp = bp_cta + (size_t)g * p.maxN * B;
+            int r = r0;
+            for (int i = N - 1; i >= 0; --i) {
+              const unsigned e = bp[(size_t)i * B + r];
+              lab[i] = (int)(e & 0xffffu);
+              r = (int)(e >> 16);
+            }
+          }
+          if (j == 0) {
+            if (p.spk_out) p.spk_out[u] = ok ? fK[r0] : 0;
+            if (p.nbest_count) p.nbest_count[u] = ok ? nbest_n(fK, nwin, ls[LS_KLO], p.n_best) : 0;
+          }
+          nbest_store(p, u, j, r0, fK, fNl);
+        }
+        if (p.dbg_final_scores && tap_leader) {
+          for (int b = ttid; b < B; b += TT) p.dbg_final_scores[(size_t)u * B + b] = (ok && b < nwin) ? fNl[b] : INF;
+          if (ttid == 0 && p.dbg_final_k) p.dbg_final_k[u] = ok ? fK[0] : 0;
+        }
+        if (ls[LS_TRACED] && ok && p.dbg_best_mean) {
+          // (stationary-weights mode: the slots are in the group's pool, published by the group barrier that ended the
+          //  last weight pass; other CTAs wrote most of them, so the reads bypass L1)
+          const TabEntry* ftab = reinterpret_cast<const TabEntry*>(lane_base(g) + L.l_tabs) + (size_t)ngen * B * Kcap;
+          for (int c = 0; c < fK[0]; ++c) {  // best hypothesis = rank 0
+            const TabEntry en = ftab[c];
+            const float* mp = pool_mean_cta + g * pool_m_stride + (size_t)en.slot * D;
+            const float* hp = pool_hidden_cta + g * pool_h_stride + (size_t)en.slot * DH;
+            for (int d = ttid; d < D; d += TT) p.dbg_best_mean[(size_t)c * D + d] = STAT ? __ldcg(mp + d) : mp[d];
+            for (int q = ttid; q < DH; q += TT) p.dbg_best_hidden[(size_t)c * DH + q] = STAT ? __ldcg(hp + q) : hp[q];
+            if (ttid == 0) p.dbg_best_blocks[c] = en.blocks;
           }
         }
-        if (j == 0) {
-          if (p.spk_out) p.spk_out[u] = ok ? fK[r0] : 0;
-          if (p.nbest_count) p.nbest_count[u] = ok ? nbest_n(fK, nwin, ls[LS_KLO], p.n_best) : 0;
-        }
-        nbest_store(p, u, j, r0, fK, fNl);
-      }
-      if (p.dbg_final_scores && tap_leader) {
-        if (tid < B) p.dbg_final_scores[(size_t)u * B + tid] = (ok && tid < nwin) ? fNl[tid] : INF;
-        if (tid == 0 && p.dbg_final_k) p.dbg_final_k[u] = ok ? fK[0] : 0;
-      }
-      if (ls[LS_TRACED] && ok && p.dbg_best_mean) {
-        // (stationary-weights mode: the slots are in the group's pool, published by the group barrier that ended the
-        //  last weight pass; other CTAs wrote most of them, so the reads bypass L1)
-        const TabEntry* ftab = reinterpret_cast<const TabEntry*>(lane_base(g) + L.l_tabs) + (size_t)ngen * B * Kcap;
-        for (int c = 0; c < fK[0]; ++c) {  // best hypothesis = rank 0
-          const TabEntry en = ftab[c];
-          const float* mp = pool_mean_cta + g * pool_m_stride + (size_t)en.slot * D;
-          const float* hp = pool_hidden_cta + g * pool_h_stride + (size_t)en.slot * DH;
-          if (tid < D) p.dbg_best_mean[(size_t)c * D + tid] = STAT ? __ldcg(mp + tid) : mp[tid];
-          for (int q = tid; q < DH; q += NT) p.dbg_best_hidden[(size_t)c * DH + q] = STAT ? __ldcg(hp + q) : hp[q];
-          if (tid == 0) p.dbg_best_blocks[c] = en.blocks;
+        if constexpr (STAT) {
+          // The traced utterance's state is read from the group's pool above; the other CTAs may only write the slots
+          // of their next utterance (its first weight pass, before any group barrier) once the leader has read it.
+          // (One lane per CTA in this mode: the team is every consumer thread.)
+          if (u == p.trace_utt && p.dbg_best_mean)
+            stat_group_sync<NT>(p.stat_bar + (size_t)sgroup * kStatGroup, stat_epoch, tid);
         }
       }
-    }
-    if constexpr (STAT) {
-      // The traced utterance's state is read from the group's pool above; the other CTAs may only write the slots of
-      // their next utterance (its first weight pass, before any group barrier) once the leader has read it.
-      if (fin[0] && LSp(0)[LS_U] == p.trace_utt && p.dbg_best_mean)
-        stat_group_sync<NT>(p.stat_bar + (size_t)sgroup * kStatGroup, stat_epoch, tid);
-    }
-    named_bar_sync(1, NT);
-    if (tid < G) {
-      const int g = tid;
-      volatile int* ls = LSp(g);
-      if (ls[LS_ACTIVE]) {
-        if (fin[g]) {
+      team_sync();  // the finished lane's tables are read before lane_fetch reuses them
+      if (ttid == 0 && act) {
+        if (fin) {
           if (!(STAT && sq != 0)) p.status[ls[LS_U]] = ls[LS_ERR] ? -4 : ls[LS_NWIN] == 0 ? -1 : 0;
           lane_fetch(g);
         } else {
@@ -1760,13 +1747,11 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
           ls[LS_T] = ls[LS_T] + 1; ls[LS_NB] = ls[LS_NWIN]; ls[LS_GEN] = ls[LS_GEN] ^ 1; ls[LS_FRESH] = 0;
         }
       }
-    }
-    named_bar_sync(1, NT);
-    {
-      bool any = false;
-      for (int g = 0; g < G; ++g)
-        if (fin[g] && LSp(g)[LS_ACTIVE] && LSp(g)[LS_FRESH]) { lane_prefetch(g, 0); any = true; }
-      if (any) cp_async_commit();
+      team_sync();
+      if (fin && ls[LS_ACTIVE] && ls[LS_FRESH]) {
+        lane_prefetch(g, 0, ttid, TT);
+        cp_async_commit();
+      }
     }
     UIS_PHASE(5);
   }  // CTA steps
