@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define UIS_ABI_VERSION 6
+#define UIS_ABI_VERSION 7
 
 typedef enum uis_status {
   UIS_OK = 0,
@@ -225,6 +225,38 @@ int uis_predict_device_nbest(uis_model* m, const float* x_dev, const int64_t* fr
                              const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
                              const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
                              const uis_nbest_out* out);
+
+/*
+ * ABI 7: the score of given labellings.  Not in the reference, where the same quantity exists only inside the search
+ * (BeamState.neg_likelihood, uisrnn.py:388-453).  The score of utterance u is the neg_likelihood of the trace that
+ * assigns frame t to cluster labels[u][t]: per frame loss_t = fl32(f64(mse_t) - pen_t), with mse_t the Gaussian term
+ * of the frame against its cluster's running mean before that frame (mean0 for a new cluster; +inf by the first-column
+ * rule) and pen_t the transition / ddCRP term of the trace so far; the score is the fp32 running sum of loss_t in frame
+ * order.  That is the arithmetic of the search, so a hypothesis the FFMA beam kernel kept (engine 1, no cluster mode)
+ * scores exactly the value its N-best entry reports.  Lower is better.  test_iteration is not applied: the sequence
+ * is scored once, as given (tile both the rows and the labels to score a tiled decode).  An empty utterance scores 0.
+ *   labels       canonical int32 ids: 0, 1, 2, ... in order of first appearance (the ids a trace holds); anything
+ *                else is UIS_ERR_INVALID, and uis_last_error() names the utterance and the frame.  Any number of
+ *                clusters per utterance (no kcap).
+ *   scores_out   [U] float32 neg_likelihood.
+ *   frame_out    per-frame increments loss_t (may be NULL); summed in fp32 in frame order they give the score bit for
+ *                bit.
+ * uis_score: host buffers (seqs[u] float64 [n_frames[u], D] as in uis_predict, labels[u] int32 [n_frames[u]],
+ * frame_out[u] float32 [n_frames[u]]); returns when the scores have landed.  uis_score_device: device buffers in the
+ * layout of uis_predict_device (x_dev fp32 [frame_offsets[U], D], labels_dev int32 [frame_offsets[U]], scores_dev [U],
+ * frame_dev [frame_offsets[U]]; frame_offsets on the host).  It copies the labels back to plan the chains, which
+ * synchronises `stream` once at the start of the call; the kernels are then enqueued without waiting.
+ * Work: one GRU + MLP column per frame that is not the first of its cluster, in the FFMA weight pass of the beam
+ * kernels (every kernel shape and depth).  Workspace: the handle's cache, about (12 H + 4 D + 24) bytes per frame; a
+ * list that does not fit the device fails with UIS_ERR_NOMEM (it is not split into groups).  uis_get_stats after a
+ * score call fills utterances, frames, gru_columns, weight_passes, kernel_launches, ctas, max_k (most clusters in one
+ * utterance), prepass_ms, beam_ms (the chain kernel), engine = 1 and, for uis_score, the host-path fields; the rest
+ * is zero.
+ */
+int uis_score(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+              const int32_t* const* labels, float* scores_out, float* const* frame_out, void* stream);
+int uis_score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                     const int32_t* labels_dev, float* scores_dev, float* frame_dev, void* stream);
 
 /* Device bytes uis_predict_device() will hold for this problem (workspace is cached in the handle). */
 size_t uis_predict_workspace_bytes(uis_model* m, const int64_t* frame_offsets, int U,

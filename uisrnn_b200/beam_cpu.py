@@ -22,7 +22,7 @@ def nbest_ranks(clusters, min_speakers, n_best):
 
 class _Hypothesis:
   """One beam entry: per-cluster running means / hidden states / visit and block counts."""
-  __slots__ = ('means', 'hiddens', 'visits', 'blocks', 'trace', 'score')
+  __slots__ = ('means', 'hiddens', 'visits', 'blocks', 'trace', 'score', 'loss')  # loss: the last step's increment
 
   def __init__(self, parent=None):
     if parent is None:
@@ -90,6 +90,7 @@ class CpuBeamSearch:
         hyp.visits.append(1)
         hyp.blocks.append(1)
         hyp.trace.append(cluster)
+    hyp.loss = loss
     hyp.score = hyp.score + loss  # int 0 at first, float32 afterwards, as in the reference
     return True
 
@@ -120,6 +121,21 @@ class CpuBeamSearch:
 
     walk(hyp, 0, ())
     return table
+
+  @torch.no_grad()
+  def score(self, sequence, labels):
+    """(neg_likelihood, float32 [N] per-frame increments) of the trace that assigns frame t of `sequence` (float64
+    [N, D]) to cluster labels[t] (canonical ids: 0, 1, 2, ... in order of first appearance): `_advance` with the state
+    update, frame by frame from an empty hypothesis.  No test_iteration tiling."""
+    self.rnn.eval()
+    frames = torch.from_numpy(np.asarray(sequence)).float().to(self.device)
+    hyp = _Hypothesis()
+    increments = np.zeros(len(frames), np.float32)
+    for t, (frame, cluster) in enumerate(zip(frames, labels)):
+      if not self._advance(hyp, frame, int(cluster), True):
+        raise ValueError('frame %d: label %d is not canonical' % (t, int(cluster)))
+      increments[t] = hyp.loss
+    return np.float32(hyp.score), increments
 
   @torch.no_grad()
   def decode(self, sequence, beam_size, look_ahead, test_iteration, max_speakers=0, min_speakers=0,

@@ -163,12 +163,15 @@ struct uis_model {
   DevBuf spk_bound, spk_out;  // bounded calls only: [U][2] speaker bounds; [U] speaker counts (host-buffer entry point)
   DevBuf nb_scores, nb_speakers, nb_count;  // N-best calls, host-buffer entry point: [U][n_best], [U][n_best], [U]
   DevBuf tree_arena;  // look-ahead spill kernel: [spill CTAs][make_tree_arena(..).total]
+  // score calls (uis_kernels_score.cu): chain plan, per-frame Gaussian terms, reduce scratch, host entry's outputs
+  DevBuf sc_chain_off, sc_chain_rows, sc_mse, sc_blocks, sc_out;
   DevBuf dbg_win, dbg_score, dbg_off, dbg_final_scores, dbg_final_k, dbg_best_mean, dbg_best_hidden,
       dbg_best_blocks;
   // last call
   uis_stats stats{};
   int last_U = 0;
   bool last_tree_spill = false;  // the last call ran the look-ahead spill kernel (its caps name the arena in errors)
+  bool last_score = false;       // the last call was a score call (two counters, no per-utterance status)
   int last_spill_ni = 0, last_spill_nlf = 0;
   size_t last_spill_budget = 0;
   cudaStream_t last_stream = nullptr;
@@ -644,6 +647,27 @@ int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_
                       const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out,
                       const NBestOut& nb);
 
+// The model's part of the kernel parameters: weights, constants, log terms and log tables (ensure_log_tables first).
+uis::BeamParams model_params(const uis_model* m) {
+  const int H = m->H;
+  uis::BeamParams p{};
+  p.whh_t = m->whh_t.as<float>(); p.w1_t = m->w1_t.as<float>(); p.w2_t = m->w2_t.as<float>();
+  p.depth = m->depth;
+  for (int l = 1; l < m->depth; ++l) {
+    p.wih_up_t[l - 1] = m->wih_up_t.as<float>() + (size_t)(l - 1) * H * 3 * H;
+    p.whh_up_t[l - 1] = m->whh_t.as<float>() + (size_t)l * H * 3 * H;
+  }
+  p.bih_up = m->bih.as<float>() + 3 * H;   // layers >= 1
+  p.bhh_up = m->bhh.as<float>() + 3 * H;
+  p.bhh = m->bhh.as<float>(); p.b1 = m->b1.as<float>(); p.b2 = m->b2.as<float>();
+  p.wvec = m->wvec.as<float>(); p.mean0 = m->mean0.as<float>(); p.hidden0 = m->hidden0.as<float>();
+  p.log_p0 = std::log(m->p0);          // np.log(self.transition_bias)      uisrnn.py:418
+  p.log_1mp0 = std::log(1.0 - m->p0);  // np.log(1 - self.transition_bias)  uisrnn.py:416
+  p.log_alpha = std::log(m->alpha);    // np.log(self.crp_alpha)            uisrnn.py:445
+  p.logn = m->logn.as<double>(); p.logtot = m->logtot.as<double>();
+  return p;
+}
+
 int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, const Plan& pl, int32_t* labels_dev,
                const uis_debug_taps* taps, cudaStream_t st, const SpeakerBounds& sb, const NBestOut& nb,
                bool gi_ready = false) {
@@ -665,6 +689,7 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   m->stats.lanes = pl.G;
   m->stats.cluster = pl.cluster;
   m->last_U = U;
+  m->last_score = false;
   m->last_tree_spill = pl.L > 1 && pl.spill;
   m->last_spill_ni = pl.spill_ni; m->last_spill_nlf = pl.spill_nlf; m->last_spill_budget = pl.spill_budget;
   m->last_stream = st;
@@ -710,21 +735,7 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   CU(cudaMemsetAsync(m->queue_stats.p, 0, 40 * sizeof(unsigned long long), st));
   CU(cudaMemsetAsync(m->status.p, 0xff, U * sizeof(int), st));
 
-  uis::BeamParams p{};
-  p.whh_t = m->whh_t.as<float>(); p.w1_t = m->w1_t.as<float>(); p.w2_t = m->w2_t.as<float>();
-  p.depth = m->depth;
-  for (int l = 1; l < m->depth; ++l) {
-    p.wih_up_t[l - 1] = m->wih_up_t.as<float>() + (size_t)(l - 1) * H * 3 * H;
-    p.whh_up_t[l - 1] = m->whh_t.as<float>() + (size_t)l * H * 3 * H;
-  }
-  p.bih_up = m->bih.as<float>() + 3 * H;   // layers >= 1
-  p.bhh_up = m->bhh.as<float>() + 3 * H;
-  p.bhh = m->bhh.as<float>(); p.b1 = m->b1.as<float>(); p.b2 = m->b2.as<float>();
-  p.wvec = m->wvec.as<float>(); p.mean0 = m->mean0.as<float>(); p.hidden0 = m->hidden0.as<float>();
-  p.log_p0 = std::log(m->p0);          // np.log(self.transition_bias)      uisrnn.py:418
-  p.log_1mp0 = std::log(1.0 - m->p0);  // np.log(1 - self.transition_bias)  uisrnn.py:416
-  p.log_alpha = std::log(m->alpha);    // np.log(self.crp_alpha)            uisrnn.py:445
-  p.logn = m->logn.as<double>(); p.logtot = m->logtot.as<double>();
+  uis::BeamParams p = model_params(m);
   p.x = x_dev; p.gi = m->gi.as<float>();
   p.row_off = m->row_off.as<long long>(); p.order = m->order.as<int>();
   p.U = U; p.B = pl.B; p.Kcap = pl.Kcap; p.T = pl.T; p.P = pl.P; p.maxN = pl.maxN; p.G = pl.G;
@@ -876,6 +887,14 @@ int collect(uis_model* m) {
   CU(cudaStreamSynchronize(m->last_stream));
   unsigned long long s[24];
   CU(cudaMemcpy(s, m->queue_stats.as<unsigned long long>() + 8, sizeof s, cudaMemcpyDeviceToHost));
+  if (m->last_score) {  // the chain kernel's columns and passes; max_k came from the labels
+    m->stats.gru_columns = (int64_t)s[0];
+    m->stats.weight_passes = (int64_t)s[1];
+    CU(cudaEventElapsedTime(&m->stats.prepass_ms, m->ev[0], m->ev[1]));
+    CU(cudaEventElapsedTime(&m->stats.beam_ms, m->ev[1], m->ev[2]));
+    m->stats_pending = false;
+    return 0;
+  }
   for (int i = 0; i < 10; ++i) m->stats.phase_cycles[i] = (int64_t)s[8 + i];
   for (int i = 0; i < 4; ++i) m->stats.tc_cycles[i] = (int64_t)s[18 + i];
   m->stats.gru_columns = (int64_t)s[0];
@@ -1093,7 +1112,8 @@ int uis_model_destroy(uis_model* m) {
                     &m->pool_mean, &m->pool_hidden, &m->bp, &m->queue_stats, &m->labels, &m->status, &m->dbg_win,
                     &m->dbg_score, &m->dbg_off, &m->dbg_final_scores, &m->dbg_final_k, &m->dbg_best_mean,
                     &m->dbg_best_hidden, &m->dbg_best_blocks, &m->tc_planes, &m->tc_scratch, &m->pool_mse, &m->stat_bar, &m->stat_scratch,
-                    &m->tree_arena, &m->nb_scores, &m->nb_speakers, &m->nb_count};
+                    &m->tree_arena, &m->nb_scores, &m->nb_speakers, &m->nb_count, &m->sc_chain_off,
+                    &m->sc_chain_rows, &m->sc_mse, &m->sc_blocks, &m->sc_out};
   for (DevBuf* b : bufs) b->release();
   for (auto& e : m->ev)
     if (e) cudaEventDestroy(e);
@@ -1208,6 +1228,9 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
                             const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
                             const SpeakerBounds& sb, int32_t* speakers_out, const NBestOut& nb);
 
+int stage_host_rows(uis_model* m, const double* const* seqs, int U, const int64_t* off, size_t rows, cudaStream_t st,
+                    int* n_chunks_out, bool* staged_out);
+
 int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
                        const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
                        const SpeakerBounds& sb, int32_t* speakers_out, const NBestOut& nb) {
@@ -1227,20 +1250,12 @@ int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n
 int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
                             const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
                             const SpeakerBounds& sb_host, int32_t* speakers_out, const NBestOut& nb_host) {
-  const int D = m->D_user, H = m->H;  // the caller's rows; the device rows are padded to m->D floats
   const size_t rows = (size_t)pl.rows;
   if (rows == 0) {
     m->stats = uis_stats{};
     m->stats.utterances = U;
     return 0;
   }
-  if (int rc = ensure_host_path(m)) return rc;
-  const size_t chunk = std::min(staging_chunk_rows(D), rows);
-  const int n_chunks = (int)((rows + chunk - 1) / chunk);
-  const int slots = std::min(n_chunks, (int)uis_model::kSlots);
-  if (int rc = m->x64.ensure((size_t)slots * chunk * D * 8)) return rc;
-  if (int rc = m->x32.ensure(rows * m->D * 4)) return rc;
-  if (int rc = m->gi.ensure(rows * 3 * H * sizeof(float))) return rc;
   const int K = nb_host.k;  // label planes
   if (int rc = m->labels.ensure(rows * 4 * K)) return rc;
   SpeakerBounds sb = sb_host;  // speaker counts land in the handle's device buffer, then in `speakers_out`
@@ -1272,6 +1287,44 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
     }
     m->labels_pin_cap = want;
   }
+  int n_chunks = 0;
+  bool staged = false;
+  if (int rc = stage_host_rows(m, seqs, U, off, rows, st, &n_chunks, &staged)) return rc;
+  if (int rc = run_device(m, m->x32.as<float>(), off, U, pl, m->labels.as<int32_t>(), taps, st, sb, nb, /*gi_ready=*/true))
+    return rc;
+  m->stats.kernel_launches = 1 + 2 * (int64_t)n_chunks + (pl.L > 1 && pl.spill == 1 ? 1 : 0);
+  m->stats.chunks = n_chunks;
+  m->stats.staged = staged ? 1 : 0;
+  CU(cudaMemcpyAsync(m->labels_pin, m->labels.p, rows * 4 * K, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  for (int j = 0; j < K; ++j)  // plane j of the device rows -> rows j of the caller's [K][n_frames[q]] buffers
+    for (int q = 0; q < U; ++q)
+      if (n_frames[q] > 0)
+        std::memcpy(labels_out[q] + (size_t)j * n_frames[q], m->labels_pin + (size_t)j * rows + off[q], (size_t)n_frames[q] * 4);
+  if (speakers_out) CU(cudaMemcpy(speakers_out, sb.out_dev, (size_t)U * 4, cudaMemcpyDeviceToHost));
+  if (nb.scores) CU(cudaMemcpy(nb_host.scores, nb.scores, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
+  if (nb.speakers) CU(cudaMemcpy(nb_host.speakers, nb.speakers, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
+  if (nb.count) CU(cudaMemcpy(nb_host.count, nb.count, (size_t)U * 4, cudaMemcpyDeviceToHost));
+  if (int rc = collect(m)) return rc;
+  CU(cudaEventElapsedTime(&m->stats.h2d_ms, m->ev_h2d[0], m->ev_h2d[1]));
+  CU(cudaEventElapsedTime(&m->stats.pipeline_ms, m->ev_pipe, m->ev[1]));  // first cast -> beam kernel start
+  return 0;
+}
+
+// Input pipeline of the host-buffer entry points (uis_predict*, uis_score): the float64 rows of utterances [0, U)
+// (device rows off[u] ..) travel in chunks through the staging ring on the copy stream while `st` casts each landed
+// chunk to fp32 (padded to m->D) into m->x32 and runs its input projection into m->gi.  ev_h2d[0..1] bracket the
+// copies, ev_pipe marks the first cast.
+int stage_host_rows(uis_model* m, const double* const* seqs, int U, const int64_t* off, size_t rows, cudaStream_t st,
+                    int* n_chunks_out, bool* staged_out) {
+  const int D = m->D_user, H = m->H;
+  if (int rc = ensure_host_path(m)) return rc;
+  const size_t chunk = std::min(staging_chunk_rows(D), rows);
+  const int n_chunks = (int)((rows + chunk - 1) / chunk);
+  const int slots = std::min(n_chunks, (int)uis_model::kSlots);
+  if (int rc = m->x64.ensure((size_t)slots * chunk * D * 8)) return rc;
+  if (int rc = m->x32.ensure(rows * m->D * 4)) return rc;
+  if (int rc = m->gi.ensure(rows * 3 * H * sizeof(float))) return rc;
   cudaStream_t cs = m->copy_stream;
   // Pageable or pinned?  Ordinary numpy arrays are pageable: the driver would stage every cudaMemcpy itself, in one
   // thread (measured 10.8 GB/s against 44.6 GB/s from pinned memory).  Such inputs go through a pinned ring of our own,
@@ -1283,7 +1336,7 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
       staged = env[0] == '1';
     } else if (rows * (size_t)D * 8 >= ((size_t)8 << 20)) {  // small inputs: not worth waking the threads
       for (int q = 0; q < U && !staged; q += std::max(1, U / 8)) {  // a sample of the list
-        if (n_frames[q] <= 0) continue;
+        if (off[q + 1] <= off[q]) continue;
         cudaPointerAttributes attr{};
         if (cudaPointerGetAttributes(&attr, seqs[q]) != cudaSuccess) { (void)cudaGetLastError(); staged = true; }
         else if (attr.type == cudaMemoryTypeUnregistered) staged = true;
@@ -1359,24 +1412,8 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
     r0 = r1;
   }
   CU(cudaEventRecord(m->ev_h2d[1], cs));
-  if (int rc = run_device(m, m->x32.as<float>(), off, U, pl, m->labels.as<int32_t>(), taps, st, sb, nb, /*gi_ready=*/true))
-    return rc;
-  m->stats.kernel_launches = 1 + 2 * (int64_t)n_chunks + (pl.L > 1 && pl.spill == 1 ? 1 : 0);
-  m->stats.chunks = n_chunks;
-  m->stats.staged = staged ? 1 : 0;
-  CU(cudaMemcpyAsync(m->labels_pin, m->labels.p, rows * 4 * K, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  for (int j = 0; j < K; ++j)  // plane j of the device rows -> rows j of the caller's [K][n_frames[q]] buffers
-    for (int q = 0; q < U; ++q)
-      if (n_frames[q] > 0)
-        std::memcpy(labels_out[q] + (size_t)j * n_frames[q], m->labels_pin + (size_t)j * rows + off[q], (size_t)n_frames[q] * 4);
-  if (speakers_out) CU(cudaMemcpy(speakers_out, sb.out_dev, (size_t)U * 4, cudaMemcpyDeviceToHost));
-  if (nb.scores) CU(cudaMemcpy(nb_host.scores, nb.scores, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
-  if (nb.speakers) CU(cudaMemcpy(nb_host.speakers, nb.speakers, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
-  if (nb.count) CU(cudaMemcpy(nb_host.count, nb.count, (size_t)U * 4, cudaMemcpyDeviceToHost));
-  if (int rc = collect(m)) return rc;
-  CU(cudaEventElapsedTime(&m->stats.h2d_ms, m->ev_h2d[0], m->ev_h2d[1]));
-  CU(cudaEventElapsedTime(&m->stats.pipeline_ms, m->ev_pipe, m->ev[1]));  // first cast -> beam kernel start
+  *n_chunks_out = n_chunks;
+  *staged_out = staged;
   return 0;
 }
 
@@ -1503,6 +1540,243 @@ int uis_get_stats(uis_model* m, uis_stats* out) {
   const int rc = collect(m);
   *out = m->stats;
   return rc;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------------
+// score(): the neg_likelihood of given labellings (uis_kernels_score.cu)
+namespace {
+
+// Chains of a score call, one per (utterance, cluster), longest first, with their frame rows in frame order.  The
+// labels must be canonical: 0, 1, 2, ... in order of first appearance (the ids a trace holds).
+struct ChainPlan {
+  std::vector<long long> off, rows;  // [chains + 1] offsets into rows; [frames] device rows
+  int chains = 0, queued = 0, max_k = 0;  // queued: chains of length >= 2 (a prefix, longest first)
+};
+
+int plan_chains(const int32_t* labels, const int64_t* off, int U, ChainPlan* cp) {
+  std::vector<long long> base(U + 1, 0);  // first chain id of every utterance
+  for (int u = 0; u < U; ++u) {
+    int K = 0;
+    for (long long r = off[u]; r < off[u + 1]; ++r) {
+      const int c = labels[r];
+      if (c < 0 || c > K)
+        return fail(UIS_ERR_INVALID, "utterance %d frame %lld: label %d is not canonical (labels are 0, 1, 2, ... in "
+                    "order of first appearance, so at most %d here)", u, r - off[u], c, K);
+      K += (c == K) ? 1 : 0;
+    }
+    base[u + 1] = base[u] + K;
+    cp->max_k = std::max(cp->max_k, K);
+  }
+  const long long nch = base[U], rows = U > 0 ? off[U] : 0;
+  if (nch > 0x7fffffffll) return fail(UIS_ERR_INVALID, "more than 2^31 - 1 (utterance, cluster) chains");
+  std::vector<long long> len(nch, 0);
+  for (int u = 0; u < U; ++u)
+    for (long long r = off[u]; r < off[u + 1]; ++r) ++len[base[u] + labels[r]];
+  std::vector<int> order(nch);
+  std::iota(order.begin(), order.end(), 0);
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return len[a] > len[b]; });
+  cp->off.assign(nch + 1, 0);
+  std::vector<long long> cursor(nch);
+  for (long long i = 0; i < nch; ++i) {
+    cp->off[i + 1] = cp->off[i] + len[order[i]];
+    cursor[order[i]] = cp->off[i];
+  }
+  cp->rows.resize(std::max(rows, 1ll));
+  for (int u = 0; u < U; ++u)
+    for (long long r = off[u]; r < off[u + 1]; ++r) cp->rows[cursor[base[u] + labels[r]]++] = r;
+  cp->chains = (int)nch;
+  cp->queued = 0;
+  while (cp->queued < cp->chains && len[order[cp->queued]] >= 2) ++cp->queued;
+  return 0;
+}
+
+// Enqueues a score call on `st`: input projection (unless gi_ready), chain kernel, first visits, reduce.  x_dev: the
+// fp32 rows at the kernel shape (m->D); labels_dev: the canonical labels the plan was made from.
+int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const ChainPlan& cp, const int32_t* labels_dev,
+              float* scores_dev, float* frame_dev, cudaStream_t st, bool gi_ready) {
+  const int H = m->H, D = m->D;
+  const long long rows = off[U];
+  long long maxN = 0;
+  for (int u = 0; u < U; ++u) maxN = std::max<long long>(maxN, off[u + 1] - off[u]);
+  if (int rc = ensure_log_tables(m, (int)maxN)) return rc;  // block counts and totals reach N
+  const int CP = uis::score_cp(H);
+  const int ctas = (int)std::max(1ll, std::min<long long>(m->num_sms, (cp.queued + CP - 1) / CP));
+  if (uis::score_smem(H, D) > 227u * 1024u) return fail(UIS_ERR_UNSUPPORTED, "no score kernel for hidden=%d dim=%d", H, D);
+  if (int rc = m->row_off.ensure((U + 1) * sizeof(long long))) return rc;
+  if (int rc = m->queue_stats.ensure(40 * sizeof(unsigned long long))) return rc;
+  if (int rc = m->gi.ensure((size_t)rows * 3 * H * sizeof(float))) return rc;
+  if (int rc = m->pool_mean.ensure((size_t)ctas * CP * 2 * D * sizeof(float))) return rc;
+  if (int rc = m->pool_hidden.ensure((size_t)ctas * CP * 2 * m->depth * H * sizeof(float))) return rc;
+  if (int rc = m->sc_chain_off.ensure(cp.off.size() * sizeof(long long))) return rc;
+  if (int rc = m->sc_chain_rows.ensure(cp.rows.size() * sizeof(long long))) return rc;
+  if (int rc = m->sc_mse.ensure((size_t)rows * sizeof(float))) return rc;
+  if (int rc = m->sc_blocks.ensure((size_t)rows * sizeof(int))) return rc;
+  std::vector<long long> off_ll(off, off + U + 1);
+  CU(cudaMemcpyAsync(m->row_off.p, off_ll.data(), (U + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(m->sc_chain_off.p, cp.off.data(), cp.off.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(m->sc_chain_rows.p, cp.rows.data(), cp.rows.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+  CU(cudaMemsetAsync(m->queue_stats.p, 0, 40 * sizeof(unsigned long long), st));
+
+  uis::ScoreParams sp{};
+  sp.b = model_params(m);
+  sp.b.x = x_dev; sp.b.gi = m->gi.as<float>();
+  sp.b.row_off = m->row_off.as<long long>();
+  sp.b.U = U; sp.b.P = 2;
+  sp.b.pool_mean = m->pool_mean.as<float>(); sp.b.pool_hidden = m->pool_hidden.as<float>();
+  sp.b.queue = m->queue_stats.as<int>();
+  sp.b.stats = m->queue_stats.as<unsigned long long>() + 8;
+  sp.chain_off = m->sc_chain_off.as<long long>(); sp.chain_rows = m->sc_chain_rows.as<long long>();
+  sp.chains = cp.chains; sp.queued = cp.queued;
+  sp.mse = m->sc_mse.as<float>(); sp.labels = labels_dev; sp.scores = scores_dev; sp.frame_out = frame_dev;
+  sp.blocks = m->sc_blocks.as<int>();
+
+  for (auto& e : m->ev)
+    if (!e) CU(cudaEventCreate(&e));
+  CU(cudaEventRecord(m->ev[0], st));
+  if (!gi_ready) {
+    dim3 grid((3 * H + uis::PBN - 1) / uis::PBN, (unsigned)((rows + uis::PBM - 1) / uis::PBM));
+    uis::input_proj_kernel<<<grid, 256, 0, st>>>(x_dev, m->wih_t.as<float>(), m->bih.as<float>(), m->gi.as<float>(),
+                                                (int)rows, 3 * H, D);
+    CU(cudaGetLastError());
+  }
+  CU(cudaEventRecord(m->ev[1], st));
+  cudaError_t e = cudaSuccess;
+  if (cp.queued > 0) {
+    if (!uis::launch_score_chains(H, D, sp, ctas, st, &e))
+      return fail(UIS_ERR_UNSUPPORTED, "no score kernel for hidden=%d dim=%d", H, D);
+    if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score chain kernel launch failed: %s", cudaGetErrorString(e));
+  }
+  CU(cudaEventRecord(m->ev[2], st));
+  if (!uis::launch_score_first(D, sp, st, &e)) return fail(UIS_ERR_UNSUPPORTED, "no score kernel for dim=%d", D);
+  if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score first-visit kernel launch failed: %s", cudaGetErrorString(e));
+  e = uis::launch_score_reduce(sp, st);
+  if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score reduce kernel launch failed: %s", cudaGetErrorString(e));
+  m->stats.ctas = cp.queued > 0 ? ctas : 0;
+  m->stats.kernel_launches = (gi_ready ? 0 : 1) + (cp.queued > 0 ? 1 : 0) + 2;
+  m->stats_pending = true;
+  return 0;
+}
+
+// Stats of a score call before it runs (the rest is zero; collect() adds the chain kernel's counters and times).
+void begin_score_stats(uis_model* m, int U, long long rows, const ChainPlan& cp, cudaStream_t st) {
+  m->stats = uis_stats{};
+  m->stats.utterances = U;
+  m->stats.frames = rows;
+  m->stats.max_k = cp.max_k;
+  m->stats.engine = 1;
+  m->last_U = U;
+  m->last_score = true;
+  m->last_tree_spill = false;
+  m->last_stream = st;
+  m->stats_pending = false;
+}
+
+int score_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                    const int32_t* const* labels, float* scores_out, float* const* frame_out, cudaStream_t st) {
+  const auto t_begin = std::chrono::steady_clock::now();
+  std::vector<int64_t> off(U + 1, 0);
+  for (int u = 0; u < U; ++u) {
+    if (n_frames[u] < 0) return fail(UIS_ERR_INVALID, "utterance %d: negative length", u);
+    if (n_frames[u] > 0 && (!seqs[u] || !labels[u] || (frame_out && !frame_out[u])))
+      return fail(UIS_ERR_INVALID, "utterance %d: null buffer", u);
+    off[u + 1] = off[u] + n_frames[u];
+  }
+  const long long rows = off[U];
+  std::vector<int32_t> lab((size_t)rows);
+  for (int u = 0; u < U; ++u)
+    if (n_frames[u] > 0) std::memcpy(lab.data() + off[u], labels[u], (size_t)n_frames[u] * 4);
+  ChainPlan cp;
+  if (int rc = plan_chains(lab.data(), off.data(), U, &cp)) return rc;
+  begin_score_stats(m, U, rows, cp, st);
+  std::fill(scores_out, scores_out + U, 0.f);  // empty utterances score 0
+  if (rows == 0) return 0;
+  int n_chunks = 0;
+  bool staged = false;
+  if (int rc = stage_host_rows(m, seqs, U, off.data(), (size_t)rows, st, &n_chunks, &staged)) return rc;
+  if (int rc = m->labels.ensure((size_t)rows * 4)) return rc;
+  CU(cudaMemcpyAsync(m->labels.p, lab.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, st));
+  if (int rc = m->sc_out.ensure(((size_t)U + (frame_out ? (size_t)rows : 0)) * 4)) return rc;
+  float* dev_frames = frame_out ? m->sc_out.as<float>() + U : nullptr;
+  if (int rc = run_score(m, m->x32.as<float>(), off.data(), U, cp, m->labels.as<int32_t>(), m->sc_out.as<float>(),
+                         dev_frames, st, /*gi_ready=*/true))
+    return rc;
+  m->stats.kernel_launches += 2 * (int64_t)n_chunks;
+  m->stats.chunks = n_chunks;
+  m->stats.staged = staged ? 1 : 0;
+  CU(cudaMemcpyAsync(scores_out, m->sc_out.p, (size_t)U * 4, cudaMemcpyDeviceToHost, st));
+  if (frame_out) {
+    CU(cudaMemcpyAsync(lab.data(), dev_frames, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));  // (lab: spent)
+    CU(cudaStreamSynchronize(st));
+    for (int u = 0; u < U; ++u)
+      if (n_frames[u] > 0) std::memcpy(frame_out[u], lab.data() + off[u], (size_t)n_frames[u] * 4);
+  }
+  CU(cudaStreamSynchronize(st));
+  if (int rc = collect(m)) return rc;
+  CU(cudaEventElapsedTime(&m->stats.h2d_ms, m->ev_h2d[0], m->ev_h2d[1]));
+  CU(cudaEventElapsedTime(&m->stats.pipeline_ms, m->ev_pipe, m->ev[1]));
+  m->stats.groups = 1;
+  m->stats.host_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int uis_score(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int32_t* const* labels,
+              float* scores_out, float* const* frame_out, void* stream) {
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  if (U < 0 || (U > 0 && (!seqs || !n_frames || !labels || !scores_out))) return fail(UIS_ERR_INVALID, "null argument");
+  uis::DeviceGuard device_guard_(m->device);
+  CU(device_guard_.status);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int rc = score_host_impl(m, seqs, n_frames, U, labels, scores_out, frame_out, st);
+  if (rc != 0 && rc != UIS_ERR_INVALID) {  // drain what a failed call may have left in flight (see predict_host_group)
+    const std::string keep = g_err;
+    if (m->copy_stream) cudaStreamSynchronize(m->copy_stream);
+    cudaStreamSynchronize(st);
+    (void)cudaGetLastError();
+    g_err = keep;
+  }
+  return rc;
+}
+
+int uis_score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U, const int32_t* labels_dev,
+                     float* scores_dev, float* frame_dev, void* stream) {
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  if (U < 0 || (U > 0 && (!frame_offsets || !scores_dev))) return fail(UIS_ERR_INVALID, "null argument");
+  for (int u = 0; u < U; ++u)
+    if (frame_offsets[u + 1] < frame_offsets[u]) return fail(UIS_ERR_INVALID, "frame_offsets not monotone");
+  const long long rows = U > 0 ? frame_offsets[U] : 0;
+  if (rows > 0 && (!x_dev || !labels_dev)) return fail(UIS_ERR_INVALID, "null device buffer");
+  uis::DeviceGuard device_guard_(m->device);
+  CU(device_guard_.status);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // the chain plan is made on the host: the labels come back first (this synchronises `stream`)
+  std::vector<int32_t> lab((size_t)std::max(rows, 0ll));
+  if (rows > 0) {
+    CU(cudaMemcpyAsync(lab.data(), labels_dev, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+  }
+  ChainPlan cp;
+  if (int rc = plan_chains(lab.data(), frame_offsets, U, &cp)) return rc;
+  begin_score_stats(m, U, rows, cp, st);
+  if (U == 0) return 0;
+  if (rows == 0) {
+    CU(cudaMemsetAsync(scores_dev, 0, (size_t)U * 4, st));  // empty utterances score 0
+    return 0;
+  }
+  if (m->D != m->D_user) {  // zero-pad the caller's rows to the kernel's row length
+    if (int rc = m->x32.ensure((size_t)rows * m->D * 4)) return rc;
+    const size_t np = (size_t)rows * m->D;
+    const int blocks = (int)std::min<size_t>((np + 255) / 256, (size_t)m->num_sms * 16);
+    uis::pad_rows_f32_kernel<<<blocks, 256, 0, st>>>(x_dev, m->x32.as<float>(), (size_t)rows, m->D_user, m->D);
+    CU(cudaGetLastError());
+    x_dev = m->x32.as<float>();
+  }
+  return run_score(m, x_dev, frame_offsets, U, cp, labels_dev, scores_dev, frame_dev, st, /*gi_ready=*/false);
 }
 
 }  // extern "C"

@@ -519,6 +519,51 @@ __device__ __forceinline__ void xch_barrier(XchCtx& x, int tid) {
   x.count += 1;
 }
 
+// weighted_mse_loss (loss_func.py:33-41) of NB mean rows against one frame, by one warp: sum_d fl(fl(diff^2) * w_d)
+// in fp32, lane l taking d = 4 l + 128 i in that order, then a butterfly over the lanes (xor 16, 8, 4, 2, 1); divided
+// by the count of rows whose first squared difference is non-zero (0 -> inf / nan).  m4[q] holds row q's values at the
+// lane's positions (rows with live[q] false are skipped and give 0); xs and wv point at the frame and the weights
+// 1 / (2 sigma2).  Lane q < NB returns row q's term, the other lanes row 0's (the tails run side by side).  The beam
+// kernels and the chain kernel of score() both call this, so a slot's term against a frame has the same bits in both.
+template <int D, int NB>
+__device__ __forceinline__ float gauss_rows(const float4 (&m4)[NB][(D + 127) / 128], const bool (&live)[NB],
+                                            const float* xs, const float* wv, int lane) {
+  float acc[NB], d0sq[NB];
+#pragma unroll
+  for (int q = 0; q < NB; ++q) {
+    acc[q] = 0.f; d0sq[q] = 1.f;
+#pragma unroll
+    for (int i = 0; i < (D + 127) / 128; ++i) {
+      const int d = lane * 4 + i * 128;
+      if (d < D && live[q]) {
+        const float4 x4 = *reinterpret_cast<const float4*>(xs + d);
+        const float4 w4 = *reinterpret_cast<const float4*>(wv + d);
+        const float e0 = __fsub_rn(m4[q][i].x, x4.x), e1 = __fsub_rn(m4[q][i].y, x4.y);
+        const float e2 = __fsub_rn(m4[q][i].z, x4.z), e3 = __fsub_rn(m4[q][i].w, x4.w);
+        const float q0 = __fmul_rn(e0, e0);
+        if (d == 0) d0sq[q] = q0;
+        acc[q] = __fadd_rn(acc[q], __fmul_rn(q0, w4.x));
+        acc[q] = __fadd_rn(acc[q], __fmul_rn(__fmul_rn(e1, e1), w4.y));
+        acc[q] = __fadd_rn(acc[q], __fmul_rn(__fmul_rn(e2, e2), w4.z));
+        acc[q] = __fadd_rn(acc[q], __fmul_rn(__fmul_rn(e3, e3), w4.w));
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {  // interleaved butterfly reductions
+#pragma unroll
+    for (int q = 0; q < NB; ++q) acc[q] = __fadd_rn(acc[q], __shfl_xor_sync(0xffffffffu, acc[q], o));
+  }
+  float my_acc = acc[0], my_d0 = __shfl_sync(0xffffffffu, d0sq[0], 0);
+#pragma unroll
+  for (int q = 1; q < NB; ++q) {
+    const float dq = __shfl_sync(0xffffffffu, d0sq[q], 0);
+    if (lane == q) { my_acc = acc[q]; my_d0 = dq; }
+  }
+  if (my_d0 == 0.f) my_acc = __fdiv_rn(my_acc, 0.f);  // zero "non-zero rows" (loss_func.py:36)
+  return my_acc;
+}
+
 // Per-column context of the current weight pass (shared memory, written in phase P4).
 struct ColCtx {
   const int* lane;  // [Mtot] lane of the column
@@ -1240,44 +1285,16 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
                                 : *reinterpret_cast<const float4*>(mu + lane * 4 + i * 128);
           }
         }
-        float acc[kBatch], d0sq[kBatch];
+        bool live[kBatch];
 #pragma unroll
-        for (int q = 0; q < kBatch; ++q) {
-          acc[q] = 0.f; d0sq[q] = 1.f;
-#pragma unroll
-          for (int i = 0; i < (D + 127) / 128; ++i) {
-            const int d = lane * 4 + i * 128;
-            if (d < D && cslot[q] >= 0) {
-              const float4 x4 = *reinterpret_cast<const float4*>(xs + d);
-              const float4 w4 = *reinterpret_cast<const float4*>(wv + d);
-              const float e0 = __fsub_rn(m4[q][i].x, x4.x), e1 = __fsub_rn(m4[q][i].y, x4.y);
-              const float e2 = __fsub_rn(m4[q][i].z, x4.z), e3 = __fsub_rn(m4[q][i].w, x4.w);
-              const float q0 = __fmul_rn(e0, e0);
-              if (d == 0) d0sq[q] = q0;
-              acc[q] = __fadd_rn(acc[q], __fmul_rn(q0, w4.x));
-              acc[q] = __fadd_rn(acc[q], __fmul_rn(__fmul_rn(e1, e1), w4.y));
-              acc[q] = __fadd_rn(acc[q], __fmul_rn(__fmul_rn(e2, e2), w4.z));
-              acc[q] = __fadd_rn(acc[q], __fmul_rn(__fmul_rn(e3, e3), w4.w));
-            }
-          }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {  // interleaved butterfly reductions
-#pragma unroll
-          for (int q = 0; q < kBatch; ++q) acc[q] = __fadd_rn(acc[q], __shfl_xor_sync(0xffffffffu, acc[q], o));
-        }
-        // lane q finishes slot q (the tails run side by side)
-        float my_acc = acc[0], my_d0 = __shfl_sync(0xffffffffu, d0sq[0], 0);
+        for (int q = 0; q < kBatch; ++q) live[q] = cslot[q] >= 0;
+        const float my_term = gauss_rows<D, kBatch>(m4, live, xs, wv, lane);
+        // lane q stores slot q
         int my_slot = cslot[0];
 #pragma unroll
-        for (int q = 1; q < kBatch; ++q) {
-          const float dq = __shfl_sync(0xffffffffu, d0sq[q], 0);
-          if (lane == q) { my_acc = acc[q]; my_d0 = dq; my_slot = cslot[q]; }
-        }
-        if (lane < kBatch && my_slot >= 0) {
-          if (my_d0 == 0.f) my_acc = __fdiv_rn(my_acc, 0.f);  // zero "non-zero rows" (loss_func.py:36)
-          mse_g[my_slot] = my_acc;
-        }
+        for (int q = 1; q < kBatch; ++q)
+          if (lane == q) my_slot = cslot[q];
+        if (lane < kBatch && my_slot >= 0) mse_g[my_slot] = my_term;
       }
       team_sync();  // the terms are visible to the whole team (ordering of global memory among the team's threads)
       if (ntot <= kSlotList) break;  // (more slots than the list holds: another round over the unlisted ones)

@@ -481,23 +481,13 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
           const bool isnew = (c == Kp);
           const TabEntry en = isnew ? TabEntry{kInitSlot, 0, 0, 0} : lookup(level - 1, par, c, tab, mK);
           const float* mu = pool_mean + (size_t)en.slot * D;
-          float acc = 0.f, d0sq = 1.f;
-          for (int d = lane * 4; d < D; d += 128) {
-            const float4 m4 = *reinterpret_cast<const float4*>(mu + d);
-            const float4 x4 = *reinterpret_cast<const float4*>(xs + d);
-            const float4 w4 = *reinterpret_cast<const float4*>(wv + d);
-            const float e0 = __fsub_rn(m4.x, x4.x), e1 = __fsub_rn(m4.y, x4.y);
-            const float e2 = __fsub_rn(m4.z, x4.z), e3 = __fsub_rn(m4.w, x4.w);
-            const float q0 = __fmul_rn(e0, e0);
-            if (d == 0) d0sq = q0;
-            acc = __fadd_rn(acc, __fmul_rn(q0, w4.x));
-            acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(e1, e1), w4.y));
-            acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(e2, e2), w4.z));
-            acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(e3, e3), w4.w));
-          }
-          acc = warp_sum(acc);
+          float4 m4[1][(D + 127) / 128];
+#pragma unroll
+          for (int i = 0; i < (D + 127) / 128; ++i)
+            if (lane * 4 + i * 128 < D) m4[0][i] = *reinterpret_cast<const float4*>(mu + lane * 4 + i * 128);
+          const bool live[1] = {true};
+          const float acc = gauss_rows<D, 1>(m4, live, xs, wv, lane);
           if (lane == 0) {
-            if (d0sq == 0.f) acc = __fdiv_rn(acc, 0.f);
             double pen;
             if (!isnew) pen = (c == lastp) ? p.log_1mp0 : (p.log_p0 + __ldg(p.logn + en.blocks)) - __ldg(p.logtot + totp);
             else pen = (p.log_p0 + p.log_alpha) - __ldg(p.logtot + totp);

@@ -20,7 +20,7 @@ UIS_ERR_CUDA = -3
 UIS_ERR_OVERFLOW = -4
 UIS_ERR_NOMEM = -5
 UIS_ERR_CAPACITY = -6
-UIS_ABI_VERSION = 6  # include/uisrnn_b200.h
+UIS_ABI_VERSION = 7  # include/uisrnn_b200.h
 
 
 class NativeError(RuntimeError):
@@ -69,7 +69,7 @@ class Stats(C.Structure):
 EXPORTS = ('uis_version', 'uis_last_error', 'uis_model_create', 'uis_model_destroy',
            'uis_model_constants', 'uis_predict', 'uis_predict_device', 'uis_predict_bounded',
            'uis_predict_device_bounded', 'uis_predict_nbest', 'uis_predict_device_nbest',
-           'uis_predict_workspace_bytes', 'uis_get_stats', 'uis_trainer_create',
+           'uis_score', 'uis_score_device', 'uis_predict_workspace_bytes', 'uis_get_stats', 'uis_trainer_create',
            'uis_trainer_destroy', 'uis_trainer_step', 'uis_trainer_get', 'uis_trainer_losses',
            'uis_trainer_comm_size', 'uis_trainer_comm_export', 'uis_trainer_comm_apply',
            'uis_trainer_set_corpus', 'uis_trainer_step_corpus')
@@ -164,6 +164,12 @@ def load_library():
   lib.uis_predict_device_nbest.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int,
                                            C.POINTER(PredictOpts), C.POINTER(DebugTaps), C.c_void_p, ip, ip,
                                            C.c_int32, C.POINTER(NBestOut)]
+  lib.uis_score.restype = C.c_int
+  lib.uis_score.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int, C.POINTER(C.c_void_p),
+                            fp, C.POINTER(C.c_void_p), C.c_void_p]
+  lib.uis_score_device.restype = C.c_int
+  lib.uis_score_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p]
   lib.uis_predict_workspace_bytes.restype = C.c_size_t
   lib.uis_predict_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.c_int,
                                               C.POINTER(PredictOpts)]
@@ -416,6 +422,42 @@ class NativeModel:
                                               mn.ctypes.data_as(ip) if mn is not None else None,
                                               C.c_void_p(speakers_ptr))
     _check(self._lib, rc)
+
+  def score(self, seqs, labels, per_frame=False):
+    """neg_likelihood of given labellings (uis_score): seqs is a list of float64 [N_u, D] arrays (host), labels a
+    list of canonical int label sequences (0, 1, 2, ... in order of first appearance), one of length N_u per
+    utterance.  Returns float32 scores [U]; with per_frame, (scores, list of float32 [N_u] per-frame increments)."""
+    if not isinstance(seqs, (list, tuple)) or not isinstance(labels, (list, tuple)):
+      raise TypeError('seqs and labels must be lists')
+    if len(seqs) != len(labels):
+      raise ValueError('{} utterances but {} label sequences'.format(len(seqs), len(labels)))
+    n = len(seqs)
+    keep = [s if (type(s) is np.ndarray and s.dtype == np.float64 and s.flags.c_contiguous)
+            else np.ascontiguousarray(s, dtype=np.float64) for s in seqs]
+    labs = [np.ascontiguousarray(l, dtype=np.int32) for l in labels]
+    for u, (s, l) in enumerate(zip(keep, labs)):
+      if s.ndim != 2 or s.shape[1] != self.D:
+        raise ValueError('utterance shape {} does not match D={}'.format(s.shape, self.D))
+      if l.ndim != 1 or len(l) != s.shape[0]:
+        raise ValueError('utterance {}: {} labels for {} frames'.format(u, l.size, s.shape[0]))
+    lens = np.array([s.shape[0] for s in keep] or [0], np.int64)
+    scores = np.zeros(max(n, 1), np.float32)
+    frames = [np.empty(s.shape[0], np.float32) for s in keep] if per_frame else None
+    ptrs = lambda arrs: (C.c_void_p * max(len(arrs), 1))(*[a.ctypes.data for a in arrs])
+    _check(self._lib, self._lib.uis_score(
+        self._h, C.cast(ptrs(keep), C.POINTER(C.c_void_p)), lens.ctypes.data_as(C.POINTER(C.c_int64)), n,
+        C.cast(ptrs(labs), C.POINTER(C.c_void_p)), scores.ctypes.data_as(C.POINTER(C.c_float)),
+        C.cast(ptrs(frames), C.POINTER(C.c_void_p)) if per_frame else None, None))
+    return (scores[:n], frames) if per_frame else scores[:n]
+
+  def score_device(self, x_ptr, frame_offsets, labels_ptr, scores_ptr, frame_ptr=0, stream=0):
+    """Device-resident variant (uis_score_device): x_ptr -> fp32 [rows, D], labels_ptr -> canonical int32 [rows],
+    scores_ptr -> float32 [U], frame_ptr -> float32 [rows] per-frame increments (0 = none); raw device addresses.
+    Reads the labels back once to plan the chains, then enqueues the kernels on `stream` without waiting."""
+    off = np.ascontiguousarray(frame_offsets, dtype=np.int64)
+    _check(self._lib, self._lib.uis_score_device(
+        self._h, C.c_void_p(x_ptr), off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1, C.c_void_p(labels_ptr),
+        C.c_void_p(scores_ptr), C.c_void_p(frame_ptr), C.c_void_p(stream)))
 
   def stats(self):
     s = Stats()

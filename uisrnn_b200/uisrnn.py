@@ -30,6 +30,9 @@ _INITIAL_SIGMA2_VALUE = 0.1
 # One utterance's N-best result (predict(..., n_best=k)): up to k hypotheses in rank order -- their label lists (the
 # last tiled copy), their neg_likelihood over the whole decode and their cluster counts.
 NBest = collections.namedtuple('NBest', ['labels', 'scores', 'speakers'])
+# One utterance's score(..., per_frame=True): the neg_likelihood of the labelling and its per-frame increments (float32
+# ndarray [N]; summed in fp32 in frame order they give `total` bit for bit).
+FrameScores = collections.namedtuple('FrameScores', ['total', 'increments'])
 
 _DEFAULT_KCAP = 0  # clusters per hypothesis held in device tables: 0 = the library's default (16 or 32, by kernel); grown on overflow
 
@@ -517,6 +520,52 @@ class UISRNN:
         return self._predict_cuda(test_sequences, args)
       return [self.predict_single(sequence, args) for sequence in test_sequences]
     raise TypeError('test_sequences should be either a list or numpy array.')
+
+  def score(self, test_sequences, test_cluster_ids, *, per_frame=False):
+    """The neg_likelihood the model gives to given speaker labellings (not in the reference, where it exists only
+    inside the beam search): the score of the trace that assigns frame t to cluster test_cluster_ids[t], the same
+    quantity as `NBest.scores` -- lower is better.  Scoring the ground truth against the decoded hypothesis tells a
+    search error (the truth scores lower) from a model error.
+
+    One sequence (float64 ndarray [N, D], validated as in `predict`) with one label sequence (N hashable values) gives
+    a float; a list of sequences with a list of label sequences gives a list of floats.  Labels are taken up to
+    renaming: they are mapped to 0, 1, 2, ... in order of first appearance.  test_iteration is not applied: the
+    sequence is scored once, as given (tile both the sequence and its labels to score a tiled decode).  An empty
+    sequence scores 0.  With per_frame=True every utterance gives a `FrameScores(total, increments)` instead.  On a
+    CUDA device a list is scored by one native call."""
+    if isinstance(test_sequences, np.ndarray):
+      return self.score([test_sequences], [test_cluster_ids], per_frame=per_frame)[0]
+    if not isinstance(test_sequences, list):
+      raise TypeError('test_sequences should be either a list or numpy array.')
+    if not isinstance(test_cluster_ids, (list, tuple)):
+      raise TypeError('test_cluster_ids should be a list with one label sequence per sequence.')
+    if len(test_cluster_ids) != len(test_sequences):
+      raise ValueError('{} sequences but {} label sequences'.format(len(test_sequences), len(test_cluster_ids)))
+    for sequence in test_sequences:
+      _check_test_sequence(sequence, self.observation_dim)
+    labels = [canonical_labels(ids) for ids in test_cluster_ids]
+    for u, (sequence, lab) in enumerate(zip(test_sequences, labels)):
+      if len(lab) != len(sequence):
+        raise ValueError('utterance {}: {} labels for {} frames'.format(u, len(lab), len(sequence)))
+    if self.device.type == 'cuda':
+      model = self._native_model()
+      with model.lock:
+        out = model.score(test_sequences, labels, per_frame=per_frame)
+      if not per_frame:
+        return [float(v) for v in out]
+      return [FrameScores(float(v), inc) for v, inc in zip(*out)]
+    decoder = beam_cpu.CpuBeamSearch(self)
+    out = [decoder.score(sequence, lab) for sequence, lab in zip(test_sequences, labels)]
+    return [FrameScores(float(t), inc) for t, inc in out] if per_frame else [float(t) for t, _ in out]
+
+
+def canonical_labels(ids):
+  """int32 ndarray of a label sequence renamed to 0, 1, 2, ... in order of first appearance (any hashable values)."""
+  if isinstance(ids, (str, bytes)) or np.ndim(ids) > 1:
+    raise ValueError('a label sequence must be a 1-D sequence of labels')
+  seen = {}
+  return np.fromiter((seen.setdefault(v.item() if isinstance(v, np.generic) else v, len(seen)) for v in ids),
+                     dtype=np.int32, count=len(ids))
 
 
 def _speaker_bounds(n, max_speakers, min_speakers):
