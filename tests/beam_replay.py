@@ -392,13 +392,40 @@ def _check(replay, inc_rtol, labels, final, state_tol, worst, visit):
   return labs
 
 
+def frame_allowance(inc, gauss, inc_rtol=INC_RTOL):
+  """How far a kernel's fp32 per-frame increment may lie from the float64 one: one fp32 ulp of the increment (its final
+  rounding) plus inc_rtol times the frame's Gaussian term.  Beyond that rounding the only error of an increment is the
+  fp32 weighted mse (the log terms are float64), so the bound scales with the Gaussian term, not with the increment,
+  which cancellation against the log terms can make small."""
+  with np.errstate(invalid='ignore'):
+    return ulp32(inc) + inc_rtol * np.asarray(gauss, np.float64)
+
+
+def frame_share(got, inc, gauss, inc_rtol=INC_RTOL):
+  """|got - inc| / frame_allowance per frame (<= 1 within it; 0 where equal, +inf included; +inf where exactly one of
+  the two is +inf)."""
+  got, inc = np.asarray(got, np.float64), np.asarray(inc, np.float64)
+  with np.errstate(invalid='ignore', divide='ignore'):
+    share = np.abs(got - inc) / frame_allowance(inc, gauss, inc_rtol)
+  return np.where(got == inc, 0.0, np.where(np.isnan(share), np.inf, share))
+
+
 class PathScores:
   """What path_score returns, per path: `score`, the float64 neg_likelihood; and the two parts of the allowance an
   fp32 accumulation of the same path may differ by, as check() bounds each step: `ulps`, one fp32 ulp of the running
-  score per sub-step, and `mass`, the sum of |increment| (the part INC_RTOL scales).  Absent paths are nan."""
+  score per sub-step, and `mass`, the sum of |increment| (the part INC_RTOL scales).  Absent paths are nan.
 
-  def __init__(self, score, ulps, mass):
+  With path_score(per_frame=True), also per path (lists in the same order, None for an absent path): `frame_inc`, the
+  float64 increment of every frame, and `frame_gauss`, its Gaussian term (the weighted mse; +inf under the
+  first-column rule)."""
+
+  def __init__(self, score, ulps, mass, frame_inc=None, frame_gauss=None):
     self.score, self.ulps, self.mass = score, ulps, mass
+    self.frame_inc, self.frame_gauss = frame_inc, frame_gauss
+
+  def frame_share(self, got, inc_rtol=INC_RTOL):
+    """frame_share of every path's fp32 per-frame increments in `got` (a list in path order): a list of arrays."""
+    return [frame_share(g, i, s, inc_rtol) for g, i, s in zip(got, self.frame_inc, self.frame_gauss)]
 
   def allowance(self, inc_rtol=INC_RTOL):
     return self.ulps + inc_rtol * self.mass
@@ -411,7 +438,7 @@ class PathScores:
       return np.where(err == 0, 0.0, err / self.allowance(inc_rtol))
 
 
-def path_score(model, xs, labels, mean0=None, device='cpu', max_slots=1 << 17):
+def path_score(model, xs, labels, mean0=None, device='cpu', max_slots=1 << 17, per_frame=False):
   """Float64 rescoring of given label paths: the neg_likelihood the search assigns to a hypothesis whose cluster at
   frame t is labels[t], summed over the frames with the score terms of Replay (running-mean off-by-one, log-term
   association, first-column rule; `mean0`, the kernel's fp32 mean0, decides that rule exactly for new clusters).
@@ -419,9 +446,10 @@ def path_score(model, xs, labels, mean0=None, device='cpu', max_slots=1 << 17):
     xs      list of [N_u, D] inputs, already tiled (np.tile(x, (test_iteration, 1))) when the path covers the tiling
     labels  list of int [R_u, N_u]: R_u paths over utterance u; a row of -1 is an absent rank (nan scores)
 
-  Returns a PathScores of arrays [sum R_u] in (utterance, row) order.  A path is its labels only at look_ahead 1 or
-  any look_ahead (the sub-steps of a tree step add the same per-frame increments), but only over the whole tiled
-  decode: predict() returns the last tiled copy, which at test_iteration > 1 leaves the earlier copies' labels, and so
+  Returns a PathScores of arrays [sum R_u] in (utterance, row) order; per_frame=True adds every path's float64
+  per-frame increments and Gaussian terms (PathScores.frame_inc / frame_gauss).  A path is its labels only at
+  look_ahead 1 or any look_ahead (the sub-steps of a tree step add the same per-frame increments), but only over the
+  whole tiled decode: predict() returns the last tiled copy, which at test_iteration > 1 leaves the earlier copies' labels, and so
   every cluster's state, undetermined.  Rescore those from the back-track of a trace instead.
 
   Batched in torch float64 on `device`: one GRU product per frame over every path of every utterance, each cluster
@@ -435,6 +463,7 @@ def path_score(model, xs, labels, mean0=None, device='cpu', max_slots=1 << 17):
   assert all(r.shape[1] == len(x) for x, r in zip(xs, rows)), 'labels and inputs of different lengths'
   first = np.concatenate([[0], np.cumsum([len(r) for r in rows])]).astype(np.int64)
   out = [np.full(int(first[-1]), np.nan) for _ in range(3)]
+  frames = [[None] * int(first[-1]) for _ in range(2)] if per_frame else None  # increments, Gaussian terms
   w = torch.as_tensor(m.w, **f64)
   mean0_64 = torch.as_tensor(m.mean0, **f64)
   hidden0 = torch.as_tensor(m.hidden0, **f64)
@@ -481,6 +510,8 @@ def path_score(model, xs, labels, mean0=None, device='cpu', max_slots=1 << 17):
       last = torch.full((P,), -1, dtype=torch.int64, device=dev)
       tot = torch.zeros(P, **f64)
       score, ulps, mass = torch.zeros(P, **f64), torch.zeros(P, **f64), torch.zeros(P, **f64)
+      if per_frame:
+        f_inc, f_gauss = torch.zeros((P, lab.shape[1]), **f64), torch.zeros((P, lab.shape[1]), **f64)
       next_id = 0
       for t in range(int(n_p.max())):
         live = torch.nonzero(n_t > t).squeeze(1)
@@ -506,6 +537,9 @@ def path_score(model, xs, labels, mean0=None, device='cpu', max_slots=1 << 17):
                           torch.where(c == last[live], torch.full_like(lt, m.pen_last),
                                       (m.log_p0 + torch.log(blocks[slot])) - lt))
         inc = mse - pen
+        if per_frame:
+          f_inc[live, t] = inc
+          f_gauss[live, t] = mse
         s = score[live] + inc
         score[live] = s
         a = s.abs().float()
@@ -534,4 +568,8 @@ def path_score(model, xs, labels, mean0=None, device='cpu', max_slots=1 << 17):
       idx = np.array([first[u] + j for u, j in paths], np.int64)
       for o, v in zip(out, (score, ulps, mass)):
         o[idx] = v.cpu().numpy()
-  return PathScores(*out)
+      if per_frame:
+        for o, v in zip(frames, (f_inc.cpu().numpy(), f_gauss.cpu().numpy())):
+          for p, i in enumerate(idx):
+            o[i] = v[p, :n_p[p]]
+  return PathScores(*out, *(frames or ()))
