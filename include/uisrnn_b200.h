@@ -258,6 +258,56 @@ int uis_score(uis_model* m, const double* const* seqs, const int64_t* n_frames, 
 int uis_score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
                      const int32_t* labels_dev, float* scores_dev, float* frame_dev, void* stream);
 
+/*
+ * Decoding-parameter sweeps (same ABI version 7; additive).  Not in the reference, which decodes with the model's
+ * crp_alpha (--crp_alpha) and transition_bias only.  One call decodes or scores a list under `count` (crp_alpha,
+ * transition_bias) pairs: config c gives exactly what the plain call returns for a model created with pair c.  The
+ * input rows cross the bus once and their input projection runs once; the kernels run U * count independent jobs,
+ * job j = utterance j % U under config j / U (the configs of one utterance are scheduled side by side).
+ *   params       count >= 1, U * count <= INT_MAX, every crp_alpha finite and > 0, every transition_bias finite and in
+ *                (0, 1); anything else is UIS_ERR_INVALID and uis_last_error() names the pair.  Host arrays, read
+ *                during the call only.
+ * uis_predict_sweep / uis_predict_device_sweep take the arguments of uis_predict_nbest / uis_predict_device_nbest
+ * (speaker bounds per utterance, the same for every config) and write config-major outputs, config c's block being
+ * what the N-best call writes:
+ *   host labels    labels_out[u] -> int32 [count][n_best][n_frames[u]]
+ *   device labels  labels_dev    -> int32 [count][n_best][frame_offsets[U]]
+ *   scores, speakers [count][U][n_best];  count [count][U]
+ * uis_score_sweep / uis_score_device_sweep take the arguments of uis_score / uis_score_device: scores [count][U];
+ * per-frame increments frame_out[u] -> float32 [count][n_frames[u]] (host) or frame_dev -> [count][frame_offsets[U]]
+ * (device).  The chain kernel and the first-visit kernel run once; the reduce kernel runs once per config.
+ * Debug taps index jobs: trace_utt = c * U + u, final_scores [count * U][beam_size], final_k [count * U].
+ * uis_get_stats after a sweep: utterances = jobs (U * count), frames = distinct input rows; the work counters cover
+ * every job (a score sweep's gru_columns equal a plain score call's).  The host-buffer predict sweep decodes a list
+ * that does not fit the device in groups of whole utterances, each with all its configs; a score sweep that does not
+ * fit fails with UIS_ERR_NOMEM.
+ * Synchronisation: the log tables of a sweep are built on the host and cached in the handle.  A sweep whose pairs (or
+ * longest tiled decode) differ from the previous sweep's rewrites them in place, and first synchronises the DEVICE
+ * (cudaDeviceSynchronize: an earlier call on any stream may still read them), so uis_predict_device_sweep /
+ * uis_score_device_sweep block in that case; a sweep that repeats the previous sweep's pairs enqueues without waiting.
+ * The tables of the model's own pair, which the plain entry points use, are kept apart and never rewritten by a sweep.
+ */
+typedef struct uis_decode_params {
+  int32_t count;
+  const double* crp_alpha;        /* [count] */
+  const double* transition_bias;  /* [count] */
+} uis_decode_params;
+
+int uis_predict_sweep(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                      const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                      const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                      const uis_nbest_out* out, const uis_decode_params* params);
+int uis_predict_device_sweep(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                             const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                             const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                             const uis_nbest_out* out, const uis_decode_params* params);
+int uis_score_sweep(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                    const int32_t* const* labels, float* scores_out, float* const* frame_out, void* stream,
+                    const uis_decode_params* params);
+int uis_score_device_sweep(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                           const int32_t* labels_dev, float* scores_dev, float* frame_dev, void* stream,
+                           const uis_decode_params* params);
+
 /* Device bytes uis_predict_device() will hold for this problem (workspace is cached in the handle). */
 size_t uis_predict_workspace_bytes(uis_model* m, const int64_t* frame_offsets, int U,
                                    const uis_predict_opts* opts);

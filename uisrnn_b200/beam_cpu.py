@@ -38,15 +38,17 @@ class _Hypothesis:
 
 
 class CpuBeamSearch:
-  """Decoder bound to one UISRNN model (weights are read at construction)."""
+  """Decoder bound to one UISRNN model (weights are read at construction).  crp_alpha / transition_bias, when given,
+  replace the model's values (a decoding-parameter sweep); the model is not changed."""
 
-  def __init__(self, model):
+  def __init__(self, model, crp_alpha=None, transition_bias=None):
     self.rnn = model.rnn_model
     self.device = model.device
-    self.log_p0 = np.log(model.transition_bias)
-    self.log_1mp0 = np.log(1 - model.transition_bias)
-    self.alpha = model.crp_alpha
-    self.log_alpha = np.log(model.crp_alpha)
+    p0 = model.transition_bias if transition_bias is None else transition_bias
+    self.alpha = model.crp_alpha if crp_alpha is None else crp_alpha
+    self.log_p0 = np.log(p0)
+    self.log_1mp0 = np.log(1 - p0)
+    self.log_alpha = np.log(self.alpha)
     self.rnn.eval()  # (mean0 / hidden0 below: no dropout between stacked layers, as in decode)
     with torch.no_grad():
       self.weight = (1 / (2 * model.sigma2)).detach()

@@ -155,9 +155,15 @@ struct uis_model {
   alignas(64) CUtensorMap tc_map;
   bool tc_ready = false;
   float tc_sh = 0, tc_sa = 0, tc_inv_hh = 0, tc_inv_1 = 0, tc_inv_2 = 0;
-  // log tables
-  DevBuf logn, logtot;
+  // log tables: logn [log_cap] is shared; the decoding-parameter tables (LogTables) of the model's own values and of
+  // the last sweep are kept apart, so that a sweep never rebuilds the tables of a plain call
+  DevBuf logn;
   int log_cap = 0;
+  struct LogTables {
+    DevBuf tot, cfg;          // [configs][cap] log(i + crp_alpha); [configs][3] log(p0), log(1 - p0), log(crp_alpha)
+    std::vector<double> key;  // (crp_alpha, transition_bias) of every config the tables hold
+    int cap = 0;
+  } own_logs, sweep_logs;
   // workspace
   DevBuf x64, x32, gi, row_off, order, pool_mean, pool_hidden, pool_mse, bp, queue_stats, labels, status;
   DevBuf spk_bound, spk_out;  // bounded calls only: [U][2] speaker bounds; [U] speaker counts (host-buffer entry point)
@@ -360,17 +366,71 @@ int tc_prepare(uis_model* m, const std::vector<float>& w_hh, const std::vector<f
   return 0;
 }
 
-int ensure_log_tables(uis_model* m, int max_tn) {
+// The decoding parameters of a call: `count` (crp_alpha, transition_bias) pairs.  A call without a sweep decodes the
+// model's own pair.
+struct DecodeParams {
+  int count = 1;
+  const double* alpha = nullptr;
+  const double* p0 = nullptr;
+};
+
+DecodeParams model_decode(const uis_model* m) { return DecodeParams{1, &m->alpha, &m->p0}; }
+
+// Rejects a sweep the kernels cannot run: no pairs, more than INT_MAX jobs, or a value out of range.
+int check_decode(const uis_decode_params* dp, int U, DecodeParams* out) {
+  if (!dp) return fail(UIS_ERR_INVALID, "decode_params is NULL");
+  if (dp->count < 1) return fail(UIS_ERR_INVALID, "decode_params: count=%d (need >= 1)", dp->count);
+  if (!dp->crp_alpha || !dp->transition_bias) return fail(UIS_ERR_INVALID, "decode_params: null value array");
+  if ((long long)std::max(U, 1) * dp->count > std::numeric_limits<int>::max())
+    return fail(UIS_ERR_INVALID, "decode_params: %d utterances x %d pairs exceeds INT_MAX jobs", U, dp->count);
+  for (int c = 0; c < dp->count; ++c) {
+    const double a = dp->crp_alpha[c], b = dp->transition_bias[c];
+    if (!(std::isfinite(a) && a > 0.0))
+      return fail(UIS_ERR_INVALID, "decode_params pair %d: crp_alpha=%g (need finite and > 0)", c, a);
+    if (!(std::isfinite(b) && b > 0.0 && b < 1.0))
+      return fail(UIS_ERR_INVALID, "decode_params pair %d: transition_bias=%g (need finite and in (0, 1))", c, b);
+  }
+  *out = DecodeParams{dp->count, dp->crp_alpha, dp->transition_bias};
+  return 0;
+}
+
+// Log tables for decodes of up to max_tn frames under `dp`, built on the host with std::log so that a config's values
+// are those a model created with its pair uses.  Fills the table pointers of `p`.
+int ensure_log_tables(uis_model* m, int max_tn, const DecodeParams& dp, uis::BeamParams* p) {
   const int need = max_tn + 2;
-  if (need <= m->log_cap) return 0;
-  const int cap = std::max(need, 4096);
-  std::vector<double> ln(cap), lt(cap);
-  ln[0] = -INFINITY;
-  for (int i = 1; i < cap; ++i) ln[i] = std::log((double)i);             // np.log(block_counts[c])
-  for (int i = 0; i < cap; ++i) lt[i] = std::log((double)i + m->alpha);  // np.log(sum(block_counts) + alpha)
-  if (int rc = upload(m->logn, ln.data(), cap * sizeof(double))) return rc;
-  if (int rc = upload(m->logtot, lt.data(), cap * sizeof(double))) return rc;
-  m->log_cap = cap;
+  if (need > m->log_cap) {
+    const int cap = std::max(need, 4096);
+    std::vector<double> ln(cap);
+    ln[0] = -INFINITY;
+    for (int i = 1; i < cap; ++i) ln[i] = std::log((double)i);  // np.log(block_counts[c])
+    if (int rc = upload(m->logn, ln.data(), cap * sizeof(double))) return rc;
+    m->log_cap = cap;
+  }
+  const bool own = dp.alpha == &m->alpha;
+  uis_model::LogTables& t = own ? m->own_logs : m->sweep_logs;
+  std::vector<double> key;
+  for (int c = 0; c < dp.count; ++c) { key.push_back(dp.alpha[c]); key.push_back(dp.p0[c]); }
+  if (need > t.cap || key != t.key) {
+    const int cap = std::max({need, 4096, t.cap});
+    if (t.cap) CU(cudaDeviceSynchronize());  // the tables are rewritten in place: no earlier call may still read them
+    std::vector<double> lt((size_t)dp.count * cap), cv((size_t)dp.count * 3);
+    for (int c = 0; c < dp.count; ++c) {
+      for (int i = 0; i < cap; ++i) lt[(size_t)c * cap + i] = std::log((double)i + dp.alpha[c]);  // np.log(sum(block_counts) + alpha)
+      cv[3 * c] = std::log(dp.p0[c]);            // np.log(self.transition_bias)      uisrnn.py:418
+      cv[3 * c + 1] = std::log(1.0 - dp.p0[c]);  // np.log(1 - self.transition_bias)  uisrnn.py:416
+      cv[3 * c + 2] = std::log(dp.alpha[c]);     // np.log(self.crp_alpha)            uisrnn.py:445
+    }
+    t.cap = 0;
+    t.key.clear();
+    if (int rc = upload(t.tot, lt.data(), lt.size() * sizeof(double))) return rc;
+    if (int rc = upload(t.cfg, cv.data(), cv.size() * sizeof(double))) return rc;
+    t.cap = cap;
+    t.key = key;
+  }
+  p->logn = m->logn.as<double>();
+  p->logtot = t.tot.as<double>();
+  p->cfg_log = t.cfg.as<double>();
+  p->logtot_stride = t.cap;
   return 0;
 }
 
@@ -441,7 +501,8 @@ void plan_tree_spill(uis_model* m, Plan* pl) {
   pl->spill_budget = budget;
 }
 
-int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o, Plan* pl) {
+// U utterances (rows, frame counts) decoded as U * configs jobs (engine, lanes, CTAs and latency modes).
+int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o, Plan* pl, int configs = 1) {
   if (!m || !o || (U > 0 && !off)) return fail(UIS_ERR_INVALID, "null argument");
   if (U < 0) return fail(UIS_ERR_INVALID, "U < 0");
   if (o->beam_size < 1 || o->look_ahead < 1 || o->test_iteration < 1)
@@ -471,10 +532,11 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
     maxN = std::max<long long>(maxN, n);
   }
   pl->maxN = std::max(maxN, 1);
+  const long long J = (long long)U * configs;  // jobs
   int ctas = o->n_ctas > 0 ? o->n_ctas : m->num_sms;
   // lanes (utterances advanced together by one CTA, sharing each weight pass): 2 when there is
   // enough work to keep every CTA's lanes busy, else 1 (latency mode); opts->lanes overrides.
-  int G = o->lanes > 0 ? std::min(o->lanes, 4) : ((long long)U >= 2ll * ctas ? 2 : 1);
+  int G = o->lanes > 0 ? std::min(o->lanes, 4) : (J >= 2ll * ctas ? 2 : 1);
   if (tree) {
     // look-ahead tree kernel: one utterance per CTA; size the on-chip node / leaf arrays to what
     // shared memory allows (internal nodes : leaves ~ 1 : 8, the typical fan-out K+2)
@@ -505,12 +567,12 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
       if (uis::beam_tc_supported(m->H, m->D, N)) {
         const int kc = o->kcap > 0 ? o->kcap : 16;
         int Gt = o->lanes > 0 ? std::min(o->lanes, (int)uis::kMaxLanes)
-                              : (int)std::min<long long>(N / 8, ((long long)U + ctas - 1) / std::max(ctas, 1));
+                              : (int)std::min<long long>(N / 8, (J + ctas - 1) / std::max(ctas, 1));
         Gt = std::max(Gt, 1);
         while (Gt > 1 && (uis::beam_tc_smem(m->H, m->D, N, pl->B, kc, Gt) > 227u * 1024u || Gt * pl->B > 256)) --Gt;
         const bool fits = uis::beam_tc_smem(m->H, m->D, N, pl->B, kc, Gt) <= 227u * 1024u &&
                           pl->B * kc + pl->B + 1 <= 65535;
-        if (fits && (o->engine == 2 || (long long)U > ctas)) {
+        if (fits && (o->engine == 2 || J > ctas)) {
           pl->tcn = N;
           pl->Kcap = kc;
           pl->P = pl->B * kc + pl->B + 1;
@@ -530,7 +592,7 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
   }
   if (tree && o->engine == 2) return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: look_ahead must be 1");
   pl->G = G;
-  pl->ctas = std::max(1, std::min(ctas, std::max((U + G - 1) / G, 1)));
+  pl->ctas = (int)std::max(1ll, std::min<long long>(ctas, std::max((J + G - 1) / G, 1ll)));
   if (tree) plan_tree_spill(m, pl);
   // Cluster (latency) mode: with fewer utterances than SMs, a thread-block cluster of 2/4/8 CTAs works on
   // each utterance (k-split of every weight matrix, uis_beam.cuh).  opts->cluster: 0 = auto (largest of 4, 2
@@ -545,12 +607,12 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
       o->lanes <= 1 && o->engine != 2) {
     const char* env = std::getenv("UISRNN_B200_STAT");
     const bool want = o->cluster == uis::kStatGroup ||
-                      (!(env && env[0] == '0') && (long long)U * uis::kStatGroup <= ctas && o->engine == 0 && o->n_ctas <= 0);
+                      (!(env && env[0] == '0') && J * uis::kStatGroup <= ctas && o->engine == 0 && o->n_ctas <= 0);
     const int kc = o->kcap > 0 ? o->kcap : 32;
     const bool can = ctas >= uis::kStatGroup && uis::beam_stat_smem(m->H, m->D, pl->B, kc) <= 227u * 1024u &&
                      pl->B * kc + pl->B + 1 <= 65535;
     if (want && can) {
-      pl->stat = std::max(1, std::min(ctas / uis::kStatGroup, U));
+      pl->stat = (int)std::max(1ll, std::min<long long>(ctas / uis::kStatGroup, J));
       pl->stat_forced = o->cluster == uis::kStatGroup;
       pl->tcn = 0;
       pl->Kcap = kc;
@@ -570,12 +632,12 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
       const char* env = std::getenv("UISRNN_B200_CLUSTER");
       if (!(env && env[0] == '0'))
         for (int c : {4, 2})
-          if ((long long)U * c <= ctas) { cs = c; break; }
+          if (J * c <= ctas) { cs = c; break; }
     } else {
       return fail(UIS_ERR_INVALID, "cluster must be -1, 0, 2, 4, 8 or 32");
     }
     if (cs > 1 && uis::beam_cluster_smem(m->H, m->D, pl->B, pl->Kcap) <= 227u * 1024u) {
-      const int clusters = std::max(1, std::min(ctas / cs, U));
+      const int clusters = (int)std::max(1ll, std::min<long long>(ctas / cs, J));
       pl->cluster = cs;
       pl->cluster_forced = o->cluster > 0;
       pl->G = 1;
@@ -587,13 +649,15 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
   return 0;
 }
 
-size_t workspace_bytes(const uis_model* m, const Plan& pl, int U) {
+size_t workspace_bytes(const uis_model* m, const Plan& pl, int U, int configs = 1) {
+  const size_t J = (size_t)U * configs;
   size_t b = 0;
   b += (size_t)pl.rows * 3 * m->H * 4;                                  // gi
   b += pool_slots(pl) * (m->D + m->depth * m->H + 1) * 4;            // slot pools (+ Gaussian term per slot)
   b += (size_t)pl.spill_ctas * pl.spill_arena;                          // look-ahead spill arenas
   b += (size_t)pl.ctas * pl.G * (pl.L > 1 ? (size_t)pl.maxTN + pl.maxSteps : (size_t)pl.maxN) * pl.B * 4;  // back-pointers
-  b += (size_t)(U + 1) * 8 + (size_t)U * 8 + 256;                       // offsets, order, status
+  b += (size_t)(U + 1) * 8 + J * 8 + 256;                               // offsets, order, status
+  if (configs > 1) b += (size_t)configs * (4096 + 3) * 8;               // log tables of the sweep (at least)
   if (pl.tcn) b += (size_t)pl.ctas * pl.tcn * m->H * 4;                 // a = relu(W1 h' + b1) between two products
   return b;
 }
@@ -614,10 +678,6 @@ struct NBestOut {
   float* scores = nullptr;     // [U][k]
   int32_t* speakers = nullptr; // [U][k]
   int32_t* count = nullptr;    // [U]
-  NBestOut at(int u0) const {
-    return NBestOut{k, scores ? scores + (size_t)u0 * k : nullptr, speakers ? speakers + (size_t)u0 * k : nullptr,
-                    count ? count + u0 : nullptr};
-  }
 };
 
 int check_bounds(int U, const int32_t* mx, const int32_t* mn) {
@@ -641,13 +701,13 @@ int check_nbest(int n_best, const uis_predict_opts* opts, const uis_nbest_out* o
 int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
                         const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
                         const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev,
-                        const NBestOut& nb);
+                        const NBestOut& nb, const DecodeParams* dp = nullptr);
 int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
                       const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
                       const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out,
-                      const NBestOut& nb);
+                      const NBestOut& nb, const DecodeParams* dp = nullptr);
 
-// The model's part of the kernel parameters: weights, constants, log terms and log tables (ensure_log_tables first).
+// The model's part of the kernel parameters: weights and constants (ensure_log_tables adds the log terms).
 uis::BeamParams model_params(const uis_model* m) {
   const int H = m->H;
   uis::BeamParams p{};
@@ -661,34 +721,34 @@ uis::BeamParams model_params(const uis_model* m) {
   p.bhh_up = m->bhh.as<float>() + 3 * H;
   p.bhh = m->bhh.as<float>(); p.b1 = m->b1.as<float>(); p.b2 = m->b2.as<float>();
   p.wvec = m->wvec.as<float>(); p.mean0 = m->mean0.as<float>(); p.hidden0 = m->hidden0.as<float>();
-  p.log_p0 = std::log(m->p0);          // np.log(self.transition_bias)      uisrnn.py:418
-  p.log_1mp0 = std::log(1.0 - m->p0);  // np.log(1 - self.transition_bias)  uisrnn.py:416
-  p.log_alpha = std::log(m->alpha);    // np.log(self.crp_alpha)            uisrnn.py:445
-  p.logn = m->logn.as<double>(); p.logtot = m->logtot.as<double>();
   return p;
 }
 
+// Decodes U utterances under dp.count configs: J = U * dp.count jobs, job j = utterance j % U under config j / U.
+// Per-job outputs (status, N-best scores / speakers / counts, taps) are [J]; labels_dev holds dp.count * nb.k planes
+// of the call's rows (plane c * nb.k + j: config c, hypothesis j).
 int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, const Plan& pl, int32_t* labels_dev,
                const uis_debug_taps* taps, cudaStream_t st, const SpeakerBounds& sb, const NBestOut& nb,
-               bool gi_ready = false) {
+               const DecodeParams& dp, bool gi_ready = false) {
   const int H = m->H, D = m->D;
-  if (sb.out_dev && U > 0) CU(cudaMemsetAsync(sb.out_dev, 0, (size_t)U * sizeof(int32_t), st));  // empty inputs: 0
+  const int J = U * dp.count;
+  if (sb.out_dev && U > 0) CU(cudaMemsetAsync(sb.out_dev, 0, (size_t)J * sizeof(int32_t), st));  // empty inputs: 0
   if (U > 0 && pl.rows == 0) {  // no kernel runs: every utterance is empty and returns no hypothesis
-    if (nb.count) CU(cudaMemsetAsync(nb.count, 0, (size_t)U * sizeof(int32_t), st));
-    if (nb.speakers) CU(cudaMemsetAsync(nb.speakers, 0, (size_t)U * nb.k * sizeof(int32_t), st));
+    if (nb.count) CU(cudaMemsetAsync(nb.count, 0, (size_t)J * sizeof(int32_t), st));
+    if (nb.speakers) CU(cudaMemsetAsync(nb.speakers, 0, (size_t)J * nb.k * sizeof(int32_t), st));
     if (nb.scores) {
-      const std::vector<float> inf((size_t)U * nb.k, std::numeric_limits<float>::infinity());
+      const std::vector<float> inf((size_t)J * nb.k, std::numeric_limits<float>::infinity());
       CU(cudaMemcpyAsync(nb.scores, inf.data(), inf.size() * sizeof(float), cudaMemcpyHostToDevice, st));
       CU(cudaStreamSynchronize(st));  // (inf is about to go out of scope)
     }
   }
   m->stats = uis_stats{};
-  m->stats.utterances = U;
+  m->stats.utterances = J;
   m->stats.frames = pl.rows;
   m->stats.ctas = pl.ctas;
   m->stats.lanes = pl.G;
   m->stats.cluster = pl.cluster;
-  m->last_U = U;
+  m->last_U = J;
   m->last_score = false;
   m->last_tree_spill = pl.L > 1 && pl.spill;
   m->last_spill_ni = pl.spill_ni; m->last_spill_nlf = pl.spill_nlf; m->last_spill_budget = pl.spill_budget;
@@ -697,20 +757,24 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   if (U == 0 || pl.rows == 0) {
     return 0;
   }
+  uis::BeamParams p = model_params(m);
   long long max_tn = 0;
   for (int u = 0; u < U; ++u) max_tn = std::max<long long>(max_tn, (off[u + 1] - off[u]) * pl.T);
-  if (int rc = ensure_log_tables(m, (int)max_tn)) return rc;
+  if (int rc = ensure_log_tables(m, (int)max_tn, dp, &p)) return rc;
 
-  // schedule: longest utterance first (LPT) -- steps are strictly sequential per utterance
-  std::vector<int> order(U);
-  std::iota(order.begin(), order.end(), 0);
-  std::stable_sort(order.begin(), order.end(),
+  // schedule: longest utterance first (LPT) -- steps are strictly sequential per utterance.  The configs of one
+  // utterance follow each other, so that they read the same input rows at about the same time.
+  std::vector<int> by_len(U), order((size_t)J);
+  std::iota(by_len.begin(), by_len.end(), 0);
+  std::stable_sort(by_len.begin(), by_len.end(),
                    [&](int a, int b) { return off[a + 1] - off[a] > off[b + 1] - off[b]; });
+  for (int i = 0; i < U; ++i)
+    for (int c = 0; c < dp.count; ++c) order[(size_t)i * dp.count + c] = c * U + by_len[i];
   std::vector<long long> off_ll(off, off + U + 1);
 
   if (int rc = m->row_off.ensure((U + 1) * sizeof(long long))) return rc;
-  if (int rc = m->order.ensure(U * sizeof(int))) return rc;
-  if (int rc = m->status.ensure(U * sizeof(int))) return rc;
+  if (int rc = m->order.ensure((size_t)J * sizeof(int))) return rc;
+  if (int rc = m->status.ensure((size_t)J * sizeof(int))) return rc;
   if (int rc = m->queue_stats.ensure(40 * sizeof(unsigned long long))) return rc;
   if (int rc = m->gi.ensure((size_t)pl.rows * 3 * H * sizeof(float))) return rc;
   if (int rc = m->pool_mean.ensure(pool_slots(pl) * D * sizeof(float))) return rc;
@@ -731,14 +795,13 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   }
 
   CU(cudaMemcpyAsync(m->row_off.p, off_ll.data(), (U + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(m->order.p, order.data(), U * sizeof(int), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(m->order.p, order.data(), (size_t)J * sizeof(int), cudaMemcpyHostToDevice, st));
   CU(cudaMemsetAsync(m->queue_stats.p, 0, 40 * sizeof(unsigned long long), st));
-  CU(cudaMemsetAsync(m->status.p, 0xff, U * sizeof(int), st));
+  CU(cudaMemsetAsync(m->status.p, 0xff, (size_t)J * sizeof(int), st));
 
-  uis::BeamParams p = model_params(m);
   p.x = x_dev; p.gi = m->gi.as<float>();
   p.row_off = m->row_off.as<long long>(); p.order = m->order.as<int>();
-  p.U = U; p.B = pl.B; p.Kcap = pl.Kcap; p.T = pl.T; p.P = pl.P; p.maxN = pl.maxN; p.G = pl.G;
+  p.U = J; p.n_utt = U; p.B = pl.B; p.Kcap = pl.Kcap; p.T = pl.T; p.P = pl.P; p.maxN = pl.maxN; p.G = pl.G;
   p.L = pl.L; p.node_cap = pl.node_cap; p.leaf_cap = pl.leaf_cap; p.maxTN = pl.maxTN; p.maxSteps = pl.maxSteps;
   { const char* e = getenv("UIS_DBG_MODE"); p.dbg_mode = e ? atoi(e) : 0; }
   p.pool_mean = m->pool_mean.as<float>(); p.pool_hidden = m->pool_hidden.as<float>(); p.pool_mse = m->pool_mse.as<float>();
@@ -771,15 +834,16 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   long long trace_steps = 0;
   if (taps) {
     if (taps->final_scores) {
-      if (int rc = m->dbg_final_scores.ensure((size_t)U * pl.B * 4)) return rc;
+      if (int rc = m->dbg_final_scores.ensure((size_t)J * pl.B * 4)) return rc;
       p.dbg_final_scores = m->dbg_final_scores.as<float>();
-      if (int rc = m->dbg_final_k.ensure((size_t)U * 4)) return rc;
+      if (int rc = m->dbg_final_k.ensure((size_t)J * 4)) return rc;
       p.dbg_final_k = m->dbg_final_k.as<int>();
     }
-    if (taps->trace_utt >= 0 && taps->trace_utt < U) {
+    if (taps->trace_utt >= 0 && taps->trace_utt < J) {  // a job: utterance trace_utt % U under config trace_utt / U
       p.trace_utt = taps->trace_utt;
       p.trace_capacity = std::max(taps->trace_capacity, 0);
-      trace_steps = ((off[p.trace_utt + 1] - off[p.trace_utt]) * pl.T + pl.L - 1) / pl.L;
+      const int tu = p.trace_utt % U;
+      trace_steps = ((off[tu + 1] - off[tu]) * pl.T + pl.L - 1) / pl.L;
       if (taps->step_winners && p.trace_capacity > 0) {
         if (int rc = m->dbg_win.ensure((size_t)p.trace_capacity * 4 * (1 + pl.L))) return rc;
         if (int rc = m->dbg_score.ensure((size_t)p.trace_capacity * 4)) return rc;
@@ -859,8 +923,8 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   if (taps) {
     CU(cudaStreamSynchronize(st));
     if (p.dbg_final_scores) {
-      CU(cudaMemcpy(taps->final_scores, p.dbg_final_scores, (size_t)U * pl.B * 4, cudaMemcpyDeviceToHost));
-      if (taps->final_k) CU(cudaMemcpy(taps->final_k, p.dbg_final_k, (size_t)U * 4, cudaMemcpyDeviceToHost));
+      CU(cudaMemcpy(taps->final_scores, p.dbg_final_scores, (size_t)J * pl.B * 4, cudaMemcpyDeviceToHost));
+      if (taps->final_k) CU(cudaMemcpy(taps->final_k, p.dbg_final_k, (size_t)J * 4, cudaMemcpyDeviceToHost));
     }
     if (p.dbg_win) {
       CU(cudaMemcpy(taps->step_winners, p.dbg_win, (size_t)p.trace_capacity * 4 * (1 + pl.L), cudaMemcpyDeviceToHost));
@@ -1108,7 +1172,7 @@ int uis_model_destroy(uis_model* m) {
   if (!m) return 0;
   uis::DeviceGuard device_guard_(m->device);
   DevBuf* bufs[] = {&m->wih_t, &m->whh_t, &m->w1_t, &m->w2_t, &m->bih, &m->bhh, &m->b1, &m->b2, &m->wvec, &m->mean0,
-                    &m->hidden0, &m->wih_up_t, &m->logn, &m->logtot, &m->x64, &m->x32, &m->gi, &m->row_off, &m->order,
+                    &m->hidden0, &m->wih_up_t, &m->logn, &m->own_logs.tot, &m->own_logs.cfg, &m->sweep_logs.tot, &m->sweep_logs.cfg, &m->x64, &m->x32, &m->gi, &m->row_off, &m->order,
                     &m->pool_mean, &m->pool_hidden, &m->bp, &m->queue_stats, &m->labels, &m->status, &m->dbg_win,
                     &m->dbg_score, &m->dbg_off, &m->dbg_final_scores, &m->dbg_final_k, &m->dbg_best_mean,
                     &m->dbg_best_hidden, &m->dbg_best_blocks, &m->tc_planes, &m->tc_scratch, &m->pool_mse, &m->stat_bar, &m->stat_scratch,
@@ -1173,6 +1237,18 @@ int uis_predict_device_nbest(uis_model* m, const float* x_dev, const int64_t* fr
                              nullptr, NBestOut{n_best, out->scores, out->speakers, out->count});
 }
 
+int uis_predict_device_sweep(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                             const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                             const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                             const uis_nbest_out* out, const uis_decode_params* params) {
+  if (!m || !opts || !out) return fail(UIS_ERR_INVALID, "null argument");
+  if (int rc = check_nbest(n_best, opts, out)) return rc;
+  DecodeParams dp;
+  if (int rc = check_decode(params, U, &dp)) return rc;
+  return predict_device_impl(m, x_dev, frame_offsets, U, opts, out->labels_dev, taps, stream, max_speakers, min_speakers,
+                             nullptr, NBestOut{n_best, out->scores, out->speakers, out->count}, &dp);
+}
+
 }  // extern "C"
 
 namespace {
@@ -1180,9 +1256,11 @@ namespace {
 int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
                         const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
                         const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev,
-                        const NBestOut& nb) {
+                        const NBestOut& nb, const DecodeParams* dpp) {
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  const DecodeParams dp = dpp ? *dpp : model_decode(m);
   Plan pl;
-  if (int rc = make_plan(m, frame_offsets, U, opts, &pl)) return rc;
+  if (int rc = make_plan(m, frame_offsets, U, opts, &pl, dp.count)) return rc;
   if (int rc = check_bounds(U, max_speakers, min_speakers)) return rc;
   if (U > 0 && pl.rows > 0 && (!x_dev || !labels_dev)) return fail(UIS_ERR_INVALID, "null device buffer");
   uis::DeviceGuard device_guard_(m->device);
@@ -1197,7 +1275,7 @@ int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_o
     x_dev = m->x32.as<float>();
   }
   return run_device(m, x_dev, frame_offsets, U, pl, labels_dev, taps, st,
-                    SpeakerBounds{max_speakers, min_speakers, speakers_dev}, nb);
+                    SpeakerBounds{max_speakers, min_speakers, speakers_dev}, nb, dp);
 }
 
 int ensure_host_path(uis_model* m) {
@@ -1226,15 +1304,19 @@ size_t staging_chunk_rows(int d_user) {
 // projection on `st`, then the beam kernel, then one D2H copy of all labels.
 int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
                             const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
-                            const SpeakerBounds& sb, int32_t* speakers_out, const NBestOut& nb);
+                            const SpeakerBounds& sb, int32_t* speakers_out, const NBestOut& nb, int u0, int U_all,
+                            const DecodeParams& dp);
 
 int stage_host_rows(uis_model* m, const double* const* seqs, int U, const int64_t* off, size_t rows, cudaStream_t st,
                     int* n_chunks_out, bool* staged_out);
 
+// Utterances [u0, u0 + U) of a list of U_all; `nb` holds the whole list's [configs][U_all][k] outputs.
 int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
                        const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
-                       const SpeakerBounds& sb, int32_t* speakers_out, const NBestOut& nb) {
-  const int rc = predict_host_group_impl(m, seqs, n_frames, U, off, pl, labels_out, taps, st, sb, speakers_out, nb);
+                       const SpeakerBounds& sb, int32_t* speakers_out, const NBestOut& nb, int u0, int U_all,
+                       const DecodeParams& dp) {
+  const int rc = predict_host_group_impl(m, seqs, n_frames, U, off, pl, labels_out, taps, st, sb, speakers_out, nb, u0,
+                                         U_all, dp);
   if (rc != 0 && rc != UIS_ERR_OVERFLOW && rc != UIS_ERR_CAPACITY) {
     // a failed call may leave copies / kernels in flight on either stream: drain them (the error already recorded in
     // uis_last_error() is the one reported) so that the staging ring and the workspace are quiescent for the next call
@@ -1249,15 +1331,18 @@ int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n
 
 int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
                             const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
-                            const SpeakerBounds& sb_host, int32_t* speakers_out, const NBestOut& nb_host) {
+                            const SpeakerBounds& sb_host, int32_t* speakers_out, const NBestOut& nb_host, int u0,
+                            int U_all, const DecodeParams& dp) {
   const size_t rows = (size_t)pl.rows;
+  const int C = dp.count, J = U * C;
   if (rows == 0) {
     m->stats = uis_stats{};
-    m->stats.utterances = U;
+    m->stats.utterances = J;
     return 0;
   }
-  const int K = nb_host.k;  // label planes
-  if (int rc = m->labels.ensure(rows * 4 * K)) return rc;
+  const int K = nb_host.k;
+  const size_t planes = (size_t)K * C;  // label planes: [config][hypothesis]
+  if (int rc = m->labels.ensure(rows * 4 * planes)) return rc;
   SpeakerBounds sb = sb_host;  // speaker counts land in the handle's device buffer, then in `speakers_out`
   if (speakers_out) {
     if (int rc = m->spk_out.ensure((size_t)U * 4)) return rc;
@@ -1265,22 +1350,22 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
   }
   NBestOut nb{K};  // likewise the N-best scores, cluster counts and hypothesis counts
   if (nb_host.scores) {
-    if (int rc = m->nb_scores.ensure((size_t)U * K * 4)) return rc;
+    if (int rc = m->nb_scores.ensure((size_t)J * K * 4)) return rc;
     nb.scores = m->nb_scores.as<float>();
   }
   if (nb_host.speakers) {
-    if (int rc = m->nb_speakers.ensure((size_t)U * K * 4)) return rc;
+    if (int rc = m->nb_speakers.ensure((size_t)J * K * 4)) return rc;
     nb.speakers = m->nb_speakers.as<int32_t>();
   }
   if (nb_host.count) {
-    if (int rc = m->nb_count.ensure((size_t)U * 4)) return rc;
+    if (int rc = m->nb_count.ensure((size_t)J * 4)) return rc;
     nb.count = m->nb_count.as<int32_t>();
   }
-  if (rows * 4 * K > m->labels_pin_cap) {
+  if (rows * 4 * planes > m->labels_pin_cap) {
     if (m->labels_pin) cudaFreeHost(m->labels_pin);
     m->labels_pin = nullptr;
     m->labels_pin_cap = 0;
-    const size_t want = rows * 4 * K + rows / 2 + 4096;
+    const size_t want = rows * 4 * planes + rows / 2 + 4096;
     if (cudaMallocHost(&m->labels_pin, want) != cudaSuccess) {
       (void)cudaGetLastError();
       return fail(UIS_ERR_NOMEM, "cudaMallocHost(%zu) for the label staging buffer failed", want);
@@ -1290,21 +1375,26 @@ int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64
   int n_chunks = 0;
   bool staged = false;
   if (int rc = stage_host_rows(m, seqs, U, off, rows, st, &n_chunks, &staged)) return rc;
-  if (int rc = run_device(m, m->x32.as<float>(), off, U, pl, m->labels.as<int32_t>(), taps, st, sb, nb, /*gi_ready=*/true))
+  if (int rc = run_device(m, m->x32.as<float>(), off, U, pl, m->labels.as<int32_t>(), taps, st, sb, nb, dp,
+                         /*gi_ready=*/true))
     return rc;
   m->stats.kernel_launches = 1 + 2 * (int64_t)n_chunks + (pl.L > 1 && pl.spill == 1 ? 1 : 0);
   m->stats.chunks = n_chunks;
   m->stats.staged = staged ? 1 : 0;
-  CU(cudaMemcpyAsync(m->labels_pin, m->labels.p, rows * 4 * K, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(m->labels_pin, m->labels.p, rows * 4 * planes, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  for (int j = 0; j < K; ++j)  // plane j of the device rows -> rows j of the caller's [K][n_frames[q]] buffers
+  for (size_t j = 0; j < planes; ++j)  // plane j of the device rows -> rows j of the caller's [C][K][n_frames[q]] buffers
     for (int q = 0; q < U; ++q)
       if (n_frames[q] > 0)
-        std::memcpy(labels_out[q] + (size_t)j * n_frames[q], m->labels_pin + (size_t)j * rows + off[q], (size_t)n_frames[q] * 4);
+        std::memcpy(labels_out[q] + j * n_frames[q], m->labels_pin + j * rows + off[q], (size_t)n_frames[q] * 4);
   if (speakers_out) CU(cudaMemcpy(speakers_out, sb.out_dev, (size_t)U * 4, cudaMemcpyDeviceToHost));
-  if (nb.scores) CU(cudaMemcpy(nb_host.scores, nb.scores, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
-  if (nb.speakers) CU(cudaMemcpy(nb_host.speakers, nb.speakers, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
-  if (nb.count) CU(cudaMemcpy(nb_host.count, nb.count, (size_t)U * 4, cudaMemcpyDeviceToHost));
+  for (int c = 0; c < C; ++c) {  // config c's block of this group -> [c][u0 ..][K] of the whole list's outputs
+    const size_t dst = (size_t)c * U_all + u0, src = (size_t)c * U;
+    if (nb.scores) CU(cudaMemcpy(nb_host.scores + dst * K, nb.scores + src * K, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
+    if (nb.speakers)
+      CU(cudaMemcpy(nb_host.speakers + dst * K, nb.speakers + src * K, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
+    if (nb.count) CU(cudaMemcpy(nb_host.count + dst, nb.count + src, (size_t)U * 4, cudaMemcpyDeviceToHost));
+  }
   if (int rc = collect(m)) return rc;
   CU(cudaEventElapsedTime(&m->stats.h2d_ms, m->ev_h2d[0], m->ev_h2d[1]));
   CU(cudaEventElapsedTime(&m->stats.pipeline_ms, m->ev_pipe, m->ev[1]));  // first cast -> beam kernel start
@@ -1455,6 +1545,18 @@ int uis_predict_nbest(uis_model* m, const double* const* seqs, const int64_t* n_
                            nullptr, NBestOut{n_best, out->scores, out->speakers, out->count});
 }
 
+int uis_predict_sweep(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                      const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                      const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                      const uis_nbest_out* out, const uis_decode_params* params) {
+  if (!m || !opts || !out) return fail(UIS_ERR_INVALID, "null argument");
+  if (int rc = check_nbest(n_best, opts, out)) return rc;
+  DecodeParams dp;
+  if (int rc = check_decode(params, U, &dp)) return rc;
+  return predict_host_impl(m, seqs, n_frames, U, opts, out->labels_out, taps, stream, max_speakers, min_speakers,
+                           nullptr, NBestOut{n_best, out->scores, out->speakers, out->count}, &dp);
+}
+
 }  // extern "C"
 
 namespace {
@@ -1462,15 +1564,17 @@ namespace {
 int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
                       const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
                       const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out,
-                      const NBestOut& nb) {
+                      const NBestOut& nb, const DecodeParams* dpp) {
   if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
   if (U < 0 || (U > 0 && (!seqs || !n_frames || !labels_out))) return fail(UIS_ERR_INVALID, "null argument");
   if (int rc = check_bounds(U, max_speakers, min_speakers)) return rc;
+  const DecodeParams dp = dpp ? *dpp : model_decode(m);
+  const size_t J = (size_t)U * dp.count;
   if (speakers_out && U > 0) std::memset(speakers_out, 0, (size_t)U * sizeof(int32_t));  // empty inputs: 0
   if (U > 0) {  // empty inputs return no N-best hypothesis
-    if (nb.scores) std::fill(nb.scores, nb.scores + (size_t)U * nb.k, std::numeric_limits<float>::infinity());
-    if (nb.speakers) std::memset(nb.speakers, 0, (size_t)U * nb.k * sizeof(int32_t));
-    if (nb.count) std::memset(nb.count, 0, (size_t)U * sizeof(int32_t));
+    if (nb.scores) std::fill(nb.scores, nb.scores + J * nb.k, std::numeric_limits<float>::infinity());
+    if (nb.speakers) std::memset(nb.speakers, 0, J * nb.k * sizeof(int32_t));
+    if (nb.count) std::memset(nb.count, 0, J * sizeof(int32_t));
   }
   const auto t_begin = std::chrono::steady_clock::now();
   std::vector<int64_t> off(U + 1, 0);
@@ -1480,7 +1584,7 @@ int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_
     off[u + 1] = off[u] + n_frames[u];
   }
   Plan pl;
-  if (int rc = make_plan(m, off.data(), U, opts, &pl)) return rc;
+  if (int rc = make_plan(m, off.data(), U, opts, &pl, dp.count)) return rc;
   uis::DeviceGuard device_guard_(m->device);
   CU(device_guard_.status);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1488,21 +1592,21 @@ int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_
   // Memory: the per-frame workspace (gi 12H B + fp32 rows 4D B + labels) is the part that grows with the input.
   // A list that does not fit the device at once is decoded in groups of whole utterances, one after the other
   // (utterances are independent, uisrnn.py:587-589); UISRNN_B200_MAX_ROWS forces a limit (tests).
-  const size_t per_row = (size_t)3 * m->H * 4 + (size_t)m->D * 4 + (size_t)4 * nb.k;  // (+ one label per plane)
+  const size_t per_row = (size_t)3 * m->H * 4 + (size_t)m->D * 4 + (size_t)4 * nb.k * dp.count;  // (+ one label per plane)
   size_t max_rows = 0;
   if (const char* env = std::getenv("UISRNN_B200_MAX_ROWS")) max_rows = (size_t)std::max(1ll, std::atoll(env));
   if (!max_rows) {
     size_t free_b = 0, total_b = 0;
     CU(cudaMemGetInfo(&free_b, &total_b));
     const size_t held = m->gi.cap + m->x32.cap + m->labels.cap + m->x64.cap;  // re-used by this call
-    const size_t fixed = workspace_bytes(m, pl, U) - (size_t)pl.rows * 3 * m->H * 4 +
-                         (size_t)uis_model::kSlots * staging_chunk_rows(m->D_user) * m->D_user * 8 + (size_t)U * (2 * nb.k + 1) * 4;
+    const size_t fixed = workspace_bytes(m, pl, U, dp.count) - (size_t)pl.rows * 3 * m->H * 4 +
+                         (size_t)uis_model::kSlots * staging_chunk_rows(m->D_user) * m->D_user * 8 + J * (2 * nb.k + 1) * 4;
     const double budget = 0.9 * (double)(free_b + held) - (double)fixed;
     max_rows = budget > (double)per_row ? (size_t)(budget / (double)per_row) : 1;
   }
   if ((size_t)pl.rows <= max_rows || taps || U <= 1) {
     if (int rc = predict_host_group(m, seqs, n_frames, U, off.data(), pl, labels_out, taps, st,
-                                    SpeakerBounds{max_speakers, min_speakers}, speakers_out, nb))
+                                    SpeakerBounds{max_speakers, min_speakers}, speakers_out, nb, 0, U, dp))
       return rc;
     m->stats.groups = 1;
   } else {
@@ -1514,10 +1618,10 @@ int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_
       std::vector<int64_t> goff(u1 - u0 + 1);
       for (int q = u0; q <= u1; ++q) goff[q - u0] = off[q] - off[u0];
       Plan gp;
-      if (int rc = make_plan(m, goff.data(), u1 - u0, opts, &gp)) return rc;
+      if (int rc = make_plan(m, goff.data(), u1 - u0, opts, &gp, dp.count)) return rc;
       if (int rc = predict_host_group(m, seqs + u0, n_frames + u0, u1 - u0, goff.data(), gp, labels_out + u0, nullptr, st,
                                       SpeakerBounds{max_speakers, min_speakers}.at(u0),
-                                      speakers_out ? speakers_out + u0 : nullptr, nb.at(u0)))
+                                      speakers_out ? speakers_out + u0 : nullptr, nb, u0, U, dp))
         return rc;
       m->stats.groups = 1;
       add_stats(&total, m->stats);
@@ -1592,15 +1696,18 @@ int plan_chains(const int32_t* labels, const int64_t* off, int U, ChainPlan* cp)
   return 0;
 }
 
-// Enqueues a score call on `st`: input projection (unless gi_ready), chain kernel, first visits, reduce.  x_dev: the
-// fp32 rows at the kernel shape (m->D); labels_dev: the canonical labels the plan was made from.
+// Enqueues a score call on `st`: input projection (unless gi_ready), chain kernel, first visits, then one reduce per
+// config of `dp` (scores_dev [configs][U], frame_dev [configs][rows]).  x_dev: the fp32 rows at the kernel shape (m->D);
+// labels_dev: the canonical labels the plan was made from.
 int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const ChainPlan& cp, const int32_t* labels_dev,
-              float* scores_dev, float* frame_dev, cudaStream_t st, bool gi_ready) {
+              float* scores_dev, float* frame_dev, cudaStream_t st, bool gi_ready, const DecodeParams& dp) {
   const int H = m->H, D = m->D;
   const long long rows = off[U];
   long long maxN = 0;
   for (int u = 0; u < U; ++u) maxN = std::max<long long>(maxN, off[u + 1] - off[u]);
-  if (int rc = ensure_log_tables(m, (int)maxN)) return rc;  // block counts and totals reach N
+  uis::ScoreParams sp{};
+  sp.b = model_params(m);
+  if (int rc = ensure_log_tables(m, (int)maxN, dp, &sp.b)) return rc;  // block counts and totals reach N
   const int CP = uis::score_cp(H);
   const int ctas = (int)std::max(1ll, std::min<long long>(m->num_sms, (cp.queued + CP - 1) / CP));
   if (uis::score_smem(H, D) > 227u * 1024u) return fail(UIS_ERR_UNSUPPORTED, "no score kernel for hidden=%d dim=%d", H, D);
@@ -1619,11 +1726,9 @@ int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const
   CU(cudaMemcpyAsync(m->sc_chain_rows.p, cp.rows.data(), cp.rows.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
   CU(cudaMemsetAsync(m->queue_stats.p, 0, 40 * sizeof(unsigned long long), st));
 
-  uis::ScoreParams sp{};
-  sp.b = model_params(m);
   sp.b.x = x_dev; sp.b.gi = m->gi.as<float>();
   sp.b.row_off = m->row_off.as<long long>();
-  sp.b.U = U; sp.b.P = 2;
+  sp.b.U = U; sp.b.n_utt = U; sp.b.P = 2;
   sp.b.pool_mean = m->pool_mean.as<float>(); sp.b.pool_hidden = m->pool_hidden.as<float>();
   sp.b.queue = m->queue_stats.as<int>();
   sp.b.stats = m->queue_stats.as<unsigned long long>() + 8;
@@ -1651,22 +1756,24 @@ int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const
   CU(cudaEventRecord(m->ev[2], st));
   if (!uis::launch_score_first(D, sp, st, &e)) return fail(UIS_ERR_UNSUPPORTED, "no score kernel for dim=%d", D);
   if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score first-visit kernel launch failed: %s", cudaGetErrorString(e));
-  e = uis::launch_score_reduce(sp, st);
-  if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score reduce kernel launch failed: %s", cudaGetErrorString(e));
+  for (int c = 0; c < dp.count; ++c) {  // the Gaussian terms in sc_mse serve every config
+    e = uis::launch_score_reduce(sp, c, st);
+    if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score reduce kernel launch failed: %s", cudaGetErrorString(e));
+  }
   m->stats.ctas = cp.queued > 0 ? ctas : 0;
-  m->stats.kernel_launches = (gi_ready ? 0 : 1) + (cp.queued > 0 ? 1 : 0) + 2;
+  m->stats.kernel_launches = (gi_ready ? 0 : 1) + (cp.queued > 0 ? 1 : 0) + 1 + dp.count;
   m->stats_pending = true;
   return 0;
 }
 
 // Stats of a score call before it runs (the rest is zero; collect() adds the chain kernel's counters and times).
-void begin_score_stats(uis_model* m, int U, long long rows, const ChainPlan& cp, cudaStream_t st) {
+void begin_score_stats(uis_model* m, int jobs, long long rows, const ChainPlan& cp, cudaStream_t st) {
   m->stats = uis_stats{};
-  m->stats.utterances = U;
+  m->stats.utterances = jobs;
   m->stats.frames = rows;
   m->stats.max_k = cp.max_k;
   m->stats.engine = 1;
-  m->last_U = U;
+  m->last_U = jobs;
   m->last_score = true;
   m->last_tree_spill = false;
   m->last_stream = st;
@@ -1674,7 +1781,9 @@ void begin_score_stats(uis_model* m, int U, long long rows, const ChainPlan& cp,
 }
 
 int score_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
-                    const int32_t* const* labels, float* scores_out, float* const* frame_out, cudaStream_t st) {
+                    const int32_t* const* labels, float* scores_out, float* const* frame_out, cudaStream_t st,
+                    const DecodeParams& dp) {
+  const int C = dp.count;
   const auto t_begin = std::chrono::steady_clock::now();
   std::vector<int64_t> off(U + 1, 0);
   for (int u = 0; u < U; ++u) {
@@ -1689,28 +1798,31 @@ int score_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_fr
     if (n_frames[u] > 0) std::memcpy(lab.data() + off[u], labels[u], (size_t)n_frames[u] * 4);
   ChainPlan cp;
   if (int rc = plan_chains(lab.data(), off.data(), U, &cp)) return rc;
-  begin_score_stats(m, U, rows, cp, st);
-  std::fill(scores_out, scores_out + U, 0.f);  // empty utterances score 0
+  begin_score_stats(m, U * C, rows, cp, st);
+  std::fill(scores_out, scores_out + (size_t)U * C, 0.f);  // empty utterances score 0
   if (rows == 0) return 0;
   int n_chunks = 0;
   bool staged = false;
   if (int rc = stage_host_rows(m, seqs, U, off.data(), (size_t)rows, st, &n_chunks, &staged)) return rc;
   if (int rc = m->labels.ensure((size_t)rows * 4)) return rc;
   CU(cudaMemcpyAsync(m->labels.p, lab.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, st));
-  if (int rc = m->sc_out.ensure(((size_t)U + (frame_out ? (size_t)rows : 0)) * 4)) return rc;
-  float* dev_frames = frame_out ? m->sc_out.as<float>() + U : nullptr;
+  if (int rc = m->sc_out.ensure(((size_t)U + (frame_out ? (size_t)rows : 0)) * C * 4)) return rc;
+  float* dev_frames = frame_out ? m->sc_out.as<float>() + (size_t)U * C : nullptr;
   if (int rc = run_score(m, m->x32.as<float>(), off.data(), U, cp, m->labels.as<int32_t>(), m->sc_out.as<float>(),
-                         dev_frames, st, /*gi_ready=*/true))
+                         dev_frames, st, /*gi_ready=*/true, dp))
     return rc;
   m->stats.kernel_launches += 2 * (int64_t)n_chunks;
   m->stats.chunks = n_chunks;
   m->stats.staged = staged ? 1 : 0;
-  CU(cudaMemcpyAsync(scores_out, m->sc_out.p, (size_t)U * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(scores_out, m->sc_out.p, (size_t)U * C * 4, cudaMemcpyDeviceToHost, st));
   if (frame_out) {
-    CU(cudaMemcpyAsync(lab.data(), dev_frames, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));  // (lab: spent)
+    lab.resize((size_t)rows * C);  // (lab: spent)
+    CU(cudaMemcpyAsync(lab.data(), dev_frames, (size_t)rows * C * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    for (int u = 0; u < U; ++u)
-      if (n_frames[u] > 0) std::memcpy(frame_out[u], lab.data() + off[u], (size_t)n_frames[u] * 4);
+    for (int c = 0; c < C; ++c)  // config c's increments -> row c of the caller's [C][n_frames[u]] buffers
+      for (int u = 0; u < U; ++u)
+        if (n_frames[u] > 0)
+          std::memcpy(frame_out[u] + (size_t)c * n_frames[u], lab.data() + (size_t)c * rows + off[u], (size_t)n_frames[u] * 4);
   }
   CU(cudaStreamSynchronize(st));
   if (int rc = collect(m)) return rc;
@@ -1721,6 +1833,11 @@ int score_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_fr
   return 0;
 }
 
+int score_host(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int32_t* const* labels,
+               float* scores_out, float* const* frame_out, void* stream, const DecodeParams& dp);
+int score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U, const int32_t* labels_dev,
+                 float* scores_dev, float* frame_dev, void* stream, const DecodeParams& dp);
+
 }  // namespace
 
 extern "C" {
@@ -1728,11 +1845,43 @@ extern "C" {
 int uis_score(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int32_t* const* labels,
               float* scores_out, float* const* frame_out, void* stream) {
   if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  return score_host(m, seqs, n_frames, U, labels, scores_out, frame_out, stream, model_decode(m));
+}
+
+int uis_score_sweep(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int32_t* const* labels,
+                    float* scores_out, float* const* frame_out, void* stream, const uis_decode_params* params) {
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  DecodeParams dp;
+  if (int rc = check_decode(params, U, &dp)) return rc;
+  return score_host(m, seqs, n_frames, U, labels, scores_out, frame_out, stream, dp);
+}
+
+int uis_score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U, const int32_t* labels_dev,
+                     float* scores_dev, float* frame_dev, void* stream) {
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  return score_device(m, x_dev, frame_offsets, U, labels_dev, scores_dev, frame_dev, stream, model_decode(m));
+}
+
+int uis_score_device_sweep(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                           const int32_t* labels_dev, float* scores_dev, float* frame_dev, void* stream,
+                           const uis_decode_params* params) {
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  DecodeParams dp;
+  if (int rc = check_decode(params, U, &dp)) return rc;
+  return score_device(m, x_dev, frame_offsets, U, labels_dev, scores_dev, frame_dev, stream, dp);
+}
+
+}  // extern "C"
+
+namespace {
+
+int score_host(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int32_t* const* labels,
+               float* scores_out, float* const* frame_out, void* stream, const DecodeParams& dp) {
   if (U < 0 || (U > 0 && (!seqs || !n_frames || !labels || !scores_out))) return fail(UIS_ERR_INVALID, "null argument");
   uis::DeviceGuard device_guard_(m->device);
   CU(device_guard_.status);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int rc = score_host_impl(m, seqs, n_frames, U, labels, scores_out, frame_out, st);
+  const int rc = score_host_impl(m, seqs, n_frames, U, labels, scores_out, frame_out, st, dp);
   if (rc != 0 && rc != UIS_ERR_INVALID) {  // drain what a failed call may have left in flight (see predict_host_group)
     const std::string keep = g_err;
     if (m->copy_stream) cudaStreamSynchronize(m->copy_stream);
@@ -1743,9 +1892,8 @@ int uis_score(uis_model* m, const double* const* seqs, const int64_t* n_frames, 
   return rc;
 }
 
-int uis_score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U, const int32_t* labels_dev,
-                     float* scores_dev, float* frame_dev, void* stream) {
-  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+int score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U, const int32_t* labels_dev,
+                 float* scores_dev, float* frame_dev, void* stream, const DecodeParams& dp) {
   if (U < 0 || (U > 0 && (!frame_offsets || !scores_dev))) return fail(UIS_ERR_INVALID, "null argument");
   for (int u = 0; u < U; ++u)
     if (frame_offsets[u + 1] < frame_offsets[u]) return fail(UIS_ERR_INVALID, "frame_offsets not monotone");
@@ -1762,10 +1910,10 @@ int uis_score_device(uis_model* m, const float* x_dev, const int64_t* frame_offs
   }
   ChainPlan cp;
   if (int rc = plan_chains(lab.data(), frame_offsets, U, &cp)) return rc;
-  begin_score_stats(m, U, rows, cp, st);
+  begin_score_stats(m, U * dp.count, rows, cp, st);
   if (U == 0) return 0;
   if (rows == 0) {
-    CU(cudaMemsetAsync(scores_dev, 0, (size_t)U * 4, st));  // empty utterances score 0
+    CU(cudaMemsetAsync(scores_dev, 0, (size_t)U * dp.count * 4, st));  // empty utterances score 0
     return 0;
   }
   if (m->D != m->D_user) {  // zero-pad the caller's rows to the kernel's row length
@@ -1776,7 +1924,7 @@ int uis_score_device(uis_model* m, const float* x_dev, const int64_t* frame_offs
     CU(cudaGetLastError());
     x_dev = m->x32.as<float>();
   }
-  return run_score(m, x_dev, frame_offsets, U, cp, labels_dev, scores_dev, frame_dev, st, /*gi_ready=*/false);
+  return run_score(m, x_dev, frame_offsets, U, cp, labels_dev, scores_dev, frame_dev, st, /*gi_ready=*/false, dp);
 }
 
-}  // extern "C"
+}  // namespace

@@ -86,14 +86,18 @@ struct BeamParams {
   const float* wvec;     // [D]  1 / (2 sigma2)
   const float* mean0;    // [D]
   const float* hidden0;  // [depth][H]
-  double log_p0, log_1mp0, log_alpha;
   const double* logn;    // [>= maxTN + 2]  log(i)
-  const double* logtot;  // [>= maxTN + 2]  log(i + crp_alpha)
+  // Decoding parameters.  The kernels decode p.U jobs: job j is utterance j % n_utt under config j / n_utt (a call
+  // without a sweep is one config holding the model's values, so job = utterance).
+  const double* cfg_log;      // [configs][3]  log(p0), log(1 - p0), log(crp_alpha)
+  const double* logtot;       // [configs][logtot_stride]  log(i + crp_alpha), i < logtot_stride (>= maxTN + 2)
+  long long logtot_stride;
+  int n_utt;                  // distinct utterances (rows, spk_bound); outputs are per job
   // inputs
   const float* x;           // [rows][D]
   const float* gi;          // [rows][3H]  W_ih x + b_ih
-  const long long* row_off; // [U + 1]
-  const int* order;         // [U] utterance ids, longest first
+  const long long* row_off; // [n_utt + 1]
+  const int* order;         // [U] job ids, longest utterance first, the configs of one utterance side by side
   int U, B, Kcap, T, P, maxN, G;
   int L, node_cap, leaf_cap, maxTN, maxSteps;  // look_ahead >= 2 (uis_beam_tree.cuh) only
   int dbg_mode;  // 0 normal; 1 = stream the weights but skip the math (timing experiment, results invalid)
@@ -141,6 +145,18 @@ struct BeamParams {
   int* nbest_speakers;     // [U][n_best]  clusters, 0 where absent (may be null)
   int* nbest_count;        // [U]          hypotheses returned (may be null)
 };
+
+// The log terms of a job's config (uisrnn.py:416-418, 445): the transition / ddCRP penalty of a candidate is
+//   existing cluster c: (c == last) ? log_1mp0 : (log_p0 + logn[blocks_c]) - logtot[tot]
+//   new cluster:        (log_p0 + log_alpha) - logtot[tot]
+struct JobLogs {
+  double log_p0, log_1mp0, log_alpha;
+  const double* logtot;
+};
+__device__ inline JobLogs job_logs(const BeamParams& p, int cfg) {
+  const double* v = p.cfg_log + 3 * cfg;
+  return JobLogs{__ldg(v), __ldg(v + 1), __ldg(v + 2), p.logtot + (size_t)cfg * p.logtot_stride};
+}
 
 // Per-utterance speaker bounds: a hypothesis may hold at most spk_max clusters; the returned one is the best-ranked
 // final hypothesis with at least spk_min clusters (rank 0 if there is none).
@@ -1170,9 +1186,9 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
         uidx = atomicAdd(p.queue, 1);
       }
       if (uidx >= p.U) { ls[LS_ACTIVE] = 0; ls[LS_FRESH] = 0; return; }
-      const int u = p.order[uidx];
-      const long long row0 = p.row_off[u];
-      const int N = (int)(p.row_off[u + 1] - row0);
+      const int u = p.order[uidx], utt = u % p.n_utt;  // u: the job
+      const long long row0 = p.row_off[utt];
+      const int N = (int)(p.row_off[utt + 1] - row0);
       if (N == 0) {
         p.status[u] = 0;
         if (p.spk_out) p.spk_out[u] = 0;
@@ -1188,7 +1204,7 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
       ls[LS_ACTIVE] = 1; ls[LS_FAILED] = 0; ls[LS_TRACED] = (u == p.trace_utt) && tap_leader; ls[LS_ERR] = 0;
       ls[LS_ROW0_LO] = (int)(row0 & 0xffffffffll); ls[LS_ROW0_HI] = (int)(row0 >> 32);
       ls[LS_DBGROWS_LO] = 0; ls[LS_DBGROWS_HI] = 0; ls[LS_FRESH] = 1;
-      ls[LS_KHI] = spk_max(p, u); ls[LS_KLO] = spk_min(p, u);
+      ls[LS_KHI] = spk_max(p, utt); ls[LS_KLO] = spk_min(p, utt);
       for (unsigned w = 0; w < PW; ++w) reinterpret_cast<unsigned*>(lane_base(g) + L.l_scored)[w] = 0;
       int* meta = reinterpret_cast<int*>(lane_base(g) + L.l_meta);  // [gen][field][B]: K,last,tot,nl
       meta[0] = 0; meta[B] = -1; meta[2 * B] = 0; reinterpret_cast<float*>(meta)[3 * B] = 0.f;
@@ -1365,6 +1381,7 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
         // P1a: one thread per candidate resolves (hypothesis, cluster) -> slot, marks the slot live, and evaluates the
         // transition / ddCRP term in fp64 from the host-built log tables (the np.log values of uisrnn.py:415-420,
         // 444-446).  Parked in keys[] / svals[].  A thread's candidates grow, so its hypothesis index only moves on.
+        const JobLogs lg = job_logs(p, ls[LS_U] / p.n_utt);
         int b = 0;
         for (int e = ttid; e < ne; e += TT) {
           while (candoff[b + 1] <= e) ++b;
@@ -1375,9 +1392,9 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
             const TabEntry en = tab[(size_t)b * Kcap + c];
             slot = en.slot;
             atomicOr(used + (slot >> 5), 1u << (slot & 31));
-            pen = (c == mLast[b]) ? p.log_1mp0 : (p.log_p0 + __ldg(p.logn + en.blocks)) - __ldg(p.logtot + mTot[b]);
+            pen = (c == mLast[b]) ? lg.log_1mp0 : (lg.log_p0 + __ldg(p.logn + en.blocks)) - __ldg(lg.logtot + mTot[b]);
           } else {
-            pen = (p.log_p0 + p.log_alpha) - __ldg(p.logtot + mTot[b]);
+            pen = (lg.log_p0 + lg.log_alpha) - __ldg(lg.logtot + mTot[b]);
           }
           pens[e] = pen;
           // slot (16 bits) | hypothesis (5 bits, or 7 when beam_size > 32: the host then caps kcap at 511) | cluster
@@ -1710,7 +1727,8 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
         for (int j = ttid; j < p.n_best && !(STAT && sq != 0); j += TT) {
           const int r0 = ok ? nbest_rank(fK, nwin, ls[LS_KLO], j) : -1;
           const int N = ls[LS_N];
-          int* lab = p.labels + (size_t)j * p.label_plane + (((long long)ls[LS_ROW0_HI] << 32) | (unsigned)ls[LS_ROW0_LO]);
+          int* lab = p.labels + ((size_t)(u / p.n_utt) * p.n_best + j) * p.label_plane +
+                     (((long long)ls[LS_ROW0_HI] << 32) | (unsigned)ls[LS_ROW0_LO]);
           if (r0 < 0) {
             for (int i = 0; i < N; ++i) lab[i] = -1;
           } else {

@@ -375,12 +375,12 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
     named_bar_sync(1, NT);
     const int uidx = misc[TM_UIDX];
     if (uidx >= p.U) break;
-    const int u = p.order[uidx];
+    const int u = p.order[uidx], utt = u % p.n_utt;  // u: the job
     if constexpr (SPILL) {  // decoded by the shared-memory kernel (or failed there for another reason)
       if (!p.tree_spill_all && p.status[u] != -5) { named_bar_sync(1, NT); continue; }
     }
-    const long long row0 = p.row_off[u];
-    const int N = (int)(p.row_off[u + 1] - row0);
+    const long long row0 = p.row_off[utt];
+    const int N = (int)(p.row_off[utt + 1] - row0);
     const int TN = p.T * N;
     const bool traced = (u == p.trace_utt);
     long long dbg_rows = 0;
@@ -433,7 +433,7 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
           for (int q0 = pa; q0 < pb; q0 += NT) {
             const int q = q0 + tid;
             const int Kp = (q < pb) ? ((level == 1) ? mK[q] : n_k[q]) : -1;
-            const int fan = Kp + (Kp < spk_max(p, u) ? 1 : 0);  // at max_speakers: no new-cluster child
+            const int fan = Kp + (Kp < spk_max(p, utt) ? 1 : 0);  // at max_speakers: no new-cluster child
             int chunk;
             const int o = tot + block_excl_scan<NT>(fan, sc, &chunk, lane, warp);
             if (chunk > cap - tot) { if (tid == 0) misc[TM_ERR] = 3; break; }
@@ -453,7 +453,7 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
           const int base = lvl[level];
           for (int q = pa; q < pb; ++q) {
             const int Kp = (level == 1) ? mK[q] : n_k[q];
-            const int fan = Kp + (Kp < spk_max(p, u) ? 1 : 0);  // at max_speakers: no new-cluster child
+            const int fan = Kp + (Kp < spk_max(p, utt) ? 1 : 0);  // at max_speakers: no new-cluster child
             const int cap = last ? NLF : NI - base;
             if (tot + fan > cap) { misc[TM_ERR] = 3; break; }
             for (int c = 0; c < fan; ++c) {
@@ -488,9 +488,10 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
           const bool live[1] = {true};
           const float acc = gauss_rows<D, 1>(m4, live, xs, wv, lane);
           if (lane == 0) {
+            const JobLogs lg = job_logs(p, u / p.n_utt);
             double pen;
-            if (!isnew) pen = (c == lastp) ? p.log_1mp0 : (p.log_p0 + __ldg(p.logn + en.blocks)) - __ldg(p.logtot + totp);
-            else pen = (p.log_p0 + p.log_alpha) - __ldg(p.logtot + totp);
+            if (!isnew) pen = (c == lastp) ? lg.log_1mp0 : (lg.log_p0 + __ldg(p.logn + en.blocks)) - __ldg(lg.logtot + totp);
+            else pen = (lg.log_p0 + lg.log_alpha) - __ldg(lg.logtot + totp);
             const float loss = __double2float_rn((double)acc - pen);
             const float S = __fadd_rn(nlp, loss);  // per sub-step fp32 accumulation (uisrnn.py:452)
             if (last) {
@@ -626,8 +627,8 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
     // clusters (rank 0 when none has them, j = 0) and walks its own column chain into label plane j
     for (int j = tid; j < p.n_best; j += NT) {
       const int* fK = meta + gen * 4 * B;
-      const int r0 = ok ? nbest_rank(fK, nb, spk_min(p, u), j) : -1;
-      int* lab = p.labels + (size_t)j * p.label_plane + row0;
+      const int r0 = ok ? nbest_rank(fK, nb, spk_min(p, utt), j) : -1;
+      int* lab = p.labels + ((size_t)(u / p.n_utt) * p.n_best + j) * p.label_plane + row0;
       if (r0 < 0) {
         for (int i = 0; i < N; ++i) lab[i] = -1;
       } else {
@@ -643,7 +644,7 @@ __global__ void __launch_bounds__(Cfg<H, D, tree_cp<H>()>::BLOCK, 1) uis_beam_tr
       }
       // clusters of hypothesis 0, 0 for a failed utterance; an empty utterance returns no N-best hypothesis
       if (j == 0 && p.spk_out) p.spk_out[u] = ok ? fK[r0] : 0;
-      if (j == 0 && p.nbest_count) p.nbest_count[u] = (ok && N > 0) ? nbest_n(fK, nb, spk_min(p, u), p.n_best) : 0;
+      if (j == 0 && p.nbest_count) p.nbest_count[u] = (ok && N > 0) ? nbest_n(fK, nb, spk_min(p, utt), p.n_best) : 0;
       nbest_store(p, u, j, N > 0 ? r0 : -1, fK, reinterpret_cast<const float*>(fK + 3 * B));
     }
     if (p.dbg_final_scores) {

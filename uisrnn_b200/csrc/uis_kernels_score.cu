@@ -207,11 +207,14 @@ __global__ void __launch_bounds__(256) score_first_kernel(const __grid_constant_
 }
 
 // One thread per utterance: loss_t = fl32(f64(mse_t) - pen_t) and S = fl32(S + loss_t) in frame order, with pen_t the
-// beam kernel's transition / ddCRP term (phase P1a) of the trace so far.
-__global__ void __launch_bounds__(128) score_reduce_kernel(const __grid_constant__ ScoreParams sp) {
+// beam kernel's transition / ddCRP term (phase P1a) of the trace so far under config `cfg`, whose totals go to
+// scores[cfg][U] and increments to frame_out[cfg][rows].
+__global__ void __launch_bounds__(128) score_reduce_kernel(const __grid_constant__ ScoreParams sp, int cfg) {
   const BeamParams& p = sp.b;
   const int u = blockIdx.x * blockDim.x + threadIdx.x;
   if (u >= p.U) return;
+  const JobLogs lg = job_logs(p, cfg);
+  float* frame_out = sp.frame_out ? sp.frame_out + (size_t)cfg * p.row_off[p.U] : nullptr;
   const long long r0 = p.row_off[u], r1 = p.row_off[u + 1];
   int* blk = sp.blocks + r0;  // block counts of the utterance's clusters (K <= frames)
   int K = 0, last = -1, tot = 0;
@@ -220,18 +223,18 @@ __global__ void __launch_bounds__(128) score_reduce_kernel(const __grid_constant
     const int c = sp.labels[r];
     const bool isnew = c >= K;
     double pen;
-    if (!isnew) pen = (c == last) ? p.log_1mp0 : (p.log_p0 + __ldg(p.logn + blk[c])) - __ldg(p.logtot + tot);
-    else pen = (p.log_p0 + p.log_alpha) - __ldg(p.logtot + tot);
+    if (!isnew) pen = (c == last) ? lg.log_1mp0 : (lg.log_p0 + __ldg(p.logn + blk[c])) - __ldg(lg.logtot + tot);
+    else pen = (lg.log_p0 + lg.log_alpha) - __ldg(lg.logtot + tot);
     const float loss = __double2float_rn((double)sp.mse[r] - pen);
     S = __fadd_rn(S, loss);
-    if (sp.frame_out) sp.frame_out[r] = loss;
+    if (frame_out) frame_out[r] = loss;
     const bool moved = isnew || c != last;
     if (isnew) { blk[c] = 1; K += 1; }
     else if (moved) blk[c] += 1;
     tot += moved ? 1 : 0;
     last = c;
   }
-  sp.scores[u] = S;
+  sp.scores[(size_t)cfg * p.U + u] = S;
 }
 
 unsigned score_smem(int H, int D) {
@@ -272,8 +275,8 @@ bool launch_score_first(int D, const ScoreParams& sp, cudaStream_t st, cudaError
   return true;
 }
 
-cudaError_t launch_score_reduce(const ScoreParams& sp, cudaStream_t st) {
-  score_reduce_kernel<<<(sp.b.U + 127) / 128, 128, 0, st>>>(sp);
+cudaError_t launch_score_reduce(const ScoreParams& sp, int cfg, cudaStream_t st) {
+  score_reduce_kernel<<<(sp.b.U + 127) / 128, 128, 0, st>>>(sp, cfg);
   return cudaGetLastError();
 }
 

@@ -36,17 +36,18 @@ struct ScoreParams {
   int queued;                   // the first `queued` chains (length >= 2) run through the chain kernel
   float* mse;                   // [rows] Gaussian term of a frame against its cluster's mean before that frame
   const int* labels;            // [rows] canonical labels
-  float* scores;                // [U]    neg_likelihood
-  float* frame_out;             // [rows] per-frame increments (may be null)
+  float* scores;                // [configs][U]    neg_likelihood
+  float* frame_out;             // [configs][rows] per-frame increments (may be null)
   int* blocks;                  // [rows] reduce kernel scratch: block counts of utterance u's clusters at row_off[u]
 };
 constexpr int score_cp(int H) { return H > 512 ? 8 : kCPBeam; }  // columns per pass (= the FFMA beam kernel's)
 unsigned score_smem(int H, int D);
 // the three kernels of a score call, in order: chains (Gaussian terms of every visit after the first), first visits
-// (mean0 against every chain's first frame), reduce (per utterance); false if (H, D) is not an instantiated shape
+// (mean0 against every chain's first frame), reduce (per utterance, once per config of a sweep: the first two do not
+// depend on the decoding parameters); false if (H, D) is not an instantiated shape
 bool launch_score_chains(int H, int D, const ScoreParams& sp, int ctas, cudaStream_t st, cudaError_t* err);
 bool launch_score_first(int D, const ScoreParams& sp, cudaStream_t st, cudaError_t* err);
-cudaError_t launch_score_reduce(const ScoreParams& sp, cudaStream_t st);
+cudaError_t launch_score_reduce(const ScoreParams& sp, int cfg, cudaStream_t st);
 
 template <class Kern>
 inline cudaError_t launch_with_smem(Kern kern, const BeamParams& p, int ctas, int block, unsigned smem, cudaStream_t st) {

@@ -48,6 +48,10 @@ class NBestOut(C.Structure):
               ('speakers', C.POINTER(C.c_int32)), ('count', C.POINTER(C.c_int32))]
 
 
+class DecodeParams(C.Structure):
+  _fields_ = [('count', C.c_int32), ('crp_alpha', C.POINTER(C.c_double)), ('transition_bias', C.POINTER(C.c_double))]
+
+
 class Stats(C.Structure):
   _fields_ = [('utterances', C.c_int64), ('frames', C.c_int64), ('beam_steps', C.c_int64),
               ('gru_columns', C.c_int64), ('weight_passes', C.c_int64), ('candidates', C.c_int64),
@@ -69,7 +73,8 @@ class Stats(C.Structure):
 EXPORTS = ('uis_version', 'uis_last_error', 'uis_model_create', 'uis_model_destroy',
            'uis_model_constants', 'uis_predict', 'uis_predict_device', 'uis_predict_bounded',
            'uis_predict_device_bounded', 'uis_predict_nbest', 'uis_predict_device_nbest',
-           'uis_score', 'uis_score_device', 'uis_predict_workspace_bytes', 'uis_get_stats', 'uis_trainer_create',
+           'uis_score', 'uis_score_device', 'uis_predict_sweep', 'uis_predict_device_sweep', 'uis_score_sweep',
+           'uis_score_device_sweep', 'uis_predict_workspace_bytes', 'uis_get_stats', 'uis_trainer_create',
            'uis_trainer_destroy', 'uis_trainer_step', 'uis_trainer_get', 'uis_trainer_losses',
            'uis_trainer_comm_size', 'uis_trainer_comm_export', 'uis_trainer_comm_apply',
            'uis_trainer_set_corpus', 'uis_trainer_step_corpus')
@@ -170,6 +175,14 @@ def load_library():
   lib.uis_score_device.restype = C.c_int
   lib.uis_score_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p]
+  lib.uis_predict_sweep.restype = C.c_int
+  lib.uis_predict_sweep.argtypes = lib.uis_predict_nbest.argtypes + [C.POINTER(DecodeParams)]
+  lib.uis_predict_device_sweep.restype = C.c_int
+  lib.uis_predict_device_sweep.argtypes = lib.uis_predict_device_nbest.argtypes + [C.POINTER(DecodeParams)]
+  lib.uis_score_sweep.restype = C.c_int
+  lib.uis_score_sweep.argtypes = lib.uis_score.argtypes + [C.POINTER(DecodeParams)]
+  lib.uis_score_device_sweep.restype = C.c_int
+  lib.uis_score_device_sweep.argtypes = lib.uis_score_device.argtypes + [C.POINTER(DecodeParams)]
   lib.uis_predict_workspace_bytes.restype = C.c_size_t
   lib.uis_predict_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.c_int,
                                               C.POINTER(PredictOpts)]
@@ -242,6 +255,35 @@ def check_n_best(n_best, beam_size):
   if not 1 <= n_best <= beam_size:
     raise ValueError('n_best must be in [1, beam_size={}], got {}'.format(beam_size, n_best))
   return int(n_best)
+
+
+def decode_params(pairs):
+  """(crp_alpha, transition_bias) float64 arrays of a sweep: a non-empty sequence of pairs, crp_alpha finite and > 0,
+  transition_bias finite and in (0, 1).  Raises ValueError naming the first bad pair."""
+  if isinstance(pairs, (str, bytes)) or not hasattr(pairs, '__len__') or len(pairs) == 0:
+    raise ValueError('decode_params must be a non-empty sequence of (crp_alpha, transition_bias) pairs')
+  alpha, p0 = np.empty(len(pairs), np.float64), np.empty(len(pairs), np.float64)
+  for c, pair in enumerate(pairs):
+    try:
+      a, b = pair
+      alpha[c], p0[c] = float(a), float(b)
+    except (TypeError, ValueError):
+      raise ValueError('decode_params pair {}: {!r} is not a (crp_alpha, transition_bias) pair of floats'.format(
+          c, pair)) from None
+    if isinstance(a, (bool, np.bool_)) or isinstance(b, (bool, np.bool_)):
+      raise ValueError('decode_params pair {}: {!r} is not a (crp_alpha, transition_bias) pair of floats'.format(c, pair))
+    if not (np.isfinite(alpha[c]) and alpha[c] > 0):
+      raise ValueError('decode_params pair {}: crp_alpha={!r} (need finite and > 0)'.format(c, a))
+    if not (np.isfinite(p0[c]) and 0 < p0[c] < 1):
+      raise ValueError('decode_params pair {}: transition_bias={!r} (need finite and in (0, 1))'.format(c, b))
+  return alpha, p0
+
+
+def _decode_struct(pairs):
+  """(DecodeParams, keep-alive arrays, count) of a validated sweep."""
+  alpha, p0 = decode_params(pairs)
+  dp = C.POINTER(C.c_double)
+  return DecodeParams(len(alpha), alpha.ctypes.data_as(dp), p0.ctypes.data_as(dp)), (alpha, p0), len(alpha)
 
 
 class NativeModel:
@@ -423,6 +465,79 @@ class NativeModel:
                                               C.c_void_p(speakers_ptr))
     _check(self._lib, rc)
 
+  def predict_sweep(self, seqs, decode_params, beam_size=10, look_ahead=1, test_iteration=2, kcap=0, n_ctas=0,
+                    trace_utt=None, stream=0, lanes=0, cluster=0, engine=0, max_speakers=None, min_speakers=None,
+                    n_best=1):
+    """predict() under C (crp_alpha, transition_bias) pairs in one call (uis_predict_sweep).  Returns (labels, scores,
+    speakers, count): labels[u] int32 [C][k][N_u], scores float32 [C][U][k], speakers int32 [C][U][k], count int32
+    [C][U]; config c's entries are what predict(..., n_best=k) returns for a model created with pair c.  trace_utt
+    names a job (c * U + u); the taps' final_scores / final_k are [C * U][...]."""
+    n = len(seqs)
+    dp, keep_dp, nc = _decode_struct(decode_params)
+    mx, mn = speaker_bounds(n, max_speakers, min_speakers)
+    k = check_n_best(n_best, beam_size)
+    keep = [s if (type(s) is np.ndarray and s.dtype == np.float64 and s.flags.c_contiguous)
+            else np.ascontiguousarray(s, dtype=np.float64) for s in seqs]
+    for s in keep:
+      if s.ndim != 2 or s.shape[1] != self.D:
+        raise ValueError('utterance shape {} does not match D={}'.format(s.shape, self.D))
+    lens = np.array([s.shape[0] for s in keep] or [0], np.int64)
+    offs = np.zeros(n + 1, np.int64)
+    np.cumsum(lens[:n], out=offs[1:])
+    flat = np.empty(max(nc * k * int(offs[-1]), 1), np.int32)
+    outs = [flat[nc * k * offs[i]:nc * k * offs[i + 1]] for i in range(n)]
+    out_addr = (flat.ctypes.data + 4 * nc * k * offs[:max(n, 1)]).astype(np.uint64)
+    in_addr = np.array([s.ctypes.data for s in keep] or [0], np.uint64)
+    opts = self._opts(beam_size, look_ahead, test_iteration, kcap, n_ctas, lanes, cluster, engine)
+    taps, bufs, tp = None, None, None
+    if trace_utt is not None:
+      taps, bufs = self._taps(trace_utt, n * nc, [int(lens[j % max(n, 1)]) for j in range(n * nc)], beam_size,
+                              look_ahead, test_iteration, kcap)
+      tp = C.byref(taps)
+    ip = C.POINTER(C.c_int32)
+    scores = np.empty((nc, max(n, 1), k), np.float32)
+    spk = np.empty((nc, max(n, 1), k), np.int32)
+    count = np.empty((nc, max(n, 1)), np.int32)
+    nb = NBestOut(out_addr.ctypes.data_as(C.POINTER(C.c_void_p)), None, scores.ctypes.data_as(C.POINTER(C.c_float)),
+                  spk.ctypes.data_as(ip), count.ctypes.data_as(ip))
+    arg = lambda a: a.ctypes.data_as(ip) if a is not None else None
+    _check(self._lib, self._lib.uis_predict_sweep(
+        self._h, in_addr.ctypes.data_as(C.POINTER(C.c_void_p)), lens.ctypes.data_as(C.POINTER(C.c_int64)), n,
+        C.byref(opts), tp, C.c_void_p(stream), arg(mx), arg(mn), k, C.byref(nb), C.byref(dp)))
+    del keep_dp
+    # (a list of U utterances is held as [C][U][k]; with n == 0 the padding row is dropped)
+    out = ([o.reshape(nc, k, int(lens[i])) for i, o in enumerate(outs)], scores[:, :n], spk[:, :n], count[:, :n])
+    if bufs is not None:
+      nrows = int(bufs['off'][-1]) if len(bufs['off']) else 0
+      bufs['win'] = bufs['win'][:nrows]
+      bufs['score'] = bufs['score'][:nrows]
+      kk = int(bufs['final_k'][trace_utt]) if trace_utt >= 0 else 0
+      bufs['best_mean'] = bufs['best_mean'][:kk]
+      bufs['best_hidden'] = bufs['best_hidden'][:kk]
+      bufs['best_blocks'] = bufs['best_blocks'][:kk]
+      return out, bufs
+    return out
+
+  def predict_device_sweep(self, x_ptr, frame_offsets, labels_ptr, scores_ptr, decode_params, beam_size=10,
+                           look_ahead=1, test_iteration=2, kcap=0, n_ctas=0, stream=0, lanes=0, cluster=0, engine=0,
+                           max_speakers=None, min_speakers=None, n_best=1, speakers_ptr=0, count_ptr=0):
+    """Device-resident sweep (uis_predict_device_sweep): labels_ptr -> int32 [C][k][rows], scores_ptr -> float32
+    [C][U][k] (required), speakers_ptr -> int32 [C][U][k], count_ptr -> int32 [C][U] (0 = none).  Asynchronous on
+    `stream`."""
+    off = np.ascontiguousarray(frame_offsets, dtype=np.int64)
+    dp, keep_dp, _ = _decode_struct(decode_params)
+    mx, mn = speaker_bounds(len(off) - 1, max_speakers, min_speakers)
+    k = check_n_best(n_best, beam_size)
+    ip = C.POINTER(C.c_int32)
+    opts = self._opts(beam_size, look_ahead, test_iteration, kcap, n_ctas, lanes, cluster, engine)
+    nb = NBestOut(None, C.c_void_p(labels_ptr), C.cast(C.c_void_p(scores_ptr), C.POINTER(C.c_float)),
+                  C.cast(C.c_void_p(speakers_ptr), ip), C.cast(C.c_void_p(count_ptr), ip))
+    _check(self._lib, self._lib.uis_predict_device_sweep(
+        self._h, C.c_void_p(x_ptr), off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1, C.byref(opts), None,
+        C.c_void_p(stream), mx.ctypes.data_as(ip) if mx is not None else None,
+        mn.ctypes.data_as(ip) if mn is not None else None, k, C.byref(nb), C.byref(dp)))
+    del keep_dp
+
   def score(self, seqs, labels, per_frame=False):
     """neg_likelihood of given labellings (uis_score): seqs is a list of float64 [N_u, D] arrays (host), labels a
     list of canonical int label sequences (0, 1, 2, ... in order of first appearance), one of length N_u per
@@ -449,6 +564,44 @@ class NativeModel:
         C.cast(ptrs(labs), C.POINTER(C.c_void_p)), scores.ctypes.data_as(C.POINTER(C.c_float)),
         C.cast(ptrs(frames), C.POINTER(C.c_void_p)) if per_frame else None, None))
     return (scores[:n], frames) if per_frame else scores[:n]
+
+  def score_sweep(self, seqs, labels, decode_params, per_frame=False):
+    """score() under C (crp_alpha, transition_bias) pairs in one call (uis_score_sweep): float32 scores [C][U]; with
+    per_frame, (scores, list of float32 [C][N_u] per-frame increments)."""
+    if not isinstance(seqs, (list, tuple)) or not isinstance(labels, (list, tuple)):
+      raise TypeError('seqs and labels must be lists')
+    if len(seqs) != len(labels):
+      raise ValueError('{} utterances but {} label sequences'.format(len(seqs), len(labels)))
+    dp, keep_dp, nc = _decode_struct(decode_params)
+    n = len(seqs)
+    keep = [s if (type(s) is np.ndarray and s.dtype == np.float64 and s.flags.c_contiguous)
+            else np.ascontiguousarray(s, dtype=np.float64) for s in seqs]
+    labs = [np.ascontiguousarray(l, dtype=np.int32) for l in labels]
+    for u, (s, l) in enumerate(zip(keep, labs)):
+      if s.ndim != 2 or s.shape[1] != self.D:
+        raise ValueError('utterance shape {} does not match D={}'.format(s.shape, self.D))
+      if l.ndim != 1 or len(l) != s.shape[0]:
+        raise ValueError('utterance {}: {} labels for {} frames'.format(u, l.size, s.shape[0]))
+    lens = np.array([s.shape[0] for s in keep] or [0], np.int64)
+    scores = np.zeros((nc, max(n, 1)), np.float32)
+    frames = [np.empty((nc, s.shape[0]), np.float32) for s in keep] if per_frame else None
+    ptrs = lambda arrs: (C.c_void_p * max(len(arrs), 1))(*[a.ctypes.data for a in arrs])
+    _check(self._lib, self._lib.uis_score_sweep(
+        self._h, C.cast(ptrs(keep), C.POINTER(C.c_void_p)), lens.ctypes.data_as(C.POINTER(C.c_int64)), n,
+        C.cast(ptrs(labs), C.POINTER(C.c_void_p)), scores.ctypes.data_as(C.POINTER(C.c_float)),
+        C.cast(ptrs(frames), C.POINTER(C.c_void_p)) if per_frame else None, None, C.byref(dp)))
+    del keep_dp
+    return (scores[:, :n], frames) if per_frame else scores[:, :n]
+
+  def score_device_sweep(self, x_ptr, frame_offsets, labels_ptr, scores_ptr, decode_params, frame_ptr=0, stream=0):
+    """Device-resident score sweep (uis_score_device_sweep): scores_ptr -> float32 [C][U], frame_ptr -> float32
+    [C][rows] (0 = none)."""
+    off = np.ascontiguousarray(frame_offsets, dtype=np.int64)
+    dp, keep_dp, _ = _decode_struct(decode_params)
+    _check(self._lib, self._lib.uis_score_device_sweep(
+        self._h, C.c_void_p(x_ptr), off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1, C.c_void_p(labels_ptr),
+        C.c_void_p(scores_ptr), C.c_void_p(frame_ptr), C.c_void_p(stream), C.byref(dp)))
+    del keep_dp
 
   def score_device(self, x_ptr, frame_offsets, labels_ptr, scores_ptr, frame_ptr=0, stream=0):
     """Device-resident variant (uis_score_device): x_ptr -> fp32 [rows, D], labels_ptr -> canonical int32 [rows],

@@ -477,7 +477,7 @@ class UISRNN:
     _warn_min_speakers([0], [len(test_sequence)], speakers, bounds[1])
     return labels[0]
 
-  def predict(self, test_sequences, args, *, max_speakers=None, min_speakers=None, n_best=None):
+  def predict(self, test_sequences, args, *, max_speakers=None, min_speakers=None, n_best=None, decode_params=None):
     """Labels for one sequence (ndarray -> list of ints) or many (list -> list of lists)
     (uisrnn.py:564-590).  On CUDA a list is decoded by a single native call.
 
@@ -494,7 +494,16 @@ class UISRNN:
     alone when none has them -- so hypothesis 0 is what the call returns without n_best.  `scores` are the
     hypotheses' neg_likelihood accumulated over the whole decode (lower is better; the gap between the first two is
     a confidence), `speakers` their cluster counts.  An empty sequence gives no hypothesis.  With test_iteration > 1
-    two hypotheses can differ only in an earlier tiled copy and so carry the same labels; they are kept apart."""
+    two hypotheses can differ only in an earlier tiled copy and so carry the same labels; they are kept apart.
+
+    Decoding-parameter sweeps (not in the reference): `decode_params` is a non-empty sequence of (crp_alpha,
+    transition_bias) pairs, crp_alpha finite and > 0, transition_bias finite and in (0, 1).  The result is then a list
+    with one entry per pair, entry c being exactly what this call returns without `decode_params` for a model whose
+    crp_alpha / transition_bias are pair c (bounds and n_best apply to every pair).  The model is not changed.  On a
+    CUDA device the whole grid is one native call: the inputs are copied and projected once.  Pick a pair by scoring
+    each entry on a labelled dev set (e.g. `evals.compute_sequence_match_accuracy`)."""
+    if decode_params is not None:
+      return self._predict_sweep(test_sequences, args, max_speakers, min_speakers, n_best, decode_params)
     if isinstance(test_sequences, np.ndarray):
       return self.predict_single(test_sequences, args, max_speakers=max_speakers, min_speakers=min_speakers,
                                  n_best=n_best)
@@ -521,7 +530,48 @@ class UISRNN:
       return [self.predict_single(sequence, args) for sequence in test_sequences]
     raise TypeError('test_sequences should be either a list or numpy array.')
 
-  def score(self, test_sequences, test_cluster_ids, *, per_frame=False):
+  def _predict_sweep(self, test_sequences, args, max_speakers, min_speakers, n_best, decode_params):
+    """predict() under every (crp_alpha, transition_bias) pair of `decode_params`: one entry per pair."""
+    pairs = _decode_params(decode_params)
+    single = isinstance(test_sequences, np.ndarray)
+    if single:
+      if np.ndim(max_speakers) or np.ndim(min_speakers):
+        raise ValueError('predict_single takes one int per bound')
+      sequences = [test_sequences]
+    elif isinstance(test_sequences, list):
+      sequences = test_sequences
+    else:
+      raise TypeError('test_sequences should be either a list or numpy array.')
+    for sequence in sequences:
+      _check_test_sequence(sequence, self.observation_dim)
+    k = _check_n_best(n_best, args) if n_best is not None else None
+    bounds = _speaker_bounds(len(sequences), max_speakers, min_speakers)
+    if self.device.type == 'cuda':
+      results, speakers = _native_predict_sweep(self._native_model(), sequences, args, bounds, k, pairs)
+    else:
+      mx, mn = bounds
+      results, speakers = [], []
+      for alpha, bias in pairs:
+        decoder = beam_cpu.CpuBeamSearch(self, crp_alpha=alpha, transition_bias=bias)
+        outs = [decoder.decode(s, args.beam_size, args.look_ahead, args.test_iteration,
+                               int(mx[i]) if mx is not None else 0, int(mn[i]) if mn is not None else 0,
+                               return_speakers=True, n_best=k) for i, s in enumerate(sequences)]
+        if k is None:
+          results.append([o[0] for o in outs])
+          speakers.append([o[1] for o in outs])
+        else:
+          results.append([NBest(*o) for o in outs])
+          speakers.append([o[2][0] if o[2] else 0 for o in outs])
+    if bounds[1] is not None:
+      lengths = [len(s) for s in sequences]
+      short = [(u, c) for c, row in enumerate(speakers)
+               for u, (n, got, lo) in enumerate(zip(lengths, row, bounds[1])) if n > 0 and got < lo]
+      if short:
+        warnings.warn('min_speakers: the final beam of (utterance, pair) {} held no hypothesis with that many '
+                      'speakers; the best hypothesis was returned instead'.format(short), RuntimeWarning, stacklevel=3)
+    return [r[0] for r in results] if single else results
+
+  def score(self, test_sequences, test_cluster_ids, *, per_frame=False, decode_params=None):
     """The neg_likelihood the model gives to given speaker labellings (not in the reference, where it exists only
     inside the beam search): the score of the trace that assigns frame t to cluster test_cluster_ids[t], the same
     quantity as `NBest.scores` -- lower is better.  Scoring the ground truth against the decoded hypothesis tells a
@@ -532,9 +582,15 @@ class UISRNN:
     renaming: they are mapped to 0, 1, 2, ... in order of first appearance.  test_iteration is not applied: the
     sequence is scored once, as given (tile both the sequence and its labels to score a tiled decode).  An empty
     sequence scores 0.  With per_frame=True every utterance gives a `FrameScores(total, increments)` instead.  On a
-    CUDA device a list is scored by one native call."""
+    CUDA device a list is scored by one native call.
+
+    With `decode_params` (a non-empty sequence of (crp_alpha, transition_bias) pairs, validated as in `predict`) the
+    result is a list with one entry per pair, each being what this call returns for a model with that pair.  On a CUDA
+    device the GRU work is done once for all pairs."""
+    pairs = _decode_params(decode_params) if decode_params is not None else None
     if isinstance(test_sequences, np.ndarray):
-      return self.score([test_sequences], [test_cluster_ids], per_frame=per_frame)[0]
+      out = self.score([test_sequences], [test_cluster_ids], per_frame=per_frame, decode_params=pairs)
+      return out[0] if pairs is None else [entry[0] for entry in out]
     if not isinstance(test_sequences, list):
       raise TypeError('test_sequences should be either a list or numpy array.')
     if not isinstance(test_cluster_ids, (list, tuple)):
@@ -547,6 +603,21 @@ class UISRNN:
     for u, (sequence, lab) in enumerate(zip(test_sequences, labels)):
       if len(lab) != len(sequence):
         raise ValueError('utterance {}: {} labels for {} frames'.format(u, len(lab), len(sequence)))
+    if pairs is not None:
+      if self.device.type == 'cuda':
+        model = self._native_model()
+        with model.lock:
+          out = model.score_sweep(test_sequences, labels, pairs, per_frame=per_frame)
+        if not per_frame:
+          return [[float(v) for v in row] for row in out]
+        totals, increments = out
+        return [[FrameScores(float(v), inc[c]) for v, inc in zip(row, increments)] for c, row in enumerate(totals)]
+      result = []
+      for alpha, bias in pairs:
+        decoder = beam_cpu.CpuBeamSearch(self, crp_alpha=alpha, transition_bias=bias)
+        out = [decoder.score(sequence, lab) for sequence, lab in zip(test_sequences, labels)]
+        result.append([FrameScores(float(t), inc) for t, inc in out] if per_frame else [float(t) for t, _ in out])
+      return result
     if self.device.type == 'cuda':
       model = self._native_model()
       with model.lock:
@@ -584,6 +655,13 @@ def _warn_min_speakers(indices, lengths, speakers, min_speakers):
                   'the best hypothesis was returned instead'.format(short), RuntimeWarning, stacklevel=3)
 
 
+def _decode_params(decode_params):
+  """Validated list of (crp_alpha, transition_bias) float pairs (ValueError names the first bad pair)."""
+  from . import native  # validation only: the library is not loaded
+  alpha, bias = native.decode_params(decode_params)
+  return [(float(a), float(b)) for a, b in zip(alpha, bias)]
+
+
 def _check_n_best(n_best, args):
   from . import native  # validation only: the library is not loaded
   return native.check_n_best(n_best, args.beam_size)
@@ -618,6 +696,32 @@ def _native_predict(model, sequences, args, as_arrays, bounds, n_best=None):
       if err.code != native.UIS_ERR_OVERFLOW or kcap >= 1024:
         raise
       kcap = 32 if kcap == 0 else kcap * 2  # a hypothesis opened more clusters than the device tables hold: grow and retry
+
+
+def _native_predict_sweep(model, sequences, args, bounds, n_best, pairs):
+  """NativeModel.predict_sweep with the kcap retry over the whole sweep.  Returns (per-pair results, per-pair
+  cluster counts of hypothesis 0): a result is the label lists of the utterances, or their NBest list with n_best."""
+  from . import native
+  mx, mn = bounds
+  kcap = _DEFAULT_KCAP
+  while True:
+    try:
+      with model.lock:
+        labels, scores, speakers, count = model.predict_sweep(
+            sequences, pairs, beam_size=args.beam_size, look_ahead=args.look_ahead,
+            test_iteration=args.test_iteration, kcap=kcap, max_speakers=mx, min_speakers=mn, n_best=n_best or 1)
+      break
+    except native.NativeError as err:
+      if err.code != native.UIS_ERR_OVERFLOW or kcap >= 1024:
+        raise
+      kcap = 32 if kcap == 0 else kcap * 2
+  results = []
+  for c in range(len(pairs)):
+    if n_best is None:
+      results.append([lab[c, 0].tolist() for lab in labels])
+    else:
+      results.append(_nbest_result([lab[c] for lab in labels], scores[c], speakers[c], count[c]))
+  return results, speakers[:, :, 0]
 
 
 def _predict_shard(model, args, device_index, sequences, out, position, bounds, n_best=None):
