@@ -116,6 +116,29 @@ def test_fit_on_cuda_then_native_predict_matches_cpu_decoder():
   assert model._native[0] != before              # pylint: disable=protected-access
 
 
+def test_edit_through_data_rebuilds_the_device_twin():
+  """A sign flip of one W2 row through `.data` keeps `_version` and every |value|: predict() and score() must still
+  decode the edited weights, as a fresh model that loaded them does."""
+  import torch
+  w = load_weights('model_toy100.npz')
+  model = uisrnn_from_weights(w, enable_cuda=True)
+  xs, _ = toy_utterances()
+  xs = xs[:3]
+  args = inference_args()
+  model.predict(xs, args)  # builds the device twin
+  path = [[0, 1] * (len(x) // 2) + [0] * (len(x) % 2) for x in xs]
+  before_sc = model.score(xs, path)
+  with torch.no_grad():
+    model.rnn_model.linear_mean2.weight.data[0].neg_()
+  edited = {k: (np.array(v) if not np.isscalar(v) else v) for k, v in w.items()}
+  edited['w2'][0] = -edited['w2'][0]
+  fresh = uisrnn_from_weights(edited, enable_cuda=True)
+  want, want_sc = fresh.predict(xs, args), fresh.score(xs, path)
+  assert model.predict(xs, args) == want
+  assert model.score(xs, path) == want_sc
+  assert want_sc != before_sc  # the edit is visible in the scores (the labels may not move)
+
+
 def test_parallel_predict_thread_branch_on_two_devices(toy_model):
   """SURVEY 8(f) f3: with >= 2 visible GPUs `parallel_predict(num_processes=k)` shards the list by frame count and
   decodes every shard on its own device from its own host thread (one uis_model per device).  The caller's current

@@ -300,18 +300,34 @@ float tc_pow2_scale(double bound) {
   return std::ldexp(1.0f, e);
 }
 
-// Splits w * scale into fp16 hi + lo (22 significant bits) -- the A operand planes of the wgmma pass.
-void tc_split(const std::vector<float>& w, float scale, __half* hi, __half* lo) {
-  for (size_t i = 0; i < w.size(); ++i) {
-    const float v = w[i] * scale;
-    const __half h = __float2half_rn(v);
-    hi[i] = h;
-    lo[i] = __float2half_rn(v - __half2float(h));
+// Splits w * scale into fp16 hi + lo (22 significant bits) -- the A operand planes of the wgmma pass.  Returns the
+// largest share of a row's sum |w * scale| that the split loses, sum_j |hi + lo - w * scale| over sum_j |w * scale|: the
+// relative error the planes add to that row's dot product with a uniformly bounded operand.
+double tc_split(const std::vector<float>& w, int cols, float scale, __half* hi, __half* lo) {
+  double worst = 0;
+  for (size_t r0 = 0; r0 < w.size(); r0 += cols) {
+    double lost = 0, mass = 0;
+    for (size_t i = r0; i < r0 + cols; ++i) {
+      const float v = w[i] * scale;
+      const __half h = __float2half_rn(v);
+      hi[i] = h;
+      lo[i] = __float2half_rn(v - __half2float(h));
+      lost += std::fabs((double)__half2float(h) + (double)__half2float(lo[i]) - (double)v);
+      mass += std::fabs((double)v);
+    }
+    if (mass > 0) worst = std::max(worst, lost / mass);
   }
+  return worst;
 }
 
 // w_hh [3H,H], w1 [H,H], w2 [D,H] are the row-major (= K-major) PyTorch tensors; hidden0 [H] = CoreRNN(0, h0).
-// Leaves tc_ready false (the FFMA kernels serve the model) when the shape does not tile or a bound is not finite.
+// Leaves tc_ready false (the FFMA kernels serve the model) when the shape does not tile, a bound is not finite or
+// clamps, or a weight matrix's split loses more than kTcSplitLoss of some row's sum |w * scale| (tc_split): that
+// happens when a few weights far above the rest set the matrix's scale and leave the others' lo halves subnormal.
+// 2^-20 is below the ~2^-19.5 that a 512-term fp32 FMA chain typically loses relative to its sum of |terms|.  Uniform
+// (512, 512) weights lose 2^-25.0; with one entry 2^17 times their largest 2^-21.3 (tensor cores), 2^24 times 2^-14.3
+// (FFMA).
+constexpr double kTcSplitLoss = 0x1p-20;
 int tc_prepare(uis_model* m, const std::vector<float>& w_hh, const std::vector<float>& w1, const std::vector<float>& b1,
                const std::vector<float>& w2, const std::vector<float>& hidden0) {
   const int H = m->H, D = m->D;
@@ -331,19 +347,20 @@ int tc_prepare(uis_model* m, const std::vector<float>& w_hh, const std::vector<f
   if (s_hh == 0.f || s_1 == 0.f || s_2 == 0.f || s_h == 0.f || s_a == 0.f) return 0;
   const size_t rows = (size_t)3 * H + H + D, n = rows * H;
   std::vector<__half> planes(2 * n);  // [plane 0 = lo | plane 1 = hi][rows][H]
-  tc_split(w_hh, s_hh, planes.data() + n, planes.data());
+  double lost = tc_split(w_hh, H, s_hh, planes.data() + n, planes.data());
   {
     std::vector<__half> hi((size_t)H * H), lo((size_t)H * H);
-    tc_split(w1, s_1, hi.data(), lo.data());
+    lost = std::max(lost, tc_split(w1, H, s_1, hi.data(), lo.data()));
     std::copy(lo.begin(), lo.end(), planes.begin() + (size_t)3 * H * H);
     std::copy(hi.begin(), hi.end(), planes.begin() + n + (size_t)3 * H * H);
   }
   {
     std::vector<__half> hi((size_t)D * H), lo((size_t)D * H);
-    tc_split(w2, s_2, hi.data(), lo.data());
+    lost = std::max(lost, tc_split(w2, H, s_2, hi.data(), lo.data()));
     std::copy(lo.begin(), lo.end(), planes.begin() + (size_t)4 * H * H);
     std::copy(hi.begin(), hi.end(), planes.begin() + n + (size_t)4 * H * H);
   }
+  if (!(lost <= kTcSplitLoss)) return 0;
   if (int r = upload(m->tc_planes, planes.data(), planes.size() * sizeof(__half))) return r;
   TensorMapEncodeFn encode = nullptr;
   cudaDriverEntryPointQueryResult qres;
@@ -584,7 +601,8 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
         return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: no kernel for hidden=%d dim=%d columns=%d", m->H, m->D, N);
       }
     } else if (o->engine == 2) {
-      return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine needs look_ahead 1, depth 1, hidden/dim multiples of 128 and no cluster mode");
+      return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine needs look_ahead 1, depth 1, hidden/dim multiples of 128, no "
+                                       "cluster mode and weights its fp16 split holds (uis_model_create)");
     }
     if (!pl->tcn)
       while (G > 1 && smem_bytes(m->H, m->D, pl->B, pl->Kcap, G) > 227u * 1024u) --G;

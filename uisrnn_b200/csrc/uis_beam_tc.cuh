@@ -9,8 +9,10 @@
 //     a shared-memory ring by tensor-map TMA (cp.async.bulk.tensor.2d, 128-byte swizzle, boxes of 128 rows x 64 k =
 //     16 KB); each of the two consumer warpgroups multiplies the 64 rows of a box that are its own (m64 instructions);
 //   * the hidden columns of the pass are split the same way by the consumer warps and stay in shared memory as the
-//     B operand: per 64-wide k atom, rows [0, N) hold the hi halves and rows [N, 2N) the lo halves of the N columns,
-//     so ONE instruction with N' = 2N multiplies a weight box with both:  D[:, 0:N] += A * Bhi,  D[:, N:2N] += A * Blo;
+//     B operand: per 64-wide k atom, rows [0, N) hold the hi halves and rows [N, 2N) the lo halves * 2^11 of the N
+//     columns, so ONE instruction with N' = 2N multiplies a weight box with both:  D[:, 0:N] += A * Bhi,
+//     D[:, N:2N] += A * Blo * 2^11 (the fold scales it back; the lo halves stay normal fp16 numbers, with all 11 bits,
+//     when a loose bound on the columns leaves their values far below 2^14);
 //   * per 128-row tile the lo boxes go first, then the hi boxes: the tensor core adds into its fp32 accumulator
 //     with truncation, and the small products cost nothing while the accumulator is still small (max |error| 2.7e-6
 //     against fp64 for 512-term sums of magnitude ~3; the fp32 FMA chain of the FFMA kernel: 2.3e-6);
@@ -206,12 +208,13 @@ __device__ __forceinline__ void tc_tile(float (&acc)[TC::NACC], const unsigned c
   if (lane == 0) mbar_arrive(&b.empty[prev]);
 }
 
-// hi + lo column halves of a finished tile, scaled back: v[4 i + 2 h + e] <- row 8 h, column 8 i + 2 (lane % 4) + e
+// hi + lo column halves of a finished tile, scaled back: v[4 i + 2 h + e] <- row 8 h, column 8 i + 2 (lane % 4) + e.
+// The lo columns hold lo * 2^11 (tc_gather_b): the FMA scales them back exactly and rounds once.
 template <class TC>
 __device__ __forceinline__ void tc_fold(const float (&acc)[TC::NACC], float (&v)[TC::NV], float inv) {
   constexpr int LO = TC::NACC / 2;  // register offset of the lo halves (columns N .. 2N - 1)
 #pragma unroll
-  for (int i = 0; i < TC::NV; ++i) v[i] = __fmul_rn(__fadd_rn(acc[i], acc[LO + i]), inv);
+  for (int i = 0; i < TC::NV; ++i) v[i] = __fmul_rn(__fmaf_rn(acc[LO + i], 0x1p-11f, acc[i]), inv);
 }
 
 // ---- consumer warps: B operand ---------------------------------------------------------------------------------
@@ -240,7 +243,10 @@ __device__ __forceinline__ void tc_gather_b(unsigned char* bop, SrcFn src, int M
       if (m < Mp) {
         const float x0 = v[u].x * scale, x1 = v[u].y * scale;
         const __half h0 = __float2half_rn(x0), h1 = __float2half_rn(x1);
-        const __half l0 = __float2half_rn(x0 - __half2float(h0)), l1 = __float2half_rn(x1 - __half2float(h1));
+        // lo * 2^11 (exact before the rounding; |lo * 2^11| <= |hi|): stays a normal fp16 number, with its 11 bits,
+        // down to |x| ~ 2^-14 where x's own scale (a loose bound on the column) left the unscaled lo subnormal
+        const __half l0 = __float2half_rn((x0 - __half2float(h0)) * 2048.f);
+        const __half l1 = __float2half_rn((x1 - __half2float(h1)) * 2048.f);
         const uint32_t off = koff + (uint32_t)m * 128u + ((kchunk ^ ((uint32_t)m & 7u)) << 4);
         *reinterpret_cast<__half2*>(bop + off) = __halves2half2(h0, h1);
         *reinterpret_cast<__half2*>(bop + off + (uint32_t)N * 128u) = __halves2half2(l0, l1);

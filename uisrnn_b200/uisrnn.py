@@ -89,6 +89,34 @@ def _check_test_sequence(test_sequence, observation_dim):
     raise ValueError('test_sequence does not match the dimension specified by args.observation_dim.')
 
 
+class _Fingerprint:
+  """Parameter tensors (copied, or the live ones) and scalars, compared exactly: per device, one fused difference and
+  one fused max-norm of the tensors there, and one device -> host copy."""
+
+  def __init__(self, tensors, scalars, copy):
+    with torch.no_grad():
+      self.tensors = [t.detach().clone() if copy else t.detach() for t in tensors]
+    self.scalars = scalars
+
+  def __eq__(self, other):
+    if not isinstance(other, _Fingerprint) or self.scalars != other.scalars or len(self.tensors) != len(other.tensors):
+      return False
+    by_device = {}  # the parameters need not share a device (callers assign rnn_init_hidden / sigma2 freely)
+    for a, b in zip(self.tensors, other.tensors):
+      if a.shape != b.shape or a.dtype != b.dtype or a.device != b.device:
+        return False
+      by_device.setdefault(a.device, []).append((a, b))
+    with torch.no_grad():
+      for pairs in by_device.values():
+        diff = torch._foreach_sub([a for a, _ in pairs], [b for _, b in pairs])  # pylint: disable=protected-access
+        worst = torch.stack(torch._foreach_norm(diff, float('inf'))).max()  # pylint: disable=protected-access
+        if not worst.item() == 0:  # NaN (a NaN element, or inf - inf) is unequal
+          return False
+    return True
+
+  __hash__ = None
+
+
 class UISRNN:
   """Unbounded Interleaved-State Recurrent Neural Network."""
 
@@ -371,28 +399,14 @@ class UISRNN:
     self.fit_concatenated(sequence, cluster_id, args)
 
   # ------------------------------------------------------------------ inference
-  def _fingerprint(self):
-    """Identity of the parameter values the device-side twin was built from.  `_version` does not move on
-    edits through `.data` (an idiom the reference's own tests use), so a cheap content checksum -- the L2 and L1
-    norms of every tensor, two fused multi-tensor reductions -- is part of the key."""
+  def _fingerprint(self, copy=True):
+    """Identity of the parameter values the device-side twin is built from: equal to another fingerprint exactly when
+    every parameter has the same shape, dtype, device and elements (a NaN never equals), and the decoding scalars are
+    equal.  `_version` does not move on edits through `.data` (an idiom the reference's own tests use), and norms
+    miss edits that keep every |value| (a sign flip, a swap of rows), so the twin keeps a copy of the parameters
+    (copy=True) and each call compares the live ones (copy=False) with it."""
     tensors = list(self.rnn_model.parameters()) + [self.rnn_init_hidden, self.sigma2]
-    with torch.no_grad():
-      by_device = {}  # the parameters need not share a device (callers assign rnn_init_hidden / sigma2 freely)
-      for i, t in enumerate(tensors):
-        by_device.setdefault(t.device, []).append((i, t.detach()))
-      sums = [None] * len(tensors)
-      for parts in by_device.values():  # two fused multi-tensor reductions and one device -> host copy per device
-        ts = [t for _, t in parts]
-        try:
-          n2, n1 = torch._foreach_norm(ts, 2), torch._foreach_norm(ts, 1)  # pylint: disable=protected-access
-          flat = torch.stack(list(n2) + list(n1)).double().cpu().tolist()
-          pairs = list(zip(flat[:len(ts)], flat[len(ts):]))
-        except (AttributeError, RuntimeError, TypeError):  # no multi-tensor kernels in this torch: one by one
-          pairs = [tuple(torch.stack((t.double().norm(2), t.double().norm(1))).cpu().tolist()) for t in ts]
-        for (i, _), pair in zip(parts, pairs):
-          sums[i] = tuple(pair)
-    return (tuple((t.data_ptr(), t._version) for t in tensors), tuple(sums),
-            self.transition_bias, self.crp_alpha)
+    return _Fingerprint(tensors, (self.transition_bias, self.crp_alpha), copy)
 
   def export_weights(self):
     """Weights as float32 numpy arrays in the layout libuisrnn_b200.so / the oracle expect."""
@@ -414,11 +428,10 @@ class UISRNN:
     from . import native  # raises NativeError if the library has not been built
     index = (self.device.index or 0) if device_index is None else device_index
     with self._native_lock:
-      key = (self._fingerprint(), index)
-      if self._native is None or self._native[0] != key:
+      if self._native is None or self._native[0] != (self._fingerprint(copy=False), index):
         if self.transition_bias is None:
           raise TypeError('transition_bias is not set: call fit() or pass --transition_bias.')
-        self._native = (key, native.NativeModel(self.export_weights(), device=index))
+        self._native = ((self._fingerprint(), index), native.NativeModel(self.export_weights(), device=index))
       return self._native[1]
 
   def _predict_cuda(self, sequences, args, device_index=None, as_arrays=False, bounds=(None, None), n_best=None):
