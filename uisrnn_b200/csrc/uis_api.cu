@@ -423,7 +423,10 @@ int ensure_log_tables(uis_model* m, int max_tn, const DecodeParams& dp, uis::Bea
     if (int rc = upload(m->logn, ln.data(), cap * sizeof(double))) return rc;
     m->log_cap = cap;
   }
-  const bool own = dp.alpha == &m->alpha;
+  // the model's own pair (by value: the Python binding passes it as a one-pair sweep) keeps its own tables, so that
+  // alternating plain calls with a sweep does not rebuild a table on every call
+  const bool own = dp.count == 1 && std::memcmp(dp.alpha, &m->alpha, sizeof(double)) == 0 &&
+                   std::memcmp(dp.p0, &m->p0, sizeof(double)) == 0;
   uis_model::LogTables& t = own ? m->own_logs : m->sweep_logs;
   std::vector<double> key;
   for (int c = 0; c < dp.count; ++c) { key.push_back(dp.alpha[c]); key.push_back(dp.p0[c]); }
@@ -1271,6 +1274,29 @@ int uis_predict_device_sweep(uis_model* m, const float* x_dev, const int64_t* fr
 
 namespace {
 
+// Zero-pads the caller's `rows` device rows (D_user wide) to the kernel's row length D in m->x32 and points *x_dev
+// there; a model whose D_user is the kernel's D is left alone.
+int pad_to_kernel_d(uis_model* m, const float** x_dev, size_t rows, cudaStream_t st) {
+  if (m->D == m->D_user || rows == 0) return 0;
+  if (int rc = m->x32.ensure(rows * m->D * 4)) return rc;
+  const size_t np = rows * m->D;
+  const int blocks = (int)std::min<size_t>((np + 255) / 256, (size_t)m->num_sms * 16);
+  uis::pad_rows_f32_kernel<<<blocks, 256, 0, st>>>(*x_dev, m->x32.as<float>(), rows, m->D_user, m->D);
+  CU(cudaGetLastError());
+  *x_dev = m->x32.as<float>();
+  return 0;
+}
+
+// A failed call may leave copies / kernels in flight on either stream: drain them (the error already recorded in
+// uis_last_error() is the one reported) so that the staging ring and the workspace are quiescent for the next call.
+void drain_after_failure(uis_model* m, cudaStream_t st) {
+  const std::string keep = g_err;
+  if (m->copy_stream) cudaStreamSynchronize(m->copy_stream);
+  cudaStreamSynchronize(st);
+  (void)cudaGetLastError();
+  g_err = keep;
+}
+
 int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
                         const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
                         const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev,
@@ -1284,14 +1310,7 @@ int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_o
   uis::DeviceGuard device_guard_(m->device);
   CU(device_guard_.status);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (m->D != m->D_user && pl.rows > 0) {  // zero-pad the caller's rows to the kernel's row length
-    if (int rc = m->x32.ensure((size_t)pl.rows * m->D * 4)) return rc;
-    const size_t np = (size_t)pl.rows * m->D;
-    const int blocks = (int)std::min<size_t>((np + 255) / 256, (size_t)m->num_sms * 16);
-    uis::pad_rows_f32_kernel<<<blocks, 256, 0, st>>>(x_dev, m->x32.as<float>(), (size_t)pl.rows, m->D_user, m->D);
-    CU(cudaGetLastError());
-    x_dev = m->x32.as<float>();
-  }
+  if (int rc = pad_to_kernel_d(m, &x_dev, (size_t)pl.rows, st)) return rc;
   return run_device(m, x_dev, frame_offsets, U, pl, labels_dev, taps, st,
                     SpeakerBounds{max_speakers, min_speakers, speakers_dev}, nb, dp);
 }
@@ -1335,15 +1354,7 @@ int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n
                        const DecodeParams& dp) {
   const int rc = predict_host_group_impl(m, seqs, n_frames, U, off, pl, labels_out, taps, st, sb, speakers_out, nb, u0,
                                          U_all, dp);
-  if (rc != 0 && rc != UIS_ERR_OVERFLOW && rc != UIS_ERR_CAPACITY) {
-    // a failed call may leave copies / kernels in flight on either stream: drain them (the error already recorded in
-    // uis_last_error() is the one reported) so that the staging ring and the workspace are quiescent for the next call
-    const std::string keep = g_err;
-    if (m->copy_stream) cudaStreamSynchronize(m->copy_stream);
-    cudaStreamSynchronize(st);
-    (void)cudaGetLastError();
-    g_err = keep;
-  }
+  if (rc != 0 && rc != UIS_ERR_OVERFLOW && rc != UIS_ERR_CAPACITY) drain_after_failure(m, st);
   return rc;
 }
 
@@ -1900,13 +1911,7 @@ int score_host(uis_model* m, const double* const* seqs, const int64_t* n_frames,
   CU(device_guard_.status);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int rc = score_host_impl(m, seqs, n_frames, U, labels, scores_out, frame_out, st, dp);
-  if (rc != 0 && rc != UIS_ERR_INVALID) {  // drain what a failed call may have left in flight (see predict_host_group)
-    const std::string keep = g_err;
-    if (m->copy_stream) cudaStreamSynchronize(m->copy_stream);
-    cudaStreamSynchronize(st);
-    (void)cudaGetLastError();
-    g_err = keep;
-  }
+  if (rc != 0 && rc != UIS_ERR_INVALID) drain_after_failure(m, st);
   return rc;
 }
 
@@ -1934,14 +1939,7 @@ int score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets,
     CU(cudaMemsetAsync(scores_dev, 0, (size_t)U * dp.count * 4, st));  // empty utterances score 0
     return 0;
   }
-  if (m->D != m->D_user) {  // zero-pad the caller's rows to the kernel's row length
-    if (int rc = m->x32.ensure((size_t)rows * m->D * 4)) return rc;
-    const size_t np = (size_t)rows * m->D;
-    const int blocks = (int)std::min<size_t>((np + 255) / 256, (size_t)m->num_sms * 16);
-    uis::pad_rows_f32_kernel<<<blocks, 256, 0, st>>>(x_dev, m->x32.as<float>(), (size_t)rows, m->D_user, m->D);
-    CU(cudaGetLastError());
-    x_dev = m->x32.as<float>();
-  }
+  if (int rc = pad_to_kernel_d(m, &x_dev, (size_t)rows, st)) return rc;
   return run_score(m, x_dev, frame_offsets, U, cp, labels_dev, scores_dev, frame_dev, st, /*gi_ready=*/false, dp);
 }
 

@@ -10,7 +10,7 @@ import torch
 import torch.distributed as dist
 
 from . import native
-from .uisrnn import _warn_min_speakers, shard_by_frames
+from .uisrnn import _check_test_sequence, _warn_min_speakers, shard_by_frames
 
 
 def predict_sharded(model, test_sequences, args, group=None, lengths=None, root=None, as_arrays=False, *,
@@ -36,20 +36,16 @@ def predict_sharded(model, test_sequences, args, group=None, lengths=None, root=
     raise TypeError('test_sequences must be a list.')
   if lengths is not None and len(lengths) != len(test_sequences):
     raise ValueError('lengths must have one entry per test sequence.')
-  bounded = max_speakers is not None or min_speakers is not None
-  bounds = native.speaker_bounds(len(test_sequences), max_speakers, min_speakers) if bounded else (None, None)
+  bounds = native.speaker_bounds(len(test_sequences), max_speakers, min_speakers)
   if not (dist.is_available() and dist.is_initialized()):
-    if as_arrays or bounded:
-      labels = _predict_arrays(model, [_materialise(s) for s in test_sequences], args, range(len(test_sequences)),
-                               bounds)
-      return labels if as_arrays else [lab.tolist() for lab in labels]
-    return model.predict([_materialise(s) for s in test_sequences], args)
+    return _decode_labels(model, [_materialise(s) for s in test_sequences], args, range(len(test_sequences)), bounds,
+                          as_arrays)
   world = dist.get_world_size(group)
   rank = dist.get_rank(group)
   lengths = [len(s) for s in test_sequences] if lengths is None else [int(n) for n in lengths]
   shards = shard_by_frames(lengths, world)
-  mine = _predict_arrays(model, [_materialise(test_sequences[i]) for i in shards[rank]], args, shards[rank],
-                         bounds) if shards[rank] else []
+  mine = _decode_labels(model, [_materialise(test_sequences[i]) for i in shards[rank]], args, shards[rank], bounds,
+                        True) if shards[rank] else []
   counts = [sum(lengths[i] for i in shard) for shard in shards]
   use_cuda = getattr(model, 'device', None) is not None and model.device.type == 'cuda' and \
       dist.get_backend(group) == 'nccl'
@@ -82,24 +78,17 @@ def predict_sharded(model, test_sequences, args, group=None, lengths=None, root=
   return merged
 
 
-def _predict_arrays(model, sequences, args, indices, bounds):
-  """model.predict, but int32 arrays straight from the device when the model has the native path.  `indices`: the
-  positions of `sequences` in the caller's list; `bounds`: speaker bounds over that whole list (None = absent)."""
-  if bounds[0] is not None or bounds[1] is not None:
-    from .uisrnn import _check_test_sequence
-    for sequence in sequences:
-      _check_test_sequence(sequence, model.observation_dim)
-    indices = list(indices)
-    mine = tuple(b[indices] if b is not None else None for b in bounds)
-    labels, speakers = model._predict_bounded(sequences, args, mine, as_arrays=True)  # pylint: disable=protected-access
-    _warn_min_speakers(indices, [len(s) for s in sequences], speakers, mine[1])
-    return labels
-  if getattr(model, 'device', None) is not None and model.device.type == 'cuda' and hasattr(model, '_predict_cuda'):
-    from .uisrnn import _check_test_sequence
-    for sequence in sequences:
-      _check_test_sequence(sequence, model.observation_dim)  # the reference's TypeError / ValueError sites
-    return model._predict_cuda(sequences, args, as_arrays=True)  # pylint: disable=protected-access
-  return [np.asarray(o, dtype=np.int32) for o in model.predict(sequences, args)]
+def _decode_labels(model, sequences, args, indices, bounds, as_arrays):
+  """Hypothesis 0's labels of `sequences` (int32 arrays with as_arrays), one warning for those that fell short of
+  min_speakers.  `indices`: the positions of `sequences` in the caller's list; `bounds`: speaker bounds over that whole
+  list (None = absent)."""
+  for sequence in sequences:
+    _check_test_sequence(sequence, model.observation_dim)  # the reference's TypeError / ValueError sites
+  indices = list(indices)
+  mine = tuple(b[indices] if b is not None else None for b in bounds)
+  hyps, speakers = model._decode(sequences, args, mine, None, None, as_arrays)  # pylint: disable=protected-access
+  _warn_min_speakers([len(s) for s in sequences], speakers, mine[1], False, stacklevel=4, indices=indices)
+  return [np.asarray(lab, np.int32) for lab in hyps[0]] if as_arrays else hyps[0]
 
 
 def my_shard(lengths, group=None):

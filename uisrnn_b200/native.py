@@ -286,6 +286,17 @@ def _decode_struct(pairs):
   return DecodeParams(len(alpha), alpha.ctypes.data_as(dp), p0.ctypes.data_as(dp)), (alpha, p0), len(alpha)
 
 
+def _trim_taps(bufs, trace_utt):
+  """Debug taps cut to what the call wrote: the traced job's step rows and its best hypothesis' clusters."""
+  nrows = int(bufs['off'][-1]) if len(bufs['off']) else 0
+  bufs['win'] = bufs['win'][:nrows]
+  bufs['score'] = bufs['score'][:nrows]
+  k = int(bufs['final_k'][trace_utt]) if trace_utt >= 0 else 0
+  for key in ('best_mean', 'best_hidden', 'best_blocks'):
+    bufs[key] = bufs[key][:k]
+  return bufs
+
+
 class NativeModel:
   """Owns a `uis_model*`.  Weights are numpy arrays in PyTorch state_dict layout."""
 
@@ -315,8 +326,13 @@ class NativeModel:
       if e is not None and tuple(a.shape) != e:
         raise ValueError('weight shape {} != expected {}'.format(a.shape, e))
     ptrs = [a.ctypes.data_as(C.c_void_p) for a in arrs]
+    self.crp_alpha, self.transition_bias = float(w['crp_alpha']), float(w['transition_bias'])
     _check(lib, lib.uis_model_create(C.byref(self._h), device, self.D, self.H, depth, *ptrs,
-                                     float(w['transition_bias']), float(w['crp_alpha'])))
+                                     self.transition_bias, self.crp_alpha))
+    # the model's own pair as a one-pair sweep: the call every entry point without decode_params makes
+    self._own = (np.array([self.crp_alpha]), np.array([self.transition_bias]))
+    dp = C.POINTER(C.c_double)
+    self._own_dp = DecodeParams(1, self._own[0].ctypes.data_as(dp), self._own[1].ctypes.data_as(dp))
 
   def close(self):
     if getattr(self, '_h', None) is not None and self._h:
@@ -365,73 +381,50 @@ class NativeModel:
                   bufs['best_blocks'].ctypes.data_as(ip))
     return t, bufs
 
+  def _rows(self, seqs):
+    """(arrays, lengths, offsets) of host utterances: each as a C-contiguous float64 [N_u, D] array (the caller's own
+    when it already is one), their int64 lengths (one 0 entry for an empty list) and frame offsets [U + 1]."""
+    n = len(seqs)
+    keep = [s if (type(s) is np.ndarray and s.dtype == np.float64 and s.flags.c_contiguous)
+            else np.ascontiguousarray(s, dtype=np.float64) for s in seqs]
+    for s in keep:
+      if s.ndim != 2 or s.shape[1] != self.D:
+        raise ValueError('utterance shape {} does not match D={}'.format(s.shape, self.D))
+    lens = np.fromiter((s.shape[0] for s in keep), dtype=np.int64, count=n) if n else np.zeros(1, np.int64)
+    offs = np.zeros(n + 1, np.int64)
+    np.cumsum(lens[:n], out=offs[1:])
+    return keep, lens, offs
+
+  def _sweep(self, decode_params):
+    """(DecodeParams, keep-alive arrays, count) of a sweep; None is the model's own pair."""
+    return (self._own_dp, None, 1) if decode_params is None else _decode_struct(decode_params)
+
   def predict(self, seqs, beam_size=10, look_ahead=1, test_iteration=2, kcap=0, n_ctas=0,
               trace_utt=None, stream=0, lanes=0, cluster=0, engine=0, max_speakers=None, min_speakers=None,
               return_speakers=False, n_best=None):
     """seqs: list of C-contiguous float64 [N_u, D] arrays (host).  Returns a list of int32
     label arrays (and a dict of debug arrays when trace_utt is not None).
 
-    n_best=k (1 <= k <= beam_size, uis_predict_nbest): returns (labels, scores, speakers, count) instead, where
-    labels[u] is int32 [k][N_u] (row 0 = the labels of the same call without n_best), scores float32 [U][k]
-    (neg_likelihood, +inf where absent), speakers int32 [U][k] and count int32 [U]; return_speakers is ignored.
+    n_best=k (1 <= k <= beam_size): returns (labels, scores, speakers, count) instead, where labels[u] is int32
+    [k][N_u] (row 0 = the labels of the same call without n_best), scores float32 [U][k] (neg_likelihood, +inf where
+    absent), speakers int32 [U][k] and count int32 [U]; return_speakers is ignored.
 
     max_speakers / min_speakers: an int for every utterance or one value per utterance, 0 = no bound
     (uis_predict_bounded in include/uisrnn_b200.h).  return_speakers=True appends an int32 array with the
-    cluster count of every returned hypothesis to the result."""
-    n = len(seqs)
-    mx, mn = speaker_bounds(n, max_speakers, min_speakers)
-    k = 1 if n_best is None else check_n_best(n_best, beam_size)
-    keep = [s if (type(s) is np.ndarray and s.dtype == np.float64 and s.flags.c_contiguous)
-            else np.ascontiguousarray(s, dtype=np.float64) for s in seqs]
-    for s in keep:
-      if s.ndim != 2 or s.shape[1] != self.D:
-        raise ValueError('utterance shape {} does not match D={}'.format(s.shape, self.D))
-    # one flat int32 output buffer; the per-utterance pointers are base + 4 * offsets (no per-utterance allocation)
-    lens = np.fromiter((s.shape[0] for s in keep), dtype=np.int64, count=n) if n else np.zeros(1, np.int64)
-    offs = np.zeros(n + 1, np.int64)
-    np.cumsum(lens[:n], out=offs[1:])
-    flat = np.empty(max(k * int(offs[-1]), 1), np.int32)
-    outs = [flat[k * offs[i]:k * offs[i + 1]] for i in range(n)]
-    out_addr = (flat.ctypes.data + 4 * k * offs[:max(n, 1)]).astype(np.uint64)
-    in_addr = np.fromiter((s.ctypes.data for s in keep), dtype=np.uint64, count=n) if n else np.zeros(1, np.uint64)
-    lengths = lens.ctypes.data_as(C.POINTER(C.c_int64))
-    in_ptrs = in_addr.ctypes.data_as(C.POINTER(C.c_void_p))
-    out_ptrs = out_addr.ctypes.data_as(C.POINTER(C.c_void_p))
-    opts = self._opts(beam_size, look_ahead, test_iteration, kcap, n_ctas, lanes, cluster, engine)
-    taps, bufs, tp = None, None, None
-    if trace_utt is not None:
-      taps, bufs = self._taps(trace_utt, n, [s.shape[0] for s in keep], beam_size, look_ahead,
-                              test_iteration, kcap)
-      tp = C.byref(taps)
-    ip = C.POINTER(C.c_int32)
-    spk = np.zeros(max(n, 1), np.int32) if return_speakers else None
-    arg = lambda a: a.ctypes.data_as(ip) if a is not None else None
-    if n_best is None:
-      rc = self._lib.uis_predict_bounded(self._h, in_ptrs, lengths, n, C.byref(opts), out_ptrs, tp,
-                                         C.c_void_p(stream), arg(mx), arg(mn), arg(spk))
-    else:
-      scores = np.empty((max(n, 1), k), np.float32)
-      nb_spk = np.empty((max(n, 1), k), np.int32)
-      count = np.empty(max(n, 1), np.int32)
-      nb = NBestOut(out_ptrs, None, scores.ctypes.data_as(C.POINTER(C.c_float)), nb_spk.ctypes.data_as(ip),
-                    count.ctypes.data_as(ip))
-      rc = self._lib.uis_predict_nbest(self._h, in_ptrs, lengths, n, C.byref(opts), tp, C.c_void_p(stream),
-                                       arg(mx), arg(mn), k, C.byref(nb))
-    _check(self._lib, rc)
+    cluster count of every returned hypothesis to the result.
+
+    This is predict_sweep() under the model's own pair, reshaped: hypothesis 0 at n_best 1 is what uis_predict_bounded
+    returns."""
+    out = self.predict_sweep(seqs, None, beam_size, look_ahead, test_iteration, kcap, n_ctas, trace_utt, stream, lanes,
+                             cluster, engine, max_speakers, min_speakers, n_best)
+    (labels, scores, speakers, count), bufs = out if trace_utt is not None else (out, None)
     if n_best is not None:
-      outs = ([o.reshape(k, int(lens[i])) for i, o in enumerate(outs)], scores[:n], nb_spk[:n], count[:n])
+      out = ([lab[0] for lab in labels], scores[0], speakers[0], count[0])
     elif return_speakers:
-      outs = (outs, spk[:n])
-    if bufs is not None:
-      nrows = int(bufs['off'][-1]) if len(bufs['off']) else 0
-      bufs['win'] = bufs['win'][:nrows]
-      bufs['score'] = bufs['score'][:nrows]
-      k = int(bufs['final_k'][trace_utt]) if trace_utt >= 0 else 0
-      bufs['best_mean'] = bufs['best_mean'][:k]
-      bufs['best_hidden'] = bufs['best_hidden'][:k]
-      bufs['best_blocks'] = bufs['best_blocks'][:k]
-      return outs, bufs
-    return outs
+      out = ([lab[0, 0] for lab in labels], speakers[0, :, 0])
+    else:
+      out = [lab[0, 0] for lab in labels]
+    return (out, bufs) if bufs is not None else out
 
   def predict_device(self, x_ptr, frame_offsets, labels_ptr, beam_size=10, look_ahead=1,
                      test_iteration=2, kcap=0, n_ctas=0, stream=0, lanes=0, cluster=0, engine=0,
@@ -441,21 +434,18 @@ class NativeModel:
     device addresses, e.g. torch.Tensor.data_ptr()).  Asynchronous on `stream`.  Speaker bounds as in
     predict(); speakers_ptr (device int32 [U], 0 = none) receives the cluster counts.
 
-    n_best=k (uis_predict_device_nbest): labels_ptr -> int32 [k][rows]; scores_ptr -> float32 [U][k] (required),
-    nbest_speakers_ptr -> int32 [U][k] and count_ptr -> int32 [U] (0 = none); speakers_ptr is ignored."""
+    n_best=k (predict_device_sweep under the model's own pair): labels_ptr -> int32 [k][rows]; scores_ptr -> float32
+    [U][k] (required), nbest_speakers_ptr -> int32 [U][k] and count_ptr -> int32 [U] (0 = none); speakers_ptr is
+    ignored."""
+    if n_best is not None:
+      self.predict_device_sweep(x_ptr, frame_offsets, labels_ptr, scores_ptr, None, beam_size, look_ahead,
+                                test_iteration, kcap, n_ctas, stream, lanes, cluster, engine, max_speakers,
+                                min_speakers, n_best, nbest_speakers_ptr, count_ptr)
+      return
     off = np.ascontiguousarray(frame_offsets, dtype=np.int64)
     mx, mn = speaker_bounds(len(off) - 1, max_speakers, min_speakers)
     ip = C.POINTER(C.c_int32)
     opts = self._opts(beam_size, look_ahead, test_iteration, kcap, n_ctas, lanes, cluster, engine)
-    if n_best is not None:
-      k = check_n_best(n_best, beam_size)
-      nb = NBestOut(None, C.c_void_p(labels_ptr), C.cast(C.c_void_p(scores_ptr), C.POINTER(C.c_float)),
-                    C.cast(C.c_void_p(nbest_speakers_ptr), ip), C.cast(C.c_void_p(count_ptr), ip))
-      _check(self._lib, self._lib.uis_predict_device_nbest(
-          self._h, C.c_void_p(x_ptr), off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1, C.byref(opts), None,
-          C.c_void_p(stream), mx.ctypes.data_as(ip) if mx is not None else None,
-          mn.ctypes.data_as(ip) if mn is not None else None, k, C.byref(nb)))
-      return
     rc = self._lib.uis_predict_device_bounded(self._h, C.c_void_p(x_ptr),
                                               off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1,
                                               C.byref(opts), C.c_void_p(labels_ptr), None,
@@ -471,23 +461,18 @@ class NativeModel:
     """predict() under C (crp_alpha, transition_bias) pairs in one call (uis_predict_sweep).  Returns (labels, scores,
     speakers, count): labels[u] int32 [C][k][N_u], scores float32 [C][U][k], speakers int32 [C][U][k], count int32
     [C][U]; config c's entries are what predict(..., n_best=k) returns for a model created with pair c.  trace_utt
-    names a job (c * U + u); the taps' final_scores / final_k are [C * U][...]."""
+    names a job (c * U + u); the taps' final_scores / final_k are [C * U][...].  decode_params=None is the model's
+    own pair (C = 1); n_best=None runs as 1."""
     n = len(seqs)
-    dp, keep_dp, nc = _decode_struct(decode_params)
+    dp, keep_dp, nc = self._sweep(decode_params)
     mx, mn = speaker_bounds(n, max_speakers, min_speakers)
-    k = check_n_best(n_best, beam_size)
-    keep = [s if (type(s) is np.ndarray and s.dtype == np.float64 and s.flags.c_contiguous)
-            else np.ascontiguousarray(s, dtype=np.float64) for s in seqs]
-    for s in keep:
-      if s.ndim != 2 or s.shape[1] != self.D:
-        raise ValueError('utterance shape {} does not match D={}'.format(s.shape, self.D))
-    lens = np.array([s.shape[0] for s in keep] or [0], np.int64)
-    offs = np.zeros(n + 1, np.int64)
-    np.cumsum(lens[:n], out=offs[1:])
+    k = 1 if n_best is None else check_n_best(n_best, beam_size)
+    keep, lens, offs = self._rows(seqs)
+    # one flat int32 output buffer; the per-utterance pointers are base + 4 * offsets (no per-utterance allocation)
     flat = np.empty(max(nc * k * int(offs[-1]), 1), np.int32)
     outs = [flat[nc * k * offs[i]:nc * k * offs[i + 1]] for i in range(n)]
     out_addr = (flat.ctypes.data + 4 * nc * k * offs[:max(n, 1)]).astype(np.uint64)
-    in_addr = np.array([s.ctypes.data for s in keep] or [0], np.uint64)
+    in_addr = np.fromiter((s.ctypes.data for s in keep), dtype=np.uint64, count=n) if n else np.zeros(1, np.uint64)
     opts = self._opts(beam_size, look_ahead, test_iteration, kcap, n_ctas, lanes, cluster, engine)
     taps, bufs, tp = None, None, None
     if trace_utt is not None:
@@ -507,25 +492,16 @@ class NativeModel:
     del keep_dp
     # (a list of U utterances is held as [C][U][k]; with n == 0 the padding row is dropped)
     out = ([o.reshape(nc, k, int(lens[i])) for i, o in enumerate(outs)], scores[:, :n], spk[:, :n], count[:, :n])
-    if bufs is not None:
-      nrows = int(bufs['off'][-1]) if len(bufs['off']) else 0
-      bufs['win'] = bufs['win'][:nrows]
-      bufs['score'] = bufs['score'][:nrows]
-      kk = int(bufs['final_k'][trace_utt]) if trace_utt >= 0 else 0
-      bufs['best_mean'] = bufs['best_mean'][:kk]
-      bufs['best_hidden'] = bufs['best_hidden'][:kk]
-      bufs['best_blocks'] = bufs['best_blocks'][:kk]
-      return out, bufs
-    return out
+    return (out, _trim_taps(bufs, trace_utt)) if bufs is not None else out
 
   def predict_device_sweep(self, x_ptr, frame_offsets, labels_ptr, scores_ptr, decode_params, beam_size=10,
                            look_ahead=1, test_iteration=2, kcap=0, n_ctas=0, stream=0, lanes=0, cluster=0, engine=0,
                            max_speakers=None, min_speakers=None, n_best=1, speakers_ptr=0, count_ptr=0):
     """Device-resident sweep (uis_predict_device_sweep): labels_ptr -> int32 [C][k][rows], scores_ptr -> float32
     [C][U][k] (required), speakers_ptr -> int32 [C][U][k], count_ptr -> int32 [C][U] (0 = none).  Asynchronous on
-    `stream`."""
+    `stream`.  decode_params=None is the model's own pair (C = 1)."""
     off = np.ascontiguousarray(frame_offsets, dtype=np.int64)
-    dp, keep_dp, _ = _decode_struct(decode_params)
+    dp, keep_dp, _ = self._sweep(decode_params)
     mx, mn = speaker_bounds(len(off) - 1, max_speakers, min_speakers)
     k = check_n_best(n_best, beam_size)
     ip = C.POINTER(C.c_int32)
@@ -539,50 +515,28 @@ class NativeModel:
     del keep_dp
 
   def score(self, seqs, labels, per_frame=False):
-    """neg_likelihood of given labellings (uis_score): seqs is a list of float64 [N_u, D] arrays (host), labels a
-    list of canonical int label sequences (0, 1, 2, ... in order of first appearance), one of length N_u per
-    utterance.  Returns float32 scores [U]; with per_frame, (scores, list of float32 [N_u] per-frame increments)."""
-    if not isinstance(seqs, (list, tuple)) or not isinstance(labels, (list, tuple)):
-      raise TypeError('seqs and labels must be lists')
-    if len(seqs) != len(labels):
-      raise ValueError('{} utterances but {} label sequences'.format(len(seqs), len(labels)))
-    n = len(seqs)
-    keep = [s if (type(s) is np.ndarray and s.dtype == np.float64 and s.flags.c_contiguous)
-            else np.ascontiguousarray(s, dtype=np.float64) for s in seqs]
-    labs = [np.ascontiguousarray(l, dtype=np.int32) for l in labels]
-    for u, (s, l) in enumerate(zip(keep, labs)):
-      if s.ndim != 2 or s.shape[1] != self.D:
-        raise ValueError('utterance shape {} does not match D={}'.format(s.shape, self.D))
-      if l.ndim != 1 or len(l) != s.shape[0]:
-        raise ValueError('utterance {}: {} labels for {} frames'.format(u, l.size, s.shape[0]))
-    lens = np.array([s.shape[0] for s in keep] or [0], np.int64)
-    scores = np.zeros(max(n, 1), np.float32)
-    frames = [np.empty(s.shape[0], np.float32) for s in keep] if per_frame else None
-    ptrs = lambda arrs: (C.c_void_p * max(len(arrs), 1))(*[a.ctypes.data for a in arrs])
-    _check(self._lib, self._lib.uis_score(
-        self._h, C.cast(ptrs(keep), C.POINTER(C.c_void_p)), lens.ctypes.data_as(C.POINTER(C.c_int64)), n,
-        C.cast(ptrs(labs), C.POINTER(C.c_void_p)), scores.ctypes.data_as(C.POINTER(C.c_float)),
-        C.cast(ptrs(frames), C.POINTER(C.c_void_p)) if per_frame else None, None))
-    return (scores[:n], frames) if per_frame else scores[:n]
+    """neg_likelihood of given labellings: seqs is a list of float64 [N_u, D] arrays (host), labels a list of
+    canonical int label sequences (0, 1, 2, ... in order of first appearance), one of length N_u per utterance.
+    Returns float32 scores [U]; with per_frame, (scores, list of float32 [N_u] per-frame increments).  This is
+    score_sweep() under the model's own pair."""
+    out = self.score_sweep(seqs, labels, None, per_frame)
+    return (out[0][0], [f[0] for f in out[1]]) if per_frame else out[0]
 
   def score_sweep(self, seqs, labels, decode_params, per_frame=False):
     """score() under C (crp_alpha, transition_bias) pairs in one call (uis_score_sweep): float32 scores [C][U]; with
-    per_frame, (scores, list of float32 [C][N_u] per-frame increments)."""
+    per_frame, (scores, list of float32 [C][N_u] per-frame increments).  decode_params=None is the model's own pair
+    (C = 1)."""
     if not isinstance(seqs, (list, tuple)) or not isinstance(labels, (list, tuple)):
       raise TypeError('seqs and labels must be lists')
     if len(seqs) != len(labels):
       raise ValueError('{} utterances but {} label sequences'.format(len(seqs), len(labels)))
-    dp, keep_dp, nc = _decode_struct(decode_params)
+    dp, keep_dp, nc = self._sweep(decode_params)
     n = len(seqs)
-    keep = [s if (type(s) is np.ndarray and s.dtype == np.float64 and s.flags.c_contiguous)
-            else np.ascontiguousarray(s, dtype=np.float64) for s in seqs]
+    keep, lens, _ = self._rows(seqs)
     labs = [np.ascontiguousarray(l, dtype=np.int32) for l in labels]
     for u, (s, l) in enumerate(zip(keep, labs)):
-      if s.ndim != 2 or s.shape[1] != self.D:
-        raise ValueError('utterance shape {} does not match D={}'.format(s.shape, self.D))
       if l.ndim != 1 or len(l) != s.shape[0]:
         raise ValueError('utterance {}: {} labels for {} frames'.format(u, l.size, s.shape[0]))
-    lens = np.array([s.shape[0] for s in keep] or [0], np.int64)
     scores = np.zeros((nc, max(n, 1)), np.float32)
     frames = [np.empty((nc, s.shape[0]), np.float32) for s in keep] if per_frame else None
     ptrs = lambda arrs: (C.c_void_p * max(len(arrs), 1))(*[a.ctypes.data for a in arrs])
@@ -595,22 +549,20 @@ class NativeModel:
 
   def score_device_sweep(self, x_ptr, frame_offsets, labels_ptr, scores_ptr, decode_params, frame_ptr=0, stream=0):
     """Device-resident score sweep (uis_score_device_sweep): scores_ptr -> float32 [C][U], frame_ptr -> float32
-    [C][rows] (0 = none)."""
+    [C][rows] (0 = none).  decode_params=None is the model's own pair (C = 1)."""
     off = np.ascontiguousarray(frame_offsets, dtype=np.int64)
-    dp, keep_dp, _ = _decode_struct(decode_params)
+    dp, keep_dp, _ = self._sweep(decode_params)
     _check(self._lib, self._lib.uis_score_device_sweep(
         self._h, C.c_void_p(x_ptr), off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1, C.c_void_p(labels_ptr),
         C.c_void_p(scores_ptr), C.c_void_p(frame_ptr), C.c_void_p(stream), C.byref(dp)))
     del keep_dp
 
   def score_device(self, x_ptr, frame_offsets, labels_ptr, scores_ptr, frame_ptr=0, stream=0):
-    """Device-resident variant (uis_score_device): x_ptr -> fp32 [rows, D], labels_ptr -> canonical int32 [rows],
-    scores_ptr -> float32 [U], frame_ptr -> float32 [rows] per-frame increments (0 = none); raw device addresses.
-    Reads the labels back once to plan the chains, then enqueues the kernels on `stream` without waiting."""
-    off = np.ascontiguousarray(frame_offsets, dtype=np.int64)
-    _check(self._lib, self._lib.uis_score_device(
-        self._h, C.c_void_p(x_ptr), off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1, C.c_void_p(labels_ptr),
-        C.c_void_p(scores_ptr), C.c_void_p(frame_ptr), C.c_void_p(stream)))
+    """Device-resident variant: x_ptr -> fp32 [rows, D], labels_ptr -> canonical int32 [rows], scores_ptr -> float32
+    [U], frame_ptr -> float32 [rows] per-frame increments (0 = none); raw device addresses.  Reads the labels back once
+    to plan the chains, then enqueues the kernels on `stream` without waiting.  This is score_device_sweep() under the
+    model's own pair, whose [1][U] / [1][rows] outputs are these layouts."""
+    self.score_device_sweep(x_ptr, frame_offsets, labels_ptr, scores_ptr, None, frame_ptr, stream)
 
   def stats(self):
     s = Stats()

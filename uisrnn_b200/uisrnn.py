@@ -434,36 +434,41 @@ class UISRNN:
         self._native = ((self._fingerprint(), index), native.NativeModel(self.export_weights(), device=index))
       return self._native[1]
 
-  def _predict_cuda(self, sequences, args, device_index=None, as_arrays=False, bounds=(None, None), n_best=None):
-    """Labels of `sequences` from the native library; with speaker bounds (int32 arrays from
-    native.speaker_bounds, None = absent) returns (labels, cluster counts); with n_best, (NBest list, cluster
-    counts of hypothesis 0)."""
-    return _native_predict(self._native_model(device_index), sequences, args, as_arrays, bounds, n_best)
-
-  def _decode_cpu(self, sequence, args, max_speakers=0, min_speakers=0):
-    """(labels, cluster count) of one sequence on the CPU device."""
-    decoder = beam_cpu.CpuBeamSearch(self)
-    return decoder.decode(sequence, args.beam_size, args.look_ahead, args.test_iteration, int(max_speakers),
-                          int(min_speakers), return_speakers=True)
-
-  def _predict_bounded(self, sequences, args, bounds, as_arrays=False):
-    """(labels, cluster counts) of a checked list of sequences under per-utterance speaker bounds."""
+  def _decode(self, sequences, args, bounds, n_best, pairs, as_arrays=False):
+    """The one decode behind every predict entry point, of checked `sequences` under speaker `bounds` ((max, min) int32
+    arrays from native.speaker_bounds, None = absent), `n_best` and `pairs` (checked (crp_alpha, transition_bias) pairs,
+    None = the model's own).  Returns (hypotheses, speakers): hypotheses[c][u] is the NBest of utterance u under pair c
+    with n_best, else its hypothesis 0's labels (an int32 array on CUDA with as_arrays, else a list of ints; empty for
+    an empty utterance); speakers[c][u] is the cluster count of hypothesis 0 (0 for an empty utterance)."""
     if self.device.type == 'cuda':
-      return self._predict_cuda(sequences, args, as_arrays=as_arrays, bounds=bounds)
+      return _native_decode(self._native_model(), sequences, args, bounds, n_best, pairs, as_arrays)
     mx, mn = bounds
-    out = [self._decode_cpu(s, args, mx[i] if mx is not None else 0, mn[i] if mn is not None else 0)
-           for i, s in enumerate(sequences)]
-    labels = [np.asarray(o[0], np.int32) if as_arrays else o[0] for o in out]
-    return labels, np.array([o[1] for o in out], np.int32)
+    hyps, speakers = [], []
+    for alpha, bias in pairs or [(self.crp_alpha, self.transition_bias)]:
+      decoder = beam_cpu.CpuBeamSearch(self, crp_alpha=alpha, transition_bias=bias)
+      outs = [decoder.decode(s, args.beam_size, args.look_ahead, args.test_iteration,
+                             int(mx[u]) if mx is not None else 0, int(mn[u]) if mn is not None else 0,
+                             n_best=n_best or 1) for u, s in enumerate(sequences)]
+      hyps.append([NBest(*o) if n_best else (o[0][0] if o[0] else []) for o in outs])
+      speakers.append([o[2][0] if o[2] else 0 for o in outs])
+    return hyps, speakers
 
-  def _predict_nbest(self, sequences, args, bounds, n_best):
-    """(NBest list, cluster counts of hypothesis 0) of a checked list of sequences."""
-    if self.device.type == 'cuda':
-      return self._predict_cuda(sequences, args, bounds=bounds, n_best=n_best)
-    mx, mn = bounds
-    out = [_decode_cpu_nbest(self, args, n_best, s, mx[i] if mx is not None else 0, mn[i] if mn is not None else 0)
-           for i, s in enumerate(sequences)]
-    return out, np.array([o.speakers[0] if o.speakers else 0 for o in out], np.int32)
+  def _predict(self, test_sequences, args, max_speakers, min_speakers, n_best, pairs):
+    """predict() of an ndarray or a list, after decode_params was checked (pairs, None = none given)."""
+    single = isinstance(test_sequences, np.ndarray)
+    if not single and not isinstance(test_sequences, list):
+      raise TypeError('test_sequences should be either a list or numpy array.')
+    sequences = [test_sequences] if single else test_sequences
+    for sequence in sequences:
+      _check_test_sequence(sequence, self.observation_dim)
+    if single and (np.ndim(max_speakers) or np.ndim(min_speakers)):
+      raise ValueError('predict_single takes one int per bound')
+    k = _check_n_best(n_best, args) if n_best is not None else None
+    bounds = _speaker_bounds(len(sequences), max_speakers, min_speakers)
+    hyps, speakers = self._decode(sequences, args, bounds, k, pairs)
+    _warn_min_speakers([len(s) for s in sequences], speakers, bounds[1], pairs is not None, stacklevel=4)
+    out = [row[0] for row in hyps] if single else hyps
+    return out if pairs is not None else out[0]
 
   def predict_single(self, test_sequence, args, *, max_speakers=None, min_speakers=None, n_best=None):
     """Labels (list of N ints) for one test sequence [N, D] float64 (uisrnn.py:479-562).
@@ -471,24 +476,7 @@ class UISRNN:
     max_speakers / min_speakers (ints, 0 or None = no bound) bound the number of speakers, and n_best returns
     an NBest instead: see `predict`."""
     _check_test_sequence(test_sequence, self.observation_dim)
-    if n_best is not None:
-      if np.ndim(max_speakers) or np.ndim(min_speakers):
-        raise ValueError('predict_single takes one int per bound')
-      k = _check_n_best(n_best, args)
-      bounds = _speaker_bounds(1, max_speakers, min_speakers)
-      out, speakers = self._predict_nbest([test_sequence], args, bounds, k)
-      _warn_min_speakers([0], [len(test_sequence)], speakers, bounds[1])
-      return out[0]
-    if max_speakers is None and min_speakers is None:
-      if self.device.type == 'cuda':
-        return self._predict_cuda([test_sequence], args)[0]
-      return self._decode_cpu(test_sequence, args)[0]
-    if np.ndim(max_speakers) or np.ndim(min_speakers):
-      raise ValueError('predict_single takes one int per bound')
-    bounds = _speaker_bounds(1, max_speakers, min_speakers)
-    labels, speakers = self._predict_bounded([test_sequence], args, bounds)
-    _warn_min_speakers([0], [len(test_sequence)], speakers, bounds[1])
-    return labels[0]
+    return self._predict(test_sequence, args, max_speakers, min_speakers, n_best, None)
 
   def predict(self, test_sequences, args, *, max_speakers=None, min_speakers=None, n_best=None, decode_params=None):
     """Labels for one sequence (ndarray -> list of ints) or many (list -> list of lists)
@@ -515,74 +503,8 @@ class UISRNN:
     crp_alpha / transition_bias are pair c (bounds and n_best apply to every pair).  The model is not changed.  On a
     CUDA device the whole grid is one native call: the inputs are copied and projected once.  Pick a pair by scoring
     each entry on a labelled dev set (e.g. `evals.compute_sequence_match_accuracy`)."""
-    if decode_params is not None:
-      return self._predict_sweep(test_sequences, args, max_speakers, min_speakers, n_best, decode_params)
-    if isinstance(test_sequences, np.ndarray):
-      return self.predict_single(test_sequences, args, max_speakers=max_speakers, min_speakers=min_speakers,
-                                 n_best=n_best)
-    if isinstance(test_sequences, list) and n_best is not None:
-      k = _check_n_best(n_best, args)
-      for sequence in test_sequences:
-        _check_test_sequence(sequence, self.observation_dim)
-      bounds = _speaker_bounds(len(test_sequences), max_speakers, min_speakers)
-      out, speakers = self._predict_nbest(test_sequences, args, bounds, k)
-      _warn_min_speakers(range(len(test_sequences)), [len(s) for s in test_sequences], speakers, bounds[1])
-      return out
-    if isinstance(test_sequences, list):
-      if max_speakers is not None or min_speakers is not None:
-        for sequence in test_sequences:
-          _check_test_sequence(sequence, self.observation_dim)
-        bounds = _speaker_bounds(len(test_sequences), max_speakers, min_speakers)
-        labels, speakers = self._predict_bounded(test_sequences, args, bounds)
-        _warn_min_speakers(range(len(test_sequences)), [len(s) for s in test_sequences], speakers, bounds[1])
-        return labels
-      if self.device.type == 'cuda':
-        for sequence in test_sequences:
-          _check_test_sequence(sequence, self.observation_dim)
-        return self._predict_cuda(test_sequences, args)
-      return [self.predict_single(sequence, args) for sequence in test_sequences]
-    raise TypeError('test_sequences should be either a list or numpy array.')
-
-  def _predict_sweep(self, test_sequences, args, max_speakers, min_speakers, n_best, decode_params):
-    """predict() under every (crp_alpha, transition_bias) pair of `decode_params`: one entry per pair."""
-    pairs = _decode_params(decode_params)
-    single = isinstance(test_sequences, np.ndarray)
-    if single:
-      if np.ndim(max_speakers) or np.ndim(min_speakers):
-        raise ValueError('predict_single takes one int per bound')
-      sequences = [test_sequences]
-    elif isinstance(test_sequences, list):
-      sequences = test_sequences
-    else:
-      raise TypeError('test_sequences should be either a list or numpy array.')
-    for sequence in sequences:
-      _check_test_sequence(sequence, self.observation_dim)
-    k = _check_n_best(n_best, args) if n_best is not None else None
-    bounds = _speaker_bounds(len(sequences), max_speakers, min_speakers)
-    if self.device.type == 'cuda':
-      results, speakers = _native_predict_sweep(self._native_model(), sequences, args, bounds, k, pairs)
-    else:
-      mx, mn = bounds
-      results, speakers = [], []
-      for alpha, bias in pairs:
-        decoder = beam_cpu.CpuBeamSearch(self, crp_alpha=alpha, transition_bias=bias)
-        outs = [decoder.decode(s, args.beam_size, args.look_ahead, args.test_iteration,
-                               int(mx[i]) if mx is not None else 0, int(mn[i]) if mn is not None else 0,
-                               return_speakers=True, n_best=k) for i, s in enumerate(sequences)]
-        if k is None:
-          results.append([o[0] for o in outs])
-          speakers.append([o[1] for o in outs])
-        else:
-          results.append([NBest(*o) for o in outs])
-          speakers.append([o[2][0] if o[2] else 0 for o in outs])
-    if bounds[1] is not None:
-      lengths = [len(s) for s in sequences]
-      short = [(u, c) for c, row in enumerate(speakers)
-               for u, (n, got, lo) in enumerate(zip(lengths, row, bounds[1])) if n > 0 and got < lo]
-      if short:
-        warnings.warn('min_speakers: the final beam of (utterance, pair) {} held no hypothesis with that many '
-                      'speakers; the best hypothesis was returned instead'.format(short), RuntimeWarning, stacklevel=3)
-    return [r[0] for r in results] if single else results
+    pairs = _decode_params(decode_params) if decode_params is not None else None
+    return self._predict(test_sequences, args, max_speakers, min_speakers, n_best, pairs)
 
   def score(self, test_sequences, test_cluster_ids, *, per_frame=False, decode_params=None):
     """The neg_likelihood the model gives to given speaker labellings (not in the reference, where it exists only
@@ -616,31 +538,20 @@ class UISRNN:
     for u, (sequence, lab) in enumerate(zip(test_sequences, labels)):
       if len(lab) != len(sequence):
         raise ValueError('utterance {}: {} labels for {} frames'.format(u, len(lab), len(sequence)))
-    if pairs is not None:
-      if self.device.type == 'cuda':
-        model = self._native_model()
-        with model.lock:
-          out = model.score_sweep(test_sequences, labels, pairs, per_frame=per_frame)
-        if not per_frame:
-          return [[float(v) for v in row] for row in out]
-        totals, increments = out
-        return [[FrameScores(float(v), inc[c]) for v, inc in zip(row, increments)] for c, row in enumerate(totals)]
-      result = []
-      for alpha, bias in pairs:
-        decoder = beam_cpu.CpuBeamSearch(self, crp_alpha=alpha, transition_bias=bias)
-        out = [decoder.score(sequence, lab) for sequence, lab in zip(test_sequences, labels)]
-        result.append([FrameScores(float(t), inc) for t, inc in out] if per_frame else [float(t) for t, _ in out])
-      return result
     if self.device.type == 'cuda':
       model = self._native_model()
       with model.lock:
-        out = model.score(test_sequences, labels, per_frame=per_frame)
-      if not per_frame:
-        return [float(v) for v in out]
-      return [FrameScores(float(v), inc) for v, inc in zip(*out)]
-    decoder = beam_cpu.CpuBeamSearch(self)
-    out = [decoder.score(sequence, lab) for sequence, lab in zip(test_sequences, labels)]
-    return [FrameScores(float(t), inc) for t, inc in out] if per_frame else [float(t) for t, _ in out]
+        out = model.score_sweep(test_sequences, labels, pairs, per_frame=per_frame)
+      totals, increments = out if per_frame else (out, None)
+      result = [[FrameScores(float(v), inc[c]) for v, inc in zip(row, increments)] if per_frame else
+                [float(v) for v in row] for c, row in enumerate(totals)]
+    else:
+      result = []
+      for alpha, bias in pairs or [(self.crp_alpha, self.transition_bias)]:
+        decoder = beam_cpu.CpuBeamSearch(self, crp_alpha=alpha, transition_bias=bias)
+        out = [decoder.score(sequence, lab) for sequence, lab in zip(test_sequences, labels)]
+        result.append([FrameScores(float(t), inc) for t, inc in out] if per_frame else [float(t) for t, _ in out])
+    return result if pairs is not None else result[0]
 
 
 def canonical_labels(ids):
@@ -657,15 +568,18 @@ def _speaker_bounds(n, max_speakers, min_speakers):
   return native.speaker_bounds(n, max_speakers, min_speakers)
 
 
-def _warn_min_speakers(indices, lengths, speakers, min_speakers):
-  """One warning naming the utterances (by `indices`) whose final beam held no hypothesis with min_speakers
-  clusters."""
+def _warn_min_speakers(lengths, speakers, min_speakers, swept, stacklevel, indices=None):
+  """One warning naming the utterances (by `indices`, default their positions), or the (utterance, pair)s of a sweep,
+  whose final beam held no hypothesis with min_speakers clusters.  speakers[c][u]: hypothesis 0's cluster count."""
   if min_speakers is None:
     return
-  short = [int(i) for i, n, k, lo in zip(indices, lengths, speakers, min_speakers) if n > 0 and k < lo]
+  indices = range(len(lengths)) if indices is None else indices
+  short = [(int(i), c) if swept else int(i) for c, row in enumerate(speakers)
+           for i, n, k, lo in zip(indices, lengths, row, min_speakers) if n > 0 and k < lo]
   if short:
-    warnings.warn('min_speakers: the final beam of utterance(s) {} held no hypothesis with that many speakers; '
-                  'the best hypothesis was returned instead'.format(short), RuntimeWarning, stacklevel=3)
+    warnings.warn('min_speakers: the final beam of {} {} held no hypothesis with that many speakers; the best '
+                  'hypothesis was returned instead'.format('(utterance, pair)' if swept else 'utterance(s)', short),
+                  RuntimeWarning, stacklevel=stacklevel)
 
 
 def _decode_params(decode_params):
@@ -680,81 +594,46 @@ def _check_n_best(n_best, args):
   return native.check_n_best(n_best, args.beam_size)
 
 
-def _nbest_result(labels, scores, speakers, count):
-  """NBest list of a native N-best call (entries truncated to each utterance's count)."""
-  return [NBest([row.tolist() for row in lab[:c]], [float(v) for v in sc[:c]], [int(v) for v in sp[:c]])
-          for lab, sc, sp, c in zip(labels, scores, speakers, count)]
-
-
-def _native_predict(model, sequences, args, as_arrays, bounds, n_best=None):
-  """NativeModel.predict with the kcap retry: a hypothesis that opened more clusters than the device tables hold
-  fails with UIS_ERR_OVERFLOW, and the call is repeated with larger tables.  With n_best: (NBest list, cluster
-  counts of hypothesis 0)."""
+def _native_decode(model, sequences, args, bounds, n_best, pairs, as_arrays=False):
+  """UISRNN._decode on a NativeModel: one NativeModel.predict_sweep call, repeated with larger device tables (kcap)
+  while a hypothesis opens more clusters than they hold (UIS_ERR_OVERFLOW)."""
   from . import native
   mx, mn = bounds
-  bounded = mx is not None or mn is not None
   kcap = _DEFAULT_KCAP
   while True:
     try:
       with model.lock:  # a uis_model handle (one workspace) is not re-entrant
-        out = model.predict(sequences, beam_size=args.beam_size, look_ahead=args.look_ahead,
-                            test_iteration=args.test_iteration, kcap=kcap, max_speakers=mx, min_speakers=mn,
-                            return_speakers=bounded, n_best=n_best)
-      if n_best is not None:
-        return _nbest_result(*out), out[2][:, 0].copy()
-      labels, speakers = out if bounded else (out, None)
-      labels = labels if as_arrays else [lab.tolist() for lab in labels]
-      return (labels, speakers) if bounded else labels
-    except native.NativeError as err:
-      if err.code != native.UIS_ERR_OVERFLOW or kcap >= 1024:
-        raise
-      kcap = 32 if kcap == 0 else kcap * 2  # a hypothesis opened more clusters than the device tables hold: grow and retry
-
-
-def _native_predict_sweep(model, sequences, args, bounds, n_best, pairs):
-  """NativeModel.predict_sweep with the kcap retry over the whole sweep.  Returns (per-pair results, per-pair
-  cluster counts of hypothesis 0): a result is the label lists of the utterances, or their NBest list with n_best."""
-  from . import native
-  mx, mn = bounds
-  kcap = _DEFAULT_KCAP
-  while True:
-    try:
-      with model.lock:
         labels, scores, speakers, count = model.predict_sweep(
             sequences, pairs, beam_size=args.beam_size, look_ahead=args.look_ahead,
-            test_iteration=args.test_iteration, kcap=kcap, max_speakers=mx, min_speakers=mn, n_best=n_best or 1)
+            test_iteration=args.test_iteration, kcap=kcap, max_speakers=mx, min_speakers=mn, n_best=n_best)
       break
     except native.NativeError as err:
       if err.code != native.UIS_ERR_OVERFLOW or kcap >= 1024:
         raise
       kcap = 32 if kcap == 0 else kcap * 2
-  results = []
-  for c in range(len(pairs)):
-    if n_best is None:
-      results.append([lab[c, 0].tolist() for lab in labels])
-    else:
-      results.append(_nbest_result([lab[c] for lab in labels], scores[c], speakers[c], count[c]))
-  return results, speakers[:, :, 0]
+  if n_best is None:  # hypothesis 0's labels: label plane 0, which an empty utterance leaves empty
+    hyps = [[lab[c, 0] if as_arrays else lab[c, 0].tolist() for lab in labels] for c in range(len(count))]
+  else:
+    hyps = [[NBest(lab[c, :n].tolist(), s[:n], k[:n]) for lab, s, k, n in zip(labels, sc, sp, cn)]
+            for c, (sc, sp, cn) in enumerate(zip(scores.tolist(), speakers.tolist(), count.tolist()))]
+  return hyps, speakers[:, :, 0]
 
 
-def _predict_shard(model, args, device_index, sequences, out, position, bounds, n_best=None):
-  out[position] = model._predict_cuda(sequences, args, device_index, bounds=bounds, n_best=n_best)  # pylint: disable=protected-access
+def _decode_task(model, args, n_best, sequence, max_speakers, min_speakers):
+  """One pool task of the CPU parallel_predict (module level: the pool pickles it): (hypotheses, speakers) of one
+  sequence, as UISRNN._decode gives them."""
+  bounds = tuple(None if b is None else np.array([b], np.int32) for b in (max_speakers, min_speakers))
+  hyps, speakers = model._decode([sequence], args, bounds, n_best, None)  # pylint: disable=protected-access
+  return hyps[0][0], speakers[0][0]
+
+
+def _decode_shard(native_model, sequences, args, bounds, n_best, out, position):
+  """One device's shard of the CUDA parallel_predict, run on its own host thread (the C ABI releases the GIL)."""
+  out[position] = _native_decode(native_model(), sequences, args, bounds, n_best, None)
 
 
 def _take(bound, indices):
   return bound[indices] if bound is not None else None
-
-
-def _decode_cpu_bounded(model, args, sequence, max_speakers, min_speakers):
-  """One pool task of the CPU parallel_predict with speaker bounds (module level: the pool pickles it)."""
-  return model._decode_cpu(sequence, args, max_speakers, min_speakers)  # pylint: disable=protected-access
-
-
-def _decode_cpu_nbest(model, args, n_best, sequence, max_speakers, min_speakers):
-  """NBest of one sequence on the CPU device (module level: the CPU parallel_predict's pool pickles it)."""
-  decoder = beam_cpu.CpuBeamSearch(model)
-  return NBest(*decoder.decode(sequence, args.beam_size, args.look_ahead, args.test_iteration, int(max_speakers),
-                               int(min_speakers), n_best=n_best))
 
 
 def parallel_predict(model, test_sequences, args, num_processes=4, *, max_speakers=None, min_speakers=None,
@@ -771,81 +650,45 @@ def parallel_predict(model, test_sequences, args, num_processes=4, *, max_speake
     raise TypeError('test_sequences must be a list.')
   if n_best is not None:
     n_best = _check_n_best(n_best, args)
-  bounded = max_speakers is not None or min_speakers is not None or n_best is not None
-  bounds = _speaker_bounds(len(test_sequences), max_speakers, min_speakers) if bounded else (None, None)
-  if model.device.type == 'cuda':
-    for sequence in test_sequences:
-      _check_test_sequence(sequence, model.observation_dim)
-    n_dev = max(1, min(int(num_processes), torch.cuda.device_count()))
-    if n_dev == 1 or len(test_sequences) < 2:
-      if bounded:
-        return model.predict(test_sequences, args, max_speakers=bounds[0], min_speakers=bounds[1], n_best=n_best)
-      return model._predict_cuda(test_sequences, args)  # pylint: disable=protected-access
+  bounds = _speaker_bounds(len(test_sequences), max_speakers, min_speakers)
+  for sequence in test_sequences:
+    _check_test_sequence(sequence, model.observation_dim)
+  n = len(test_sequences)
+  n_dev = max(1, min(int(num_processes), torch.cuda.device_count())) if model.device.type == 'cuda' else 0
+  if n_dev == 1 or (n_dev and n < 2):
+    hyps, speakers = model._decode(test_sequences, args, bounds, n_best, None)  # pylint: disable=protected-access
+    hyps, speakers = hyps[0], speakers[0]
+  elif n_dev:
+    from . import native
     shards = shard_by_frames([len(s) for s in test_sequences], n_dev)
-    twins = [model] + [_clone_for_device(model, d) for d in range(1, n_dev)]
+    weights = model.export_weights()
+    makers = [functools.partial(model._native_model, 0)] + [  # pylint: disable=protected-access
+        functools.partial(native.NativeModel, weights, device=d) for d in range(1, n_dev)]
     results, threads = [None] * n_dev, []
     for d, shard in enumerate(shards):
-      thread = threading.Thread(target=_predict_shard, args=(
-          twins[d], args, d, [test_sequences[i] for i in shard], results, d,
-          (_take(bounds[0], shard), _take(bounds[1], shard)), n_best))
+      thread = threading.Thread(target=_decode_shard, args=(
+          makers[d], [test_sequences[i] for i in shard], args, (_take(bounds[0], shard), _take(bounds[1], shard)),
+          n_best, results, d))
       thread.start()
       threads.append(thread)
     for thread in threads:
       thread.join()
-    merged = [None] * len(test_sequences)
-    speakers = np.zeros(len(test_sequences), np.int32)
+    hyps, speakers = [None] * n, np.zeros(n, np.int32)
     for shard, result in zip(shards, results):
       if result is None:
         raise RuntimeError('parallel_predict: a device shard failed')
-      labels = result[0] if bounded else result
-      for j, (i, lab) in enumerate(zip(shard, labels)):
-        merged[i] = lab
-        if bounded:
-          speakers[i] = result[1][j]
-    if bounded:
-      _warn_min_speakers(range(len(test_sequences)), [len(s) for s in test_sequences], speakers, bounds[1])
-    return merged
-  ctx = multiprocessing.get_context('forkserver')
-  model.rnn_model.share_memory()
-  with ctx.Pool(num_processes) as pool:
-    if not bounded:
-      return pool.map(functools.partial(model.predict_single, args=args), test_sequences)
-    for sequence in test_sequences:
-      _check_test_sequence(sequence, model.observation_dim)
-    n = len(test_sequences)
-    task = functools.partial(_decode_cpu_bounded, model, args) if n_best is None else \
-        functools.partial(_decode_cpu_nbest, model, args, n_best)
-    out = pool.starmap(task, zip(
-        test_sequences, bounds[0] if bounds[0] is not None else [0] * n,
-        bounds[1] if bounds[1] is not None else [0] * n))
-  if n_best is not None:
-    _warn_min_speakers(range(n), [len(s) for s in test_sequences], [o.speakers[0] if o.speakers else 0 for o in out],
-                       bounds[1])
-    return out
-  _warn_min_speakers(range(n), [len(s) for s in test_sequences], [o[1] for o in out], bounds[1])
-  return [o[0] for o in out]
-
-
-class _DeviceTwin:
-  """Just enough of a UISRNN to own a NativeModel on another device."""
-
-  def __init__(self, weights):
-    self._weights = weights
-    self._models = {}
-    self._lock = threading.Lock()
-
-  def _predict_cuda(self, sequences, args, device_index, bounds=(None, None), n_best=None):
-    from . import native
-    with self._lock:
-      if device_index not in self._models:
-        self._models[device_index] = native.NativeModel(self._weights, device=device_index)
-      model = self._models[device_index]
-    return _native_predict(model, sequences, args, False, bounds, n_best)
-
-
-def _clone_for_device(model, device_index):
-  del device_index
-  return _DeviceTwin(model.export_weights())
+      for j, i in enumerate(shard):
+        hyps[i], speakers[i] = result[0][0][j], result[1][0][j]
+  else:
+    ctx = multiprocessing.get_context('forkserver')
+    model.rnn_model.share_memory()
+    with ctx.Pool(num_processes) as pool:
+      out = pool.starmap(functools.partial(_decode_task, model, args, n_best), zip(
+          test_sequences, bounds[0] if bounds[0] is not None else [None] * n,
+          bounds[1] if bounds[1] is not None else [None] * n))
+    hyps, speakers = [o[0] for o in out], [o[1] for o in out]
+  _warn_min_speakers([len(s) for s in test_sequences], [speakers], bounds[1], False, stacklevel=3)
+  return hyps
 
 
 def shard_columns(width, rank, world):
