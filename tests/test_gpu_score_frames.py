@@ -237,11 +237,11 @@ def test_chains_of_two_frames_take_one_pass_and_retire(native):
   both_entry_points(m, w, xs, labels, 'chain plan')
   st = m.stats()
   queued = sum(len(x) // 2 for x in xs)
-  assert st['gru_columns'] == queued and st['ctas'] == (queued + 19) // 20  # 20 columns per CTA (score_cp)
+  assert st['gru_columns'] == queued and st['ctas'] == (queued + 19) // 20  # 20 columns per CTA (beam_cp)
 
 
 def test_more_chains_than_resident_columns_refill(native):
-  """More queued chains than SMs x columns per CTA (20 at hidden <= 512: score_cp in uis_launch.cuh): every CTA
+  """More queued chains than SMs x columns per CTA (20 at hidden <= 512: beam_cp in uis_beam.cuh): every CTA
   refills columns from the queue while others still run."""
   import torch
   w, m = small(native)

@@ -85,10 +85,25 @@ struct DevBuf {
   template <class T> T* as() const { return static_cast<T*>(p); }
 };
 
+int fetch(std::vector<float>& dst, const float* src, size_t n) {
+  dst.resize(n);
+  CU(cudaMemcpy(dst.data(), src, n * sizeof(float), cudaMemcpyDefault));
+  return 0;
+}
 
-}  // namespace
+int upload(DevBuf& b, const void* src, size_t bytes) {
+  if (int rc = b.ensure(bytes)) return rc;
+  CU(cudaMemcpy(b.p, src, bytes, cudaMemcpyHostToDevice));
+  return 0;
+}
 
-namespace {
+std::vector<float> transpose(const std::vector<float>& w, int rows, int cols) {
+  std::vector<float> t((size_t)rows * cols);
+  for (int r = 0; r < rows; ++r)
+    for (int c = 0; c < cols; ++c) t[(size_t)c * rows + r] = w[(size_t)r * cols + c];
+  return t;
+}
+
 // Host threads that copy the pieces of one staging chunk from the caller's PAGEABLE arrays into pinned memory, side by
 // side (a cudaMemcpy from pageable memory is staged by the driver in one thread at ~11 GB/s; several threads reach
 // the PCIe rate).  run() hands the same piece list to every worker; worker i copies bytes [total * i / n, total * (i + 1) / n).
@@ -202,89 +217,85 @@ struct uis_model {
 
 namespace {
 
-unsigned smem_bytes(int H, int D, int B, int Kcap, int G) {
-  if (H == 512 && D == 256) return uis::make_layout<512, 256>(B, Kcap, G).total;
-  if (H == 256 && D == 128) return uis::make_layout<256, 128>(B, Kcap, G).total;
-  if (H == 128 && D == 64) return uis::make_layout<128, 64>(B, Kcap, G).total;
-  if (H == 1024 && D == 512) return uis::make_layout<1024, 512, uis::beam_cp<1024>()>(B, Kcap, G).total;
-  return 0xffffffffu;
-}
+// ---- the kernel variants (uis::Kernel, uis_launch.cuh): shared memory and launch ----------------------------------
 
-unsigned tree_smem_bytes(int H, int D, int B, int Kcap, int L, int NI, int NLF, int P) {
-  if (H == 512 && D == 256) return uis::make_tree_layout<512, 256>(B, Kcap, L, NI, NLF, P).total;
-  if (H == 256 && D == 128) return uis::make_tree_layout<256, 128>(B, Kcap, L, NI, NLF, P).total;
-  if (H == 128 && D == 64) return uis::make_tree_layout<128, 64>(B, Kcap, L, NI, NLF, P).total;
-  if (H == 1024 && D == 512) return uis::make_tree_layout<1024, 512>(B, Kcap, L, NI, NLF, P).total;
-  return 0xffffffffu;
-}
-
-// spill: the kernel whose tree-sized arrays live in p.tree_arena; its shared memory holds the rest and a small scratch
-int dispatch_tree(int H, int D, const uis::BeamParams& p, int ctas, bool spill, cudaStream_t st) {
-  const unsigned smem = spill ? tree_smem_bytes(H, D, p.B, p.Kcap, p.L, 0, 0, 0) + uis::kTreeSpillScratch
-                              : tree_smem_bytes(H, D, p.B, p.Kcap, p.L, p.node_cap, p.leaf_cap, p.P);
-  if (smem > 227u * 1024u)
-    return fail(UIS_ERR_UNSUPPORTED, "look_ahead=%d beam_size=%d kcap=%d needs %u B of shared memory (> 227 KB)", p.L,
-                p.B, p.Kcap, smem);
-  cudaError_t e = cudaSuccess;
-  const bool have = spill ? uis::launch_tree_spill_large(H, D, p, ctas, smem, st, &e) ||
-                                uis::launch_tree_spill_small(H, D, p, ctas, smem, st, &e)
-                          : uis::launch_tree_large(H, D, p, ctas, smem, st, &e) ||
-                                uis::launch_tree_small(H, D, p, ctas, smem, st, &e);
-  if (!have) return fail(UIS_ERR_UNSUPPORTED, "no sm_90a kernel instantiated for hidden=%d dim=%d", H, D);
-  if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "look-ahead kernel launch failed: %s", cudaGetErrorString(e));
-  return 0;
-}
-
-bool shape_supported(int H, int D) {
-  return (H == 512 && D == 256) || (H == 256 && D == 128) || (H == 128 && D == 64) || (H == 1024 && D == 512);
-}
-
-// *cluster: in = planned cluster size, out = the one that was launched.  When the cluster size was chosen
-// automatically and the cluster launch is refused (e.g. a partitioned GPU that cannot co-schedule the CTAs), the
-// one-CTA-per-utterance kernel runs on the same grid instead: its extra CTAs find the utterance queue empty.
-int dispatch_beam(int H, int D, const uis::BeamParams& p, int ctas, int* cluster, bool cluster_forced, cudaStream_t st) {
-  if (*cluster > 1) {
-    cudaError_t e = cudaSuccess;
-    const bool have = uis::launch_beam_cluster(H, D, p, ctas, *cluster, uis::beam_cluster_smem(H, D, p.B, p.Kcap), st, &e);
-    if (have && e == cudaSuccess) return 0;
-    if (cluster_forced) {
-      if (!have) return fail(UIS_ERR_UNSUPPORTED, "no cluster-mode kernel for hidden=%d dim=%d", H, D);
-      return fail(UIS_ERR_CUDA, "cluster beam kernel launch failed: %s", cudaGetErrorString(e));
-    }
-    (void)cudaGetLastError();  // clear the launch error and fall back
-    *cluster = 1;
+// Shared memory of kernel k at the model's shape for the sizes in p (B, Kcap, G; the tree kernels: L, node_cap,
+// leaf_cap, P); tcn = columns per tensor-core pass.  uis::kNoKernel if the shape has no such kernel.
+unsigned kernel_smem(const uis_model* m, uis::Kernel k, const uis::BeamParams& p, int tcn = 0) {
+  using namespace uis;
+  unsigned smem = kNoKernel;
+  switch (k) {
+    case Kernel::Beam:
+      with_shape(AllShapes{}, m->H, m->D, [&](auto s) {
+        using S = decltype(s);
+        smem = make_layout<S::H, S::D, beam_cp<S::H>()>(p.B, p.Kcap, p.G).total;
+      });
+      break;
+    case Kernel::Cluster:
+      with_shape(LatencyShapes{}, m->H, m->D, [&](auto s) {
+        using S = decltype(s);
+        smem = make_layout<S::H, S::D, kCPCluster, true>(p.B, p.Kcap, p.G).total;
+      });
+      break;
+    case Kernel::Stat:
+      with_shape(LatencyShapes{}, m->H, m->D, [&](auto s) {
+        using S = decltype(s);
+        smem = make_layout<S::H, S::D, kCPCluster, false, 0, true>(p.B, p.Kcap, p.G).total;
+      });
+      break;
+    case Kernel::TensorCore:
+      with_shape(TcShapes{}, m->H, m->D, [&](auto s) {
+        with_tc_columns(tcn, [&](auto n) {
+          using S = decltype(s);
+          smem = make_layout<S::H, S::D, kCPBeam, false, decltype(n)::value>(p.B, p.Kcap, p.G).total;
+        });
+      });
+      break;
+    case Kernel::Tree:
+      with_shape(AllShapes{}, m->H, m->D, [&](auto s) {
+        using S = decltype(s);
+        smem = make_tree_layout<S::H, S::D>(p.B, p.Kcap, p.L, p.node_cap, p.leaf_cap, p.P).total;
+      });
+      break;
+    case Kernel::TreeSpill:  // the tree-sized arrays live in p.tree_arena: shared memory holds the rest and a scratch
+      with_shape(AllShapes{}, m->H, m->D, [&](auto s) {
+        smem = make_tree_layout<decltype(s)::H, decltype(s)::D>(p.B, p.Kcap, p.L, 0, 0, 0).total + kTreeSpillScratch;
+      });
+      break;
   }
-  const unsigned smem = smem_bytes(H, D, p.B, p.Kcap, p.G);
-  if (smem > 227u * 1024u)
-    return fail(UIS_ERR_UNSUPPORTED, "beam_size=%d kcap=%d lanes=%d needs %u B of shared memory (> 227 KB); lower kcap",
-                p.B, p.Kcap, p.G, smem);
-  cudaError_t e = cudaSuccess;
-  if (!uis::launch_beam_large(H, D, p, ctas, smem, st, &e) && !uis::launch_beam_small(H, D, p, ctas, smem, st, &e))
-    return fail(UIS_ERR_UNSUPPORTED, "no sm_90a kernel instantiated for hidden=%d dim=%d", H, D);
-  if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "beam kernel launch failed: %s", cudaGetErrorString(e));
-  return 0;
+  return smem;
 }
 
-int fetch(std::vector<float>& dst, const float* src, size_t n) {
-  dst.resize(n);
-  CU(cudaMemcpy(dst.data(), src, n * sizeof(float), cudaMemcpyDefault));
-  return 0;
+// The sizes the shared memory of a look_ahead-1 kernel depends on.
+uis::BeamParams beam_sizes(int B, int Kcap, int G) {
+  uis::BeamParams p{};
+  p.B = B; p.Kcap = Kcap; p.G = G;
+  return p;
 }
 
-int upload(DevBuf& b, const void* src, size_t bytes) {
-  if (int rc = b.ensure(bytes)) return rc;
-  CU(cudaMemcpy(b.p, src, bytes, cudaMemcpyHostToDevice));
-  return 0;
+// Launches kernel k at the model's shape on `ctas` CTAs (Kernel::Cluster: `cluster` CTAs per cluster;
+// Kernel::TensorCore: `tcn` columns per pass).  false if the shape has no such kernel; *err = the launch status otherwise.
+bool launch_kernel(const uis_model* m, uis::Kernel k, const uis::BeamParams& p, int ctas, int cluster, int tcn,
+                   unsigned smem, cudaStream_t st, cudaError_t* err) {
+  const int H = m->H, D = m->D;
+  switch (k) {
+    case uis::Kernel::Beam:
+      return uis::launch_beam_large(H, D, p, ctas, smem, st, err) || uis::launch_beam_small(H, D, p, ctas, smem, st, err);
+    case uis::Kernel::Cluster: return uis::launch_beam_cluster(H, D, p, ctas, cluster, smem, st, err);
+    case uis::Kernel::Stat: return uis::launch_beam_stat(H, D, p, ctas, smem, st, err);
+    case uis::Kernel::TensorCore: return uis::launch_beam_tc(H, D, tcn, p, ctas, smem, st, err);
+    case uis::Kernel::Tree:
+    case uis::Kernel::TreeSpill: {
+      const bool spill = k == uis::Kernel::TreeSpill;
+      return uis::launch_tree_large(H, D, spill, p, ctas, smem, st, err) ||
+             uis::launch_tree_small(H, D, spill, p, ctas, smem, st, err);
+    }
+  }
+  return false;
 }
 
-std::vector<float> transpose(const std::vector<float>& w, int rows, int cols) {
-  std::vector<float> t((size_t)rows * cols);
-  for (int r = 0; r < rows; ++r)
-    for (int c = 0; c < cols; ++c) t[(size_t)c * rows + r] = w[(size_t)r * cols + c];
-  return t;
-}
+// ---- model creation ----------------------------------------------------------------------------------------------
 
-// ---- tensor-core pass: one-off weight preparation --------------------------------------------------------------
 typedef CUresult (*TensorMapEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                       const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                       CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -332,7 +343,7 @@ int tc_prepare(uis_model* m, const std::vector<float>& w_hh, const std::vector<f
                const std::vector<float>& w2, const std::vector<float>& hidden0) {
   const int H = m->H, D = m->D;
   m->tc_ready = false;
-  if (m->depth != 1 || !uis::beam_tc_supported(H, D, 48)) return 0;
+  if (m->depth != 1 || kernel_smem(m, uis::Kernel::TensorCore, uis::BeamParams{}, 48) == uis::kNoKernel) return 0;
   auto maxabs = [](const std::vector<float>& v) { double a = 0; for (float x : v) a = std::max(a, (double)std::fabs(x)); return a; };
   // |h'| <= max(1, |h|) by induction (h' is a convex combination of h and tanh(.)), starting from hidden0
   const double hmax = std::max(1.0, maxabs(hidden0));
@@ -383,722 +394,10 @@ int tc_prepare(uis_model* m, const std::vector<float>& w_hh, const std::vector<f
   return 0;
 }
 
-// The decoding parameters of a call: `count` (crp_alpha, transition_bias) pairs.  A call without a sweep decodes the
-// model's own pair.
-struct DecodeParams {
-  int count = 1;
-  const double* alpha = nullptr;
-  const double* p0 = nullptr;
-};
-
-DecodeParams model_decode(const uis_model* m) { return DecodeParams{1, &m->alpha, &m->p0}; }
-
-// Rejects a sweep the kernels cannot run: no pairs, more than INT_MAX jobs, or a value out of range.
-int check_decode(const uis_decode_params* dp, int U, DecodeParams* out) {
-  if (!dp) return fail(UIS_ERR_INVALID, "decode_params is NULL");
-  if (dp->count < 1) return fail(UIS_ERR_INVALID, "decode_params: count=%d (need >= 1)", dp->count);
-  if (!dp->crp_alpha || !dp->transition_bias) return fail(UIS_ERR_INVALID, "decode_params: null value array");
-  if ((long long)std::max(U, 1) * dp->count > std::numeric_limits<int>::max())
-    return fail(UIS_ERR_INVALID, "decode_params: %d utterances x %d pairs exceeds INT_MAX jobs", U, dp->count);
-  for (int c = 0; c < dp->count; ++c) {
-    const double a = dp->crp_alpha[c], b = dp->transition_bias[c];
-    if (!(std::isfinite(a) && a > 0.0))
-      return fail(UIS_ERR_INVALID, "decode_params pair %d: crp_alpha=%g (need finite and > 0)", c, a);
-    if (!(std::isfinite(b) && b > 0.0 && b < 1.0))
-      return fail(UIS_ERR_INVALID, "decode_params pair %d: transition_bias=%g (need finite and in (0, 1))", c, b);
-  }
-  *out = DecodeParams{dp->count, dp->crp_alpha, dp->transition_bias};
-  return 0;
-}
-
-// Log tables for decodes of up to max_tn frames under `dp`, built on the host with std::log so that a config's values
-// are those a model created with its pair uses.  Fills the table pointers of `p`.
-int ensure_log_tables(uis_model* m, int max_tn, const DecodeParams& dp, uis::BeamParams* p) {
-  const int need = max_tn + 2;
-  if (need > m->log_cap) {
-    const int cap = std::max(need, 4096);
-    std::vector<double> ln(cap);
-    ln[0] = -INFINITY;
-    for (int i = 1; i < cap; ++i) ln[i] = std::log((double)i);  // np.log(block_counts[c])
-    if (int rc = upload(m->logn, ln.data(), cap * sizeof(double))) return rc;
-    m->log_cap = cap;
-  }
-  // the model's own pair (by value: the Python binding passes it as a one-pair sweep) keeps its own tables, so that
-  // alternating plain calls with a sweep does not rebuild a table on every call
-  const bool own = dp.count == 1 && std::memcmp(dp.alpha, &m->alpha, sizeof(double)) == 0 &&
-                   std::memcmp(dp.p0, &m->p0, sizeof(double)) == 0;
-  uis_model::LogTables& t = own ? m->own_logs : m->sweep_logs;
-  std::vector<double> key;
-  for (int c = 0; c < dp.count; ++c) { key.push_back(dp.alpha[c]); key.push_back(dp.p0[c]); }
-  if (need > t.cap || key != t.key) {
-    const int cap = std::max({need, 4096, t.cap});
-    if (t.cap) CU(cudaDeviceSynchronize());  // the tables are rewritten in place: no earlier call may still read them
-    std::vector<double> lt((size_t)dp.count * cap), cv((size_t)dp.count * 3);
-    for (int c = 0; c < dp.count; ++c) {
-      for (int i = 0; i < cap; ++i) lt[(size_t)c * cap + i] = std::log((double)i + dp.alpha[c]);  // np.log(sum(block_counts) + alpha)
-      cv[3 * c] = std::log(dp.p0[c]);            // np.log(self.transition_bias)      uisrnn.py:418
-      cv[3 * c + 1] = std::log(1.0 - dp.p0[c]);  // np.log(1 - self.transition_bias)  uisrnn.py:416
-      cv[3 * c + 2] = std::log(dp.alpha[c]);     // np.log(self.crp_alpha)            uisrnn.py:445
-    }
-    t.cap = 0;
-    t.key.clear();
-    if (int rc = upload(t.tot, lt.data(), lt.size() * sizeof(double))) return rc;
-    if (int rc = upload(t.cfg, cv.data(), cv.size() * sizeof(double))) return rc;
-    t.cap = cap;
-    t.key = key;
-  }
-  p->logn = m->logn.as<double>();
-  p->logtot = t.tot.as<double>();
-  p->cfg_log = t.cfg.as<double>();
-  p->logtot_stride = t.cap;
-  return 0;
-}
-
-struct Plan {
-  int B, L, T, Kcap, ctas, P, maxN, G;
-  int cluster = 1;  // CTAs per utterance (thread-block cluster size); 1 = one CTA per lane group
-  int stat = 0;     // > 0: stationary-weights mode with this many groups of 32 CTAs (uis_beam_stat.cuh)
-  bool stat_forced = false;
-  int tcn = 0;      // > 0: tensor-core beam kernel with this many columns per pass (uis_beam_tc.cuh)
-  bool cluster_forced = false;
-  int node_cap = 0, leaf_cap = 0, maxTN = 0, maxSteps = 0;  // look_ahead >= 2 only
-  // look_ahead >= 2: the spill kernel that decodes, from a device-memory arena, what outgrew shared memory
-  int spill = 0;  // 0 off, 1 after the shared-memory kernel, 2 instead of it (UISRNN_B200_TREE_SPILL=force)
-  int spill_ctas = 0, spill_ni = 0, spill_nlf = 0, spill_P = 0;
-  size_t spill_arena = 0, spill_budget = 0;  // arena bytes per spill CTA; the budget they were sized from
-  long long rows;
-};
-
-// Pool slots held by a plan's CTAs: the shared-memory kernel's and the spill kernel's run one after the other on the
-// same stream and share the pools.
-size_t pool_slots(const Plan& pl) {
-  return std::max((size_t)pl.ctas * pl.G * pl.P, (size_t)pl.spill_ctas * pl.spill_P);
-}
-
-// Sizes the spill kernel of a look-ahead plan.  The worst-case tree of one beam step at (B, Kcap, L) has
-// B * sum_{i=1}^{L-1} prod_{j<i} (Kcap + 1 + j) interior nodes plus the B winners, and B * prod_{j<L} (Kcap + 1 + j)
-// leaves.  Each spill CTA needs an arena for that tree and slot pools for its P; both are clipped (in proportion) to
-// the byte budget: UISRNN_B200_TREE_SPILL_MB, else the smaller of 2 GiB and a quarter of the free device memory.
-void plan_tree_spill(uis_model* m, Plan* pl) {
-  pl->spill = 1;
-  if (const char* env = std::getenv("UISRNN_B200_TREE_SPILL")) {
-    if (std::strcmp(env, "force") == 0) pl->spill = 2;
-    else if (env[0] == '0') pl->spill = 0;
-  }
-  if (!pl->spill) return;
-  size_t budget;
-  if (const char* env = std::getenv("UISRNN_B200_TREE_SPILL_MB")) {
-    budget = (size_t)std::max(0ll, std::atoll(env)) << 20;
-  } else {
-    size_t free_b = 0, total_b = 0;
-    uis::DeviceGuard g(m->device);
-    if (g.status != cudaSuccess || cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { (void)cudaGetLastError(); free_b = 0; }
-    budget = std::min<size_t>((size_t)2 << 30, (free_b + m->tree_arena.cap) / 4);  // the arena held is re-used
-  }
-  const int B = pl->B, K = pl->Kcap, L = pl->L;
-  const double slot_bytes = 4.0 * (m->D + m->depth * m->H + 1);
-  double ni = B, prod = 1;
-  for (int i = 1; i < L; ++i) { prod *= K + i; ni += B * prod; }
-  double nlf = B * prod * (K + L);
-  auto cost = [&](double n, double l) {
-    const int P = B * K + (int)n + B + 1;
-    return (double)uis::make_tree_arena((int)n, (int)l, P).total + P * slot_bytes;
-  };
-  // leaf positions are stored in 32 bits, parent node indices in 24 (l_pc = parent << 8 | cluster)
-  const double kMaxNi = (1 << 24) - 1, kMaxLeaves = 1 << 30;
-  if (ni > kMaxNi) { nlf *= kMaxNi / ni; ni = kMaxNi; }
-  if (nlf > kMaxLeaves) { ni *= kMaxLeaves / nlf; nlf = kMaxLeaves; }
-  for (double f = std::min(1.0, (double)budget / cost(ni, nlf)); cost(ni, nlf) > (double)budget && ni > 64; f = 0.9) {
-    ni = std::floor(ni * f);
-    nlf = std::floor(nlf * f);
-  }
-  pl->spill_ni = std::max(64, (int)ni);  // floor: one CTA with about the smallest on-chip tree
-  pl->spill_nlf = std::max(8 * 64, (int)nlf);
-  pl->spill_P = B * K + pl->spill_ni + B + 1;
-  const double per_cta = cost(pl->spill_ni, pl->spill_nlf);
-  pl->spill_ctas = (int)std::max(1.0, std::min((double)pl->ctas, std::floor((double)budget / per_cta)));
-  pl->spill_arena = uis::make_tree_arena(pl->spill_ni, pl->spill_nlf, pl->spill_P).total;
-  pl->spill_budget = budget;
-}
-
-// U utterances (rows, frame counts) decoded as U * configs jobs (engine, lanes, CTAs and latency modes).
-int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o, Plan* pl, int configs = 1) {
-  if (!m || !o || (U > 0 && !off)) return fail(UIS_ERR_INVALID, "null argument");
-  if (U < 0) return fail(UIS_ERR_INVALID, "U < 0");
-  if (o->beam_size < 1 || o->look_ahead < 1 || o->test_iteration < 1)
-    return fail(UIS_ERR_INVALID, "beam_size, look_ahead and test_iteration must be >= 1");
-  if (o->look_ahead > 8) return fail(UIS_ERR_UNSUPPORTED, "look_ahead=%d > 8 not supported", o->look_ahead);
-  if (o->beam_size > uis::kMaxBeam) return fail(UIS_ERR_UNSUPPORTED, "beam_size=%d > %d not supported", o->beam_size, uis::kMaxBeam);
-  if (o->beam_size > 32 && o->look_ahead > 1)
-    return fail(UIS_ERR_UNSUPPORTED, "beam_size=%d > 32 is supported with look_ahead 1 only (look_ahead=%d)", o->beam_size, o->look_ahead);
-  if (o->engine < 0 || o->engine > 2) return fail(UIS_ERR_INVALID, "engine must be 0 (auto), 1 (FFMA) or 2 (tensor cores)");
-  pl->B = o->beam_size;
-  pl->L = o->look_ahead;
-  pl->T = o->test_iteration;
-  const bool tree = pl->L > 1;
-  pl->Kcap = o->kcap > 0 ? o->kcap : (tree ? 16 : 32);
-  if (o->kcap <= 0 && pl->B > 32)  // wide beams: the per-hypothesis tables (B * kcap entries) must fit shared memory
-    while (pl->Kcap > 4 && smem_bytes(m->H, m->D, pl->B, pl->Kcap, 1) > 227u * 1024u) pl->Kcap /= 2;
-  pl->tcn = 0;
-  if (pl->Kcap > (pl->B > 32 ? 511 : 2047) || pl->B * pl->Kcap + pl->B + 1 > 65535) return fail(UIS_ERR_INVALID, "kcap too large");
-  if (tree && pl->Kcap > 255) return fail(UIS_ERR_UNSUPPORTED, "look_ahead >= 2 supports kcap <= 255");
-  pl->P = pl->B * pl->Kcap + pl->B + 1;
-  pl->rows = U > 0 ? off[U] : 0;
-  int maxN = 0;
-  for (int u = 0; u < U; ++u) {
-    const long long n = off[u + 1] - off[u];
-    if (n < 0) return fail(UIS_ERR_INVALID, "frame_offsets not monotone");
-    if (n * pl->T > (1ll << 30)) return fail(UIS_ERR_INVALID, "utterance too long");
-    maxN = std::max<long long>(maxN, n);
-  }
-  pl->maxN = std::max(maxN, 1);
-  const long long J = (long long)U * configs;  // jobs
-  int ctas = o->n_ctas > 0 ? o->n_ctas : m->num_sms;
-  // lanes (utterances advanced together by one CTA, sharing each weight pass): 2 when there is
-  // enough work to keep every CTA's lanes busy, else 1 (latency mode); opts->lanes overrides.
-  int G = o->lanes > 0 ? std::min(o->lanes, 4) : (J >= 2ll * ctas ? 2 : 1);
-  if (tree) {
-    // look-ahead tree kernel: one utterance per CTA; size the on-chip node / leaf arrays to what
-    // shared memory allows (internal nodes : leaves ~ 1 : 8, the typical fan-out K+2)
-    G = 1;
-    long long tn = 0;
-    for (int u = 0; u < U; ++u) tn = std::max<long long>(tn, (off[u + 1] - off[u]) * pl->T);
-    pl->maxTN = (int)std::max<long long>(tn, 1);
-    pl->maxSteps = (pl->maxTN + pl->L - 1) / pl->L;
-    int ni = 64;
-    auto fits = [&](int n) {
-      const int P = pl->B * pl->Kcap + n + pl->B + 1;
-      return tree_smem_bytes(m->H, m->D, pl->B, pl->Kcap, pl->L, n, 8 * n, P) <= 227u * 1024u;
-    };
-    if (!fits(ni)) return fail(UIS_ERR_UNSUPPORTED, "look_ahead=%d beam_size=%d kcap=%d does not fit in shared memory", pl->L, pl->B, pl->Kcap);
-    while (ni < 4096 && fits(ni + 32)) ni += 32;
-    pl->node_cap = ni;
-    pl->leaf_cap = 8 * ni;
-    pl->P = pl->B * pl->Kcap + ni + pl->B + 1;
-  } else {
-    // Tensor-core engine (look_ahead 1, depth 1, 128-row-tileable shapes): the cost of a weight pass does not depend on
-    // the number of columns, so a CTA advances up to N / 8 utterances together (a lane needs ~6 columns per step,
-    // at most beam_size + 1).  Chosen automatically when some CTA gets more than one utterance; below that the
-    // one-lane FFMA kernel or the cluster (latency) mode is faster.  Its device tables default to 16 clusters per
-    // hypothesis (UIS_ERR_OVERFLOW asks the caller for more, as always).
-    if (o->engine != 1 && m->tc_ready && o->cluster <= 0) {
-      int N = 48;
-      if (const char* env = std::getenv("UISRNN_B200_TC_N")) N = std::atoi(env);
-      if (uis::beam_tc_supported(m->H, m->D, N)) {
-        const int kc = o->kcap > 0 ? o->kcap : 16;
-        int Gt = o->lanes > 0 ? std::min(o->lanes, (int)uis::kMaxLanes)
-                              : (int)std::min<long long>(N / 8, (J + ctas - 1) / std::max(ctas, 1));
-        Gt = std::max(Gt, 1);
-        while (Gt > 1 && (uis::beam_tc_smem(m->H, m->D, N, pl->B, kc, Gt) > 227u * 1024u || Gt * pl->B > 256)) --Gt;
-        const bool fits = uis::beam_tc_smem(m->H, m->D, N, pl->B, kc, Gt) <= 227u * 1024u &&
-                          pl->B * kc + pl->B + 1 <= 65535;
-        if (fits && (o->engine == 2 || J > ctas)) {
-          pl->tcn = N;
-          pl->Kcap = kc;
-          pl->P = pl->B * kc + pl->B + 1;
-          G = Gt;
-        } else if (o->engine == 2) {
-          return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: beam_size=%d kcap=%d does not fit in shared memory", pl->B, kc);
-        }
-      } else if (o->engine == 2) {
-        return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: no kernel for hidden=%d dim=%d columns=%d", m->H, m->D, N);
-      }
-    } else if (o->engine == 2) {
-      return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine needs look_ahead 1, depth 1, hidden/dim multiples of 128, no "
-                                       "cluster mode and weights its fp16 split holds (uis_model_create)");
-    }
-    if (!pl->tcn)
-      while (G > 1 && smem_bytes(m->H, m->D, pl->B, pl->Kcap, G) > 227u * 1024u) --G;
-    while (G > 1 && G * pl->B > 256) --G;  // at most 256 (lane, winner) pairs per CTA step
-  }
-  if (tree && o->engine == 2) return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: look_ahead must be 1");
-  pl->G = G;
-  pl->ctas = (int)std::max(1ll, std::min<long long>(ctas, std::max((J + G - 1) / G, 1ll)));
-  if (tree) plan_tree_spill(m, pl);
-  // Cluster (latency) mode: with fewer utterances than SMs, a thread-block cluster of 2/4/8 CTAs works on
-  // each utterance (k-split of every weight matrix, uis_beam.cuh).  opts->cluster: 0 = auto (largest of 4, 2
-  // that still gives every utterance its own cluster), -1 = off, 2/4/8 = forced; UISRNN_B200_CLUSTER=0 disables
-  // the automatic choice.
-  pl->cluster = 1;
-  pl->stat = 0;
-  // Stationary-weights mode (uis_beam_stat.cuh): 32 CTAs per utterance keep the weights in shared memory.  The fastest
-  // way to decode up to #SMs / 32 utterances at a time; opts->cluster = 32 forces it, 0 picks it automatically,
-  // UISRNN_B200_STAT=0 disables the automatic choice.
-  if (!tree && U >= 1 && (o->cluster == 0 || o->cluster == uis::kStatGroup) && m->depth == 1 &&
-      o->lanes <= 1 && o->engine != 2) {
-    const char* env = std::getenv("UISRNN_B200_STAT");
-    const bool want = o->cluster == uis::kStatGroup ||
-                      (!(env && env[0] == '0') && J * uis::kStatGroup <= ctas && o->engine == 0 && o->n_ctas <= 0);
-    const int kc = o->kcap > 0 ? o->kcap : 32;
-    const bool can = ctas >= uis::kStatGroup && uis::beam_stat_smem(m->H, m->D, pl->B, kc) <= 227u * 1024u &&
-                     pl->B * kc + pl->B + 1 <= 65535;
-    if (want && can) {
-      pl->stat = (int)std::max(1ll, std::min<long long>(ctas / uis::kStatGroup, J));
-      pl->stat_forced = o->cluster == uis::kStatGroup;
-      pl->tcn = 0;
-      pl->Kcap = kc;
-      pl->P = pl->B * kc + pl->B + 1;
-      pl->G = 1;
-      pl->ctas = pl->stat * uis::kStatGroup;
-      return 0;
-    }
-    if (o->cluster == uis::kStatGroup)
-      return fail(UIS_ERR_UNSUPPORTED, "stationary-weights mode needs hidden=512 dim=256 depth=1, >= 32 CTAs and beam_size/kcap that fit in shared memory");
-  }
-  if (!tree && !pl->tcn && U >= 1 && o->cluster >= 0 && m->depth == 1 && o->lanes <= 1) {
-    int cs = 0;
-    if (o->cluster == 2 || o->cluster == 4 || o->cluster == 8) {
-      cs = o->cluster;
-    } else if (o->cluster == 0) {
-      const char* env = std::getenv("UISRNN_B200_CLUSTER");
-      if (!(env && env[0] == '0'))
-        for (int c : {4, 2})
-          if (J * c <= ctas) { cs = c; break; }
-    } else {
-      return fail(UIS_ERR_INVALID, "cluster must be -1, 0, 2, 4, 8 or 32");
-    }
-    if (cs > 1 && uis::beam_cluster_smem(m->H, m->D, pl->B, pl->Kcap) <= 227u * 1024u) {
-      const int clusters = (int)std::max(1ll, std::min<long long>(ctas / cs, J));
-      pl->cluster = cs;
-      pl->cluster_forced = o->cluster > 0;
-      pl->G = 1;
-      pl->ctas = clusters * cs;
-    } else if (o->cluster > 0) {
-      return fail(UIS_ERR_UNSUPPORTED, "cluster mode needs hidden=512 dim=256 depth=1 and beam_size/kcap that fit in shared memory");
-    }
-  }
-  return 0;
-}
-
-size_t workspace_bytes(const uis_model* m, const Plan& pl, int U, int configs = 1) {
-  const size_t J = (size_t)U * configs;
-  size_t b = 0;
-  b += (size_t)pl.rows * 3 * m->H * 4;                                  // gi
-  b += pool_slots(pl) * (m->D + m->depth * m->H + 1) * 4;            // slot pools (+ Gaussian term per slot)
-  b += (size_t)pl.spill_ctas * pl.spill_arena;                          // look-ahead spill arenas
-  b += (size_t)pl.ctas * pl.G * (pl.L > 1 ? (size_t)pl.maxTN + pl.maxSteps : (size_t)pl.maxN) * pl.B * 4;  // back-pointers
-  b += (size_t)(U + 1) * 8 + J * 8 + 256;                               // offsets, order, status
-  if (configs > 1) b += (size_t)configs * (4096 + 3) * 8;               // log tables of the sweep (at least)
-  if (pl.tcn) b += (size_t)pl.ctas * pl.tcn * m->H * 4;                 // a = relu(W1 h' + b1) between two products
-  return b;
-}
-
-// Speaker bounds of a bounded call (host arrays, either may be NULL): 0 = no bound, max >= 1, 0 <= min <= max.
-struct SpeakerBounds {
-  const int32_t* max = nullptr;
-  const int32_t* min = nullptr;
-  int32_t* out_dev = nullptr;  // [U] device, may be NULL
-  SpeakerBounds at(int u0) const {
-    return SpeakerBounds{max ? max + u0 : nullptr, min ? min + u0 : nullptr, out_dev ? out_dev + u0 : nullptr};
-  }
-};
-
-// N-best outputs of a call (n_best = 1 with NULL pointers: a plain call).  Labels are n_best planes of the call's rows.
-struct NBestOut {
-  int k = 1;
-  float* scores = nullptr;     // [U][k]
-  int32_t* speakers = nullptr; // [U][k]
-  int32_t* count = nullptr;    // [U]
-};
-
-int check_bounds(int U, const int32_t* mx, const int32_t* mn) {
-  for (int u = 0; u < U; ++u) {
-    const int a = mx ? mx[u] : 0, b = mn ? mn[u] : 0;
-    if (a < 0 || b < 0 || (a > 0 && b > a))
-      return fail(UIS_ERR_INVALID, "utterance %d: max_speakers=%d min_speakers=%d (need max >= 1 or 0 = none, "
-                  "min >= 0, min <= max)", u, a, b);
-  }
-  return 0;
-}
-
-// n_best in [1, beam_size]; an N-best call needs its label and score buffers.
-int check_nbest(int n_best, const uis_predict_opts* opts, const uis_nbest_out* out) {
-  if (n_best < 1 || n_best > opts->beam_size)
-    return fail(UIS_ERR_INVALID, "n_best=%d (need 1 <= n_best <= beam_size=%d)", n_best, opts->beam_size);
-  if (!out->scores) return fail(UIS_ERR_INVALID, "n_best: null scores buffer");
-  return 0;
-}
-
-int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
-                        const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
-                        const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev,
-                        const NBestOut& nb, const DecodeParams* dp = nullptr);
-int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
-                      const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
-                      const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out,
-                      const NBestOut& nb, const DecodeParams* dp = nullptr);
-
-// The model's part of the kernel parameters: weights and constants (ensure_log_tables adds the log terms).
-uis::BeamParams model_params(const uis_model* m) {
-  const int H = m->H;
-  uis::BeamParams p{};
-  p.whh_t = m->whh_t.as<float>(); p.w1_t = m->w1_t.as<float>(); p.w2_t = m->w2_t.as<float>();
-  p.depth = m->depth;
-  for (int l = 1; l < m->depth; ++l) {
-    p.wih_up_t[l - 1] = m->wih_up_t.as<float>() + (size_t)(l - 1) * H * 3 * H;
-    p.whh_up_t[l - 1] = m->whh_t.as<float>() + (size_t)l * H * 3 * H;
-  }
-  p.bih_up = m->bih.as<float>() + 3 * H;   // layers >= 1
-  p.bhh_up = m->bhh.as<float>() + 3 * H;
-  p.bhh = m->bhh.as<float>(); p.b1 = m->b1.as<float>(); p.b2 = m->b2.as<float>();
-  p.wvec = m->wvec.as<float>(); p.mean0 = m->mean0.as<float>(); p.hidden0 = m->hidden0.as<float>();
-  return p;
-}
-
-// Decodes U utterances under dp.count configs: J = U * dp.count jobs, job j = utterance j % U under config j / U.
-// Per-job outputs (status, N-best scores / speakers / counts, taps) are [J]; labels_dev holds dp.count * nb.k planes
-// of the call's rows (plane c * nb.k + j: config c, hypothesis j).
-int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, const Plan& pl, int32_t* labels_dev,
-               const uis_debug_taps* taps, cudaStream_t st, const SpeakerBounds& sb, const NBestOut& nb,
-               const DecodeParams& dp, bool gi_ready = false) {
-  const int H = m->H, D = m->D;
-  const int J = U * dp.count;
-  if (sb.out_dev && U > 0) CU(cudaMemsetAsync(sb.out_dev, 0, (size_t)J * sizeof(int32_t), st));  // empty inputs: 0
-  if (U > 0 && pl.rows == 0) {  // no kernel runs: every utterance is empty and returns no hypothesis
-    if (nb.count) CU(cudaMemsetAsync(nb.count, 0, (size_t)J * sizeof(int32_t), st));
-    if (nb.speakers) CU(cudaMemsetAsync(nb.speakers, 0, (size_t)J * nb.k * sizeof(int32_t), st));
-    if (nb.scores) {
-      const std::vector<float> inf((size_t)J * nb.k, std::numeric_limits<float>::infinity());
-      CU(cudaMemcpyAsync(nb.scores, inf.data(), inf.size() * sizeof(float), cudaMemcpyHostToDevice, st));
-      CU(cudaStreamSynchronize(st));  // (inf is about to go out of scope)
-    }
-  }
-  m->stats = uis_stats{};
-  m->stats.utterances = J;
-  m->stats.frames = pl.rows;
-  m->stats.ctas = pl.ctas;
-  m->stats.lanes = pl.G;
-  m->stats.cluster = pl.cluster;
-  m->last_U = J;
-  m->last_score = false;
-  m->last_tree_spill = pl.L > 1 && pl.spill;
-  m->last_spill_ni = pl.spill_ni; m->last_spill_nlf = pl.spill_nlf; m->last_spill_budget = pl.spill_budget;
-  m->last_stream = st;
-  m->stats_pending = false;
-  if (U == 0 || pl.rows == 0) {
-    return 0;
-  }
-  uis::BeamParams p = model_params(m);
-  long long max_tn = 0;
-  for (int u = 0; u < U; ++u) max_tn = std::max<long long>(max_tn, (off[u + 1] - off[u]) * pl.T);
-  if (int rc = ensure_log_tables(m, (int)max_tn, dp, &p)) return rc;
-
-  // schedule: longest utterance first (LPT) -- steps are strictly sequential per utterance.  The configs of one
-  // utterance follow each other, so that they read the same input rows at about the same time.
-  std::vector<int> by_len(U), order((size_t)J);
-  std::iota(by_len.begin(), by_len.end(), 0);
-  std::stable_sort(by_len.begin(), by_len.end(),
-                   [&](int a, int b) { return off[a + 1] - off[a] > off[b + 1] - off[b]; });
-  for (int i = 0; i < U; ++i)
-    for (int c = 0; c < dp.count; ++c) order[(size_t)i * dp.count + c] = c * U + by_len[i];
-  std::vector<long long> off_ll(off, off + U + 1);
-
-  if (int rc = m->row_off.ensure((U + 1) * sizeof(long long))) return rc;
-  if (int rc = m->order.ensure((size_t)J * sizeof(int))) return rc;
-  if (int rc = m->status.ensure((size_t)J * sizeof(int))) return rc;
-  if (int rc = m->queue_stats.ensure(40 * sizeof(unsigned long long))) return rc;
-  if (int rc = m->gi.ensure((size_t)pl.rows * 3 * H * sizeof(float))) return rc;
-  if (int rc = m->pool_mean.ensure(pool_slots(pl) * D * sizeof(float))) return rc;
-  if (int rc = m->pool_hidden.ensure(pool_slots(pl) * m->depth * H * sizeof(float))) return rc;
-  if (int rc = m->pool_mse.ensure(pool_slots(pl) * sizeof(float))) return rc;
-  if (pl.spill)
-    if (int rc = m->tree_arena.ensure((size_t)pl.spill_ctas * pl.spill_arena)) return rc;
-  if (int rc = m->bp.ensure((size_t)pl.ctas * pl.G * (pl.L > 1 ? (size_t)pl.maxTN + pl.maxSteps : (size_t)pl.maxN) * pl.B *
-                            sizeof(unsigned)))
-    return rc;
-
-  if (pl.tcn)
-    if (int rc = m->tc_scratch.ensure((size_t)pl.ctas * pl.tcn * H * sizeof(float))) return rc;
-  if (pl.stat) {
-    if (int rc = m->stat_bar.ensure((size_t)pl.stat * uis::kStatGroup * sizeof(unsigned))) return rc;
-    if (int rc = m->stat_scratch.ensure((size_t)pl.stat * uis::kCPCluster * H * sizeof(float))) return rc;
-    CU(cudaMemsetAsync(m->stat_bar.p, 0, (size_t)pl.stat * uis::kStatGroup * sizeof(unsigned), st));
-  }
-
-  CU(cudaMemcpyAsync(m->row_off.p, off_ll.data(), (U + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(m->order.p, order.data(), (size_t)J * sizeof(int), cudaMemcpyHostToDevice, st));
-  CU(cudaMemsetAsync(m->queue_stats.p, 0, 40 * sizeof(unsigned long long), st));
-  CU(cudaMemsetAsync(m->status.p, 0xff, (size_t)J * sizeof(int), st));
-
-  p.x = x_dev; p.gi = m->gi.as<float>();
-  p.row_off = m->row_off.as<long long>(); p.order = m->order.as<int>();
-  p.U = J; p.n_utt = U; p.B = pl.B; p.Kcap = pl.Kcap; p.T = pl.T; p.P = pl.P; p.maxN = pl.maxN; p.G = pl.G;
-  p.L = pl.L; p.node_cap = pl.node_cap; p.leaf_cap = pl.leaf_cap; p.maxTN = pl.maxTN; p.maxSteps = pl.maxSteps;
-  { const char* e = getenv("UIS_DBG_MODE"); p.dbg_mode = e ? atoi(e) : 0; }
-  p.pool_mean = m->pool_mean.as<float>(); p.pool_hidden = m->pool_hidden.as<float>(); p.pool_mse = m->pool_mse.as<float>();
-  p.bp = m->bp.as<unsigned>();
-  p.queue = m->queue_stats.as<int>();
-  p.stats = m->queue_stats.as<unsigned long long>() + 8;
-  p.labels = labels_dev; p.status = m->status.as<int>();
-  if (sb.max || sb.min) {
-    std::vector<int32_t> kb(2 * (size_t)U);
-    for (int u = 0; u < U; ++u) { kb[2 * u] = sb.max ? sb.max[u] : 0; kb[2 * u + 1] = sb.min ? sb.min[u] : 0; }
-    if (int rc = m->spk_bound.ensure(kb.size() * sizeof(int32_t))) return rc;
-    CU(cudaMemcpyAsync(m->spk_bound.p, kb.data(), kb.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    p.spk_bound = m->spk_bound.as<int>();
-  }
-  p.spk_out = sb.out_dev;
-  p.n_best = nb.k; p.label_plane = pl.rows;
-  p.nbest_scores = nb.scores; p.nbest_speakers = nb.speakers; p.nbest_count = nb.count;
-  p.trace_utt = -1;
-  if (pl.stat) {
-    p.stat_bar = m->stat_bar.as<unsigned>();
-    p.stat_scratch = m->stat_scratch.as<float>();
-  }
-  if (pl.tcn) {
-    p.tc_wmap = m->tc_map;
-    p.tc_sh = m->tc_sh; p.tc_sa = m->tc_sa;
-    p.tc_inv_hh = m->tc_inv_hh; p.tc_inv_1 = m->tc_inv_1; p.tc_inv_2 = m->tc_inv_2;
-    p.tc_scratch = m->tc_scratch.as<float>();
-  }
-
-  long long trace_steps = 0;
-  if (taps) {
-    if (taps->final_scores) {
-      if (int rc = m->dbg_final_scores.ensure((size_t)J * pl.B * 4)) return rc;
-      p.dbg_final_scores = m->dbg_final_scores.as<float>();
-      if (int rc = m->dbg_final_k.ensure((size_t)J * 4)) return rc;
-      p.dbg_final_k = m->dbg_final_k.as<int>();
-    }
-    if (taps->trace_utt >= 0 && taps->trace_utt < J) {  // a job: utterance trace_utt % U under config trace_utt / U
-      p.trace_utt = taps->trace_utt;
-      p.trace_capacity = std::max(taps->trace_capacity, 0);
-      const int tu = p.trace_utt % U;
-      trace_steps = ((off[tu + 1] - off[tu]) * pl.T + pl.L - 1) / pl.L;
-      if (taps->step_winners && p.trace_capacity > 0) {
-        if (int rc = m->dbg_win.ensure((size_t)p.trace_capacity * 4 * (1 + pl.L))) return rc;
-        if (int rc = m->dbg_score.ensure((size_t)p.trace_capacity * 4)) return rc;
-        if (int rc = m->dbg_off.ensure((size_t)(trace_steps + 1) * 8)) return rc;
-        p.dbg_win = m->dbg_win.as<int>(); p.dbg_score = m->dbg_score.as<float>();
-        p.dbg_off = m->dbg_off.as<long long>();
-      }
-      if (taps->best_mean) {
-        if (int rc = m->dbg_best_mean.ensure((size_t)pl.Kcap * D * 4)) return rc;
-        if (int rc = m->dbg_best_hidden.ensure((size_t)pl.Kcap * m->depth * H * 4)) return rc;
-        if (int rc = m->dbg_best_blocks.ensure((size_t)pl.Kcap * 4)) return rc;
-        p.dbg_best_mean = m->dbg_best_mean.as<float>(); p.dbg_best_hidden = m->dbg_best_hidden.as<float>();
-        p.dbg_best_blocks = m->dbg_best_blocks.as<int>();
-      }
-    }
-  }
-
-  for (auto& e : m->ev)
-    if (!e) CU(cudaEventCreate(&e));
-  CU(cudaEventRecord(m->ev[0], st));
-  // kernel 1: input projection GEMM (the host-buffer path has already run it chunk by chunk, under the H2D copies)
-  if (!gi_ready) {
-    dim3 grid((3 * H + uis::PBN - 1) / uis::PBN, (unsigned)((pl.rows + uis::PBM - 1) / uis::PBM));
-    uis::input_proj_kernel<<<grid, 256, 0, st>>>(x_dev, m->wih_t.as<float>(), m->bih.as<float>(), m->gi.as<float>(),
-                                                (int)pl.rows, 3 * H, D);
-    CU(cudaGetLastError());
-  }
-  CU(cudaEventRecord(m->ev[1], st));
-  // kernel 2: persistent beam search
-  int cluster_used = pl.cluster;
-  bool stat_done = false;
-  if (pl.stat) {
-    cudaError_t e = cudaSuccess;
-    const bool have = uis::launch_beam_stat(H, D, p, pl.ctas, uis::beam_stat_smem(H, D, pl.B, pl.Kcap), st, &e);
-    if (have && e == cudaSuccess) {
-      cluster_used = uis::kStatGroup;
-      stat_done = true;
-    } else if (pl.stat_forced) {
-      if (!have) return fail(UIS_ERR_UNSUPPORTED, "no stationary-weights kernel for hidden=%d dim=%d", H, D);
-      return fail(UIS_ERR_CUDA, "stationary-weights beam kernel launch failed: %s", cudaGetErrorString(e));
-    } else {
-      // chosen automatically and refused (e.g. the CTAs cannot all be co-resident on a shared / partitioned GPU): the
-      // one-CTA-per-utterance kernel runs on the same grid instead; its extra CTAs find the utterance queue empty
-      (void)cudaGetLastError();
-      cluster_used = 1;
-    }
-  }
-  if (stat_done) {
-  } else if (pl.tcn) {
-    cudaError_t e = cudaSuccess;
-    if (!uis::launch_beam_tc(H, D, pl.tcn, p, pl.ctas, uis::beam_tc_smem(H, D, pl.tcn, pl.B, pl.Kcap, pl.G), st, &e))
-      return fail(UIS_ERR_UNSUPPORTED, "no tensor-core kernel for hidden=%d dim=%d columns=%d", H, D, pl.tcn);
-    if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "tensor-core beam kernel launch failed: %s", cudaGetErrorString(e));
-  } else if (pl.L > 1) {
-    if (pl.spill != 2)
-      if (int rc = dispatch_tree(H, D, p, pl.ctas, false, st)) return rc;
-    if (pl.spill) {
-      // right behind it on the same stream: the utterances it left at status -5 (every one when forced), from a
-      // second queue; its CTAs find nothing to do and exit when every tree fitted
-      uis::BeamParams ps = p;
-      ps.node_cap = pl.spill_ni; ps.leaf_cap = pl.spill_nlf; ps.P = pl.spill_P;
-      ps.queue = p.queue + 1;
-      ps.tree_arena = m->tree_arena.as<unsigned char>();
-      ps.tree_spill_all = pl.spill == 2;
-      if (int rc = dispatch_tree(H, D, ps, pl.spill_ctas, true, st)) return rc;
-    }
-  } else if (int rc = dispatch_beam(H, D, p, pl.ctas, &cluster_used, pl.cluster_forced, st)) {
-    return rc;
-  }
-  m->stats.cluster = cluster_used;
-  m->stats.engine = pl.tcn ? 2 : 1;
-  m->stats.tc_columns = pl.tcn;
-  CU(cudaEventRecord(m->ev[2], st));
-  m->stats.kernel_launches = 2 + (pl.L > 1 && pl.spill == 1 ? 1 : 0);
-  m->stats_pending = true;
-
-  if (taps) {
-    CU(cudaStreamSynchronize(st));
-    if (p.dbg_final_scores) {
-      CU(cudaMemcpy(taps->final_scores, p.dbg_final_scores, (size_t)J * pl.B * 4, cudaMemcpyDeviceToHost));
-      if (taps->final_k) CU(cudaMemcpy(taps->final_k, p.dbg_final_k, (size_t)J * 4, cudaMemcpyDeviceToHost));
-    }
-    if (p.dbg_win) {
-      CU(cudaMemcpy(taps->step_winners, p.dbg_win, (size_t)p.trace_capacity * 4 * (1 + pl.L), cudaMemcpyDeviceToHost));
-      CU(cudaMemcpy(taps->step_scores, p.dbg_score, (size_t)p.trace_capacity * 4, cudaMemcpyDeviceToHost));
-      if (taps->step_offsets)
-        CU(cudaMemcpy(taps->step_offsets, p.dbg_off, (size_t)(trace_steps + 1) * 8, cudaMemcpyDeviceToHost));
-    }
-    if (p.dbg_best_mean) {
-      CU(cudaMemcpy2D(taps->best_mean, (size_t)m->D_user * 4, p.dbg_best_mean, (size_t)D * 4, (size_t)m->D_user * 4, pl.Kcap,
-                      cudaMemcpyDeviceToHost));
-      if (taps->best_hidden)
-        CU(cudaMemcpy2D(taps->best_hidden, (size_t)m->H_user * 4, p.dbg_best_hidden, (size_t)H * 4, (size_t)m->H_user * 4,
-                        (size_t)pl.Kcap * m->depth, cudaMemcpyDeviceToHost));
-      if (taps->best_blocks)
-        CU(cudaMemcpy(taps->best_blocks, p.dbg_best_blocks, (size_t)pl.Kcap * 4, cudaMemcpyDeviceToHost));
-    }
-  }
-  return 0;
-}
-
-// Pull the device-side counters and per-utterance status of the last call (synchronises).
-int collect(uis_model* m) {
-  if (!m->stats_pending) return 0;
-  CU(cudaStreamSynchronize(m->last_stream));
-  unsigned long long s[24];
-  CU(cudaMemcpy(s, m->queue_stats.as<unsigned long long>() + 8, sizeof s, cudaMemcpyDeviceToHost));
-  if (m->last_score) {  // the chain kernel's columns and passes; max_k came from the labels
-    m->stats.gru_columns = (int64_t)s[0];
-    m->stats.weight_passes = (int64_t)s[1];
-    CU(cudaEventElapsedTime(&m->stats.prepass_ms, m->ev[0], m->ev[1]));
-    CU(cudaEventElapsedTime(&m->stats.beam_ms, m->ev[1], m->ev[2]));
-    m->stats_pending = false;
-    return 0;
-  }
-  for (int i = 0; i < 10; ++i) m->stats.phase_cycles[i] = (int64_t)s[8 + i];
-  for (int i = 0; i < 4; ++i) m->stats.tc_cycles[i] = (int64_t)s[18 + i];
-  m->stats.gru_columns = (int64_t)s[0];
-  m->stats.weight_passes = (int64_t)s[1];
-  m->stats.candidates = (int64_t)s[2];
-  m->stats.beam_steps = (int64_t)s[3];
-  m->stats.max_k = (int32_t)s[4];
-  CU(cudaEventElapsedTime(&m->stats.prepass_ms, m->ev[0], m->ev[1]));
-  CU(cudaEventElapsedTime(&m->stats.beam_ms, m->ev[1], m->ev[2]));
-  m->stats_pending = false;
-  std::vector<int> status(m->last_U);
-  CU(cudaMemcpy(status.data(), m->status.p, (size_t)m->last_U * sizeof(int), cudaMemcpyDeviceToHost));
-  int overflow = 0, bad = 0, capacity = 0;
-  for (int v : status) {
-    if (v == -4) ++overflow;
-    else if (v == -5) ++capacity;
-    else if (v != 0) ++bad;
-  }
-  if (capacity && m->last_tree_spill)
-    return fail(UIS_ERR_CAPACITY, "%d utterance(s): the look-ahead tree of one beam step exhausted the device-memory arena "
-                "(%d nodes / %d leaves per CTA from a budget of %zu MiB; raise UISRNN_B200_TREE_SPILL_MB or lower "
-                "beam_size / look_ahead / kcap)", capacity, m->last_spill_ni, m->last_spill_nlf, m->last_spill_budget >> 20);
-  if (capacity)
-    return fail(UIS_ERR_CAPACITY, "%d utterance(s): the look-ahead tree of one beam step outgrew the on-chip node arrays "
-                "(lower beam_size / look_ahead / kcap)", capacity);
-  if (overflow)
-    return fail(UIS_ERR_OVERFLOW, "%d utterance(s) opened more clusters than kcap; retry with a larger kcap", overflow);
-  if (bad) return fail(UIS_ERR_INVALID, "%d utterance(s) ended with no finite hypothesis", bad);
-  return 0;
-}
-
-}  // namespace
-
-extern "C" {
-
-int uis_version(void) { return UIS_ABI_VERSION; }
-const char* uis_last_error(void) { return g_err.c_str(); }
-
-static int model_create_impl(uis_model** out, int device, int D, int H, int depth, const float* w_ih, const float* w_hh,
-                             const float* b_ih, const float* b_hh, const float* w1, const float* b1, const float* w2,
-                             const float* b2, const float* h0, const float* sigma2, double transition_bias,
-                             double crp_alpha, int D_user, int H_user);
-
-// Any (hidden <= 1024, dim <= 512) runs in the smallest instantiated kernel shape that holds it, zero-padded: a padded
-// hidden unit has zero weights and biases (r = z = 1/2, n = 0, so it stays at its initial 0) and feeds nothing; a
-// padded observation dimension has x = mean = 0 and adds (0 - 0)^2 * w = 0 to every Gaussian term.  Adding exact
-// zeros does not change an fp32 sum, so the results are those of a kernel instantiated for the caller's shape.
-int uis_model_create(uis_model** out, int device, int D, int H, int depth, const float* w_ih, const float* w_hh,
-                     const float* b_ih, const float* b_hh, const float* w1, const float* b1, const float* w2,
-                     const float* b2, const float* h0, const float* sigma2, double transition_bias,
-                     double crp_alpha) {
-  if (!out) return fail(UIS_ERR_INVALID, "out is NULL");
-  *out = nullptr;
-  if (!w_ih || !w_hh || !b_ih || !b_hh || !w1 || !b1 || !w2 || !b2 || !h0 || !sigma2)
-    return fail(UIS_ERR_INVALID, "NULL weight pointer");
-  if (depth < 1 || depth > uis::kMaxDepth)
-    return fail(UIS_ERR_UNSUPPORTED, "rnn_depth=%d: the sm_90a kernels support 1..%d stacked GRU layers", depth, uis::kMaxDepth);
-  if (D < 1 || H < 1) return fail(UIS_ERR_INVALID, "observation_dim and rnn_hidden_size must be >= 1");
-  if (shape_supported(H, D))
-    return model_create_impl(out, device, D, H, depth, w_ih, w_hh, b_ih, b_hh, w1, b1, w2, b2, h0, sigma2,
-                             transition_bias, crp_alpha, D, H);
-  static const int shapes[4][2] = {{128, 64}, {256, 128}, {512, 256}, {1024, 512}};
-  int Hp = 0, Dp = 0;
-  for (auto& sh : shapes)
-    if (!Hp && H <= sh[0] && D <= sh[1]) { Hp = sh[0]; Dp = sh[1]; }
-  if (!Hp)
-    return fail(UIS_ERR_UNSUPPORTED, "hidden=%d dim=%d: the sm_90a kernels hold models up to hidden=1024 dim=512", H, D);
-  uis::DeviceGuard device_guard_(device);
-  CU(device_guard_.status);
-  std::vector<float> v, p_wih((size_t)3 * Hp * Dp + (size_t)(depth - 1) * 3 * Hp * Hp, 0.f), p_whh((size_t)depth * 3 * Hp * Hp, 0.f),
-      p_bih((size_t)depth * 3 * Hp, 0.f), p_bhh((size_t)depth * 3 * Hp, 0.f), p_w1((size_t)Hp * Hp, 0.f), p_b1(Hp, 0.f),
-      p_w2((size_t)Dp * Hp, 0.f), p_b2(Dp, 0.f), p_h0((size_t)depth * Hp, 0.f), p_s2(Dp, 1.f);
-  // gate blocks (r, z, n) keep their own row ranges: row g * H + j -> g * Hp + j
-  if (int r = fetch(v, w_ih, (size_t)3 * H * D + (size_t)(depth - 1) * 3 * H * H)) return r;
-  for (int g = 0; g < 3; ++g)
-    for (int j = 0; j < H; ++j)
-      std::copy(v.begin() + ((size_t)g * H + j) * D, v.begin() + ((size_t)g * H + j + 1) * D,
-                p_wih.begin() + ((size_t)g * Hp + j) * Dp);
-  for (int l = 1; l < depth; ++l)
-    for (int g = 0; g < 3; ++g)
-      for (int j = 0; j < H; ++j) {
-        const float* src = v.data() + (size_t)3 * H * D + (size_t)(l - 1) * 3 * H * H + ((size_t)g * H + j) * H;
-        std::copy(src, src + H, p_wih.begin() + (size_t)3 * Hp * Dp + (size_t)(l - 1) * 3 * Hp * Hp + ((size_t)g * Hp + j) * Hp);
-      }
-  if (int r = fetch(v, w_hh, (size_t)depth * 3 * H * H)) return r;
-  for (int l = 0; l < depth; ++l)
-    for (int g = 0; g < 3; ++g)
-      for (int j = 0; j < H; ++j) {
-        const float* src = v.data() + (size_t)l * 3 * H * H + ((size_t)g * H + j) * H;
-        std::copy(src, src + H, p_whh.begin() + (size_t)l * 3 * Hp * Hp + ((size_t)g * Hp + j) * Hp);
-      }
-  for (int which = 0; which < 2; ++which) {
-    if (int r = fetch(v, which ? b_hh : b_ih, (size_t)depth * 3 * H)) return r;
-    std::vector<float>& dst = which ? p_bhh : p_bih;
-    for (int l = 0; l < depth; ++l)
-      for (int g = 0; g < 3; ++g)
-        std::copy(v.begin() + ((size_t)l * 3 + g) * H, v.begin() + ((size_t)l * 3 + g + 1) * H,
-                  dst.begin() + ((size_t)l * 3 + g) * Hp);
-  }
-  if (int r = fetch(v, w1, (size_t)H * H)) return r;
-  for (int j = 0; j < H; ++j) std::copy(v.begin() + (size_t)j * H, v.begin() + (size_t)(j + 1) * H, p_w1.begin() + (size_t)j * Hp);
-  if (int r = fetch(v, b1, H)) return r;
-  std::copy(v.begin(), v.end(), p_b1.begin());
-  if (int r = fetch(v, w2, (size_t)D * H)) return r;
-  for (int d = 0; d < D; ++d) std::copy(v.begin() + (size_t)d * H, v.begin() + (size_t)(d + 1) * H, p_w2.begin() + (size_t)d * Hp);
-  if (int r = fetch(v, b2, D)) return r;
-  std::copy(v.begin(), v.end(), p_b2.begin());
-  if (int r = fetch(v, h0, (size_t)depth * H)) return r;
-  for (int l = 0; l < depth; ++l) std::copy(v.begin() + (size_t)l * H, v.begin() + (size_t)(l + 1) * H, p_h0.begin() + (size_t)l * Hp);
-  if (int r = fetch(v, sigma2, D)) return r;
-  std::copy(v.begin(), v.end(), p_s2.begin());
-  return model_create_impl(out, device, Dp, Hp, depth, p_wih.data(), p_whh.data(), p_bih.data(), p_bhh.data(), p_w1.data(),
-                           p_b1.data(), p_w2.data(), p_b2.data(), p_h0.data(), p_s2.data(), transition_bias, crp_alpha, D, H);
-}
-
-static int model_create_impl(uis_model** out, int device, int D, int H, int depth, const float* w_ih, const float* w_hh,
-                             const float* b_ih, const float* b_hh, const float* w1, const float* b1, const float* w2,
-                             const float* b2, const float* h0, const float* sigma2, double transition_bias,
-                             double crp_alpha, int D_user, int H_user) {
+int model_create_impl(uis_model** out, int device, int D, int H, int depth, const float* w_ih, const float* w_hh,
+                      const float* b_ih, const float* b_hh, const float* w1, const float* b1, const float* w2,
+                      const float* b2, const float* h0, const float* sigma2, double transition_bias, double crp_alpha,
+                      int D_user, int H_user) {
   if (!(transition_bias > 0.0 && transition_bias < 1.0))
     return fail(UIS_ERR_INVALID, "transition_bias must be in (0,1), got %g", transition_bias);
   if (!(crp_alpha > 0.0)) return fail(UIS_ERR_INVALID, "crp_alpha must be > 0");
@@ -1189,90 +488,639 @@ static int model_create_impl(uis_model** out, int device, int D, int H, int dept
   return 0;
 }
 
-int uis_model_destroy(uis_model* m) {
-  if (!m) return 0;
-  uis::DeviceGuard device_guard_(m->device);
-  DevBuf* bufs[] = {&m->wih_t, &m->whh_t, &m->w1_t, &m->w2_t, &m->bih, &m->bhh, &m->b1, &m->b2, &m->wvec, &m->mean0,
-                    &m->hidden0, &m->wih_up_t, &m->logn, &m->own_logs.tot, &m->own_logs.cfg, &m->sweep_logs.tot, &m->sweep_logs.cfg, &m->x64, &m->x32, &m->gi, &m->row_off, &m->order,
-                    &m->pool_mean, &m->pool_hidden, &m->bp, &m->queue_stats, &m->labels, &m->status, &m->dbg_win,
-                    &m->dbg_score, &m->dbg_off, &m->dbg_final_scores, &m->dbg_final_k, &m->dbg_best_mean,
-                    &m->dbg_best_hidden, &m->dbg_best_blocks, &m->tc_planes, &m->tc_scratch, &m->pool_mse, &m->stat_bar, &m->stat_scratch,
-                    &m->tree_arena, &m->nb_scores, &m->nb_speakers, &m->nb_count, &m->sc_chain_off,
-                    &m->sc_chain_rows, &m->sc_mse, &m->sc_blocks, &m->sc_out};
-  for (DevBuf* b : bufs) b->release();
+// ---- planning ----------------------------------------------------------------------------------------------------
+
+// The decoding parameters of a call: `count` (crp_alpha, transition_bias) pairs.  A call without a sweep decodes the
+// model's own pair.
+struct DecodeParams {
+  int count = 1;
+  const double* alpha = nullptr;
+  const double* p0 = nullptr;
+};
+
+DecodeParams model_decode(const uis_model* m) { return DecodeParams{1, &m->alpha, &m->p0}; }
+
+// Rejects a sweep the kernels cannot run: no pairs, more than INT_MAX jobs, or a value out of range.
+int check_decode(const uis_decode_params* dp, int U, DecodeParams* out) {
+  if (!dp) return fail(UIS_ERR_INVALID, "decode_params is NULL");
+  if (dp->count < 1) return fail(UIS_ERR_INVALID, "decode_params: count=%d (need >= 1)", dp->count);
+  if (!dp->crp_alpha || !dp->transition_bias) return fail(UIS_ERR_INVALID, "decode_params: null value array");
+  if ((long long)std::max(U, 1) * dp->count > std::numeric_limits<int>::max())
+    return fail(UIS_ERR_INVALID, "decode_params: %d utterances x %d pairs exceeds INT_MAX jobs", U, dp->count);
+  for (int c = 0; c < dp->count; ++c) {
+    const double a = dp->crp_alpha[c], b = dp->transition_bias[c];
+    if (!(std::isfinite(a) && a > 0.0))
+      return fail(UIS_ERR_INVALID, "decode_params pair %d: crp_alpha=%g (need finite and > 0)", c, a);
+    if (!(std::isfinite(b) && b > 0.0 && b < 1.0))
+      return fail(UIS_ERR_INVALID, "decode_params pair %d: transition_bias=%g (need finite and in (0, 1))", c, b);
+  }
+  *out = DecodeParams{dp->count, dp->crp_alpha, dp->transition_bias};
+  return 0;
+}
+
+struct Plan {
+  int B, L, T, Kcap, ctas, P, maxN, G;
+  uis::Kernel kernel = uis::Kernel::Beam;
+  bool forced = false;  // the caller asked for this latency mode: a refused launch is an error, not a fallback
+  int cluster = 1;      // Kernel::Cluster: CTAs per utterance (thread-block cluster size)
+  int tcn = 0;          // Kernel::TensorCore: columns per pass (uis_beam_tc.cuh)
+  int node_cap = 0, leaf_cap = 0, maxTN = 0, maxSteps = 0;  // look_ahead >= 2 only
+  // look_ahead >= 2: the spill kernel that decodes, from a device-memory arena, what outgrew shared memory.  It runs
+  // after Kernel::Tree, or instead of it as Kernel::TreeSpill (UISRNN_B200_TREE_SPILL=force); spill_ctas = 0: off.
+  int spill_ctas = 0, spill_ni = 0, spill_nlf = 0, spill_P = 0;
+  size_t spill_arena = 0, spill_budget = 0;  // arena bytes per spill CTA; the budget they were sized from
+  long long rows;
+};
+
+// Pool slots held by a plan's CTAs: the shared-memory kernel's and the spill kernel's run one after the other on the
+// same stream and share the pools.
+size_t pool_slots(const Plan& pl) {
+  return std::max((size_t)pl.ctas * pl.G * pl.P, (size_t)pl.spill_ctas * pl.spill_P);
+}
+
+// Sizes the spill kernel of a look-ahead plan.  The worst-case tree of one beam step at (B, Kcap, L) has
+// B * sum_{i=1}^{L-1} prod_{j<i} (Kcap + 1 + j) interior nodes plus the B winners, and B * prod_{j<L} (Kcap + 1 + j)
+// leaves.  Each spill CTA needs an arena for that tree and slot pools for its P; both are clipped (in proportion) to
+// the byte budget: UISRNN_B200_TREE_SPILL_MB, else the smaller of 2 GiB and a quarter of the free device memory.
+void plan_tree_spill(uis_model* m, Plan* pl) {
+  if (const char* env = std::getenv("UISRNN_B200_TREE_SPILL")) {
+    if (std::strcmp(env, "force") == 0) pl->kernel = uis::Kernel::TreeSpill;
+    else if (env[0] == '0') return;
+  }
+  size_t budget;
+  if (const char* env = std::getenv("UISRNN_B200_TREE_SPILL_MB")) {
+    budget = (size_t)std::max(0ll, std::atoll(env)) << 20;
+  } else {
+    size_t free_b = 0, total_b = 0;
+    uis::DeviceGuard g(m->device);
+    if (g.status != cudaSuccess || cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { (void)cudaGetLastError(); free_b = 0; }
+    budget = std::min<size_t>((size_t)2 << 30, (free_b + m->tree_arena.cap) / 4);  // the arena held is re-used
+  }
+  const int B = pl->B, K = pl->Kcap, L = pl->L;
+  const double slot_bytes = 4.0 * (m->D + m->depth * m->H + 1);
+  double ni = B, prod = 1;
+  for (int i = 1; i < L; ++i) { prod *= K + i; ni += B * prod; }
+  double nlf = B * prod * (K + L);
+  auto cost = [&](double n, double l) {
+    const int P = B * K + (int)n + B + 1;
+    return (double)uis::make_tree_arena((int)n, (int)l, P).total + P * slot_bytes;
+  };
+  // leaf positions are stored in 32 bits, parent node indices in 24 (l_pc = parent << 8 | cluster)
+  const double kMaxNi = (1 << 24) - 1, kMaxLeaves = 1 << 30;
+  if (ni > kMaxNi) { nlf *= kMaxNi / ni; ni = kMaxNi; }
+  if (nlf > kMaxLeaves) { ni *= kMaxLeaves / nlf; nlf = kMaxLeaves; }
+  for (double f = std::min(1.0, (double)budget / cost(ni, nlf)); cost(ni, nlf) > (double)budget && ni > 64; f = 0.9) {
+    ni = std::floor(ni * f);
+    nlf = std::floor(nlf * f);
+  }
+  pl->spill_ni = std::max(64, (int)ni);  // floor: one CTA with about the smallest on-chip tree
+  pl->spill_nlf = std::max(8 * 64, (int)nlf);
+  pl->spill_P = B * K + pl->spill_ni + B + 1;
+  const double per_cta = cost(pl->spill_ni, pl->spill_nlf);
+  pl->spill_ctas = (int)std::max(1.0, std::min((double)pl->ctas, std::floor((double)budget / per_cta)));
+  pl->spill_arena = uis::make_tree_arena(pl->spill_ni, pl->spill_nlf, pl->spill_P).total;
+  pl->spill_budget = budget;
+}
+
+// U utterances (rows, frame counts) decoded as U * configs jobs (engine, lanes, CTAs and latency modes).
+int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o, Plan* pl, int configs = 1) {
+  if (!m || !o || (U > 0 && !off)) return fail(UIS_ERR_INVALID, "null argument");
+  if (U < 0) return fail(UIS_ERR_INVALID, "U < 0");
+  if (o->beam_size < 1 || o->look_ahead < 1 || o->test_iteration < 1)
+    return fail(UIS_ERR_INVALID, "beam_size, look_ahead and test_iteration must be >= 1");
+  if (o->look_ahead > 8) return fail(UIS_ERR_UNSUPPORTED, "look_ahead=%d > 8 not supported", o->look_ahead);
+  if (o->beam_size > uis::kMaxBeam) return fail(UIS_ERR_UNSUPPORTED, "beam_size=%d > %d not supported", o->beam_size, uis::kMaxBeam);
+  if (o->beam_size > 32 && o->look_ahead > 1)
+    return fail(UIS_ERR_UNSUPPORTED, "beam_size=%d > 32 is supported with look_ahead 1 only (look_ahead=%d)", o->beam_size, o->look_ahead);
+  if (o->engine < 0 || o->engine > 2) return fail(UIS_ERR_INVALID, "engine must be 0 (auto), 1 (FFMA) or 2 (tensor cores)");
+  pl->B = o->beam_size;
+  pl->L = o->look_ahead;
+  pl->T = o->test_iteration;
+  const bool tree = pl->L > 1;
+  pl->Kcap = o->kcap > 0 ? o->kcap : (tree ? 16 : 32);
+  if (o->kcap <= 0 && pl->B > 32)  // wide beams: the per-hypothesis tables (B * kcap entries) must fit shared memory
+    while (pl->Kcap > 4 && kernel_smem(m, uis::Kernel::Beam, beam_sizes(pl->B, pl->Kcap, 1)) > uis::kSmemCap) pl->Kcap /= 2;
+  if (pl->Kcap > (pl->B > 32 ? 511 : 2047) || pl->B * pl->Kcap + pl->B + 1 > 65535) return fail(UIS_ERR_INVALID, "kcap too large");
+  if (tree && pl->Kcap > 255) return fail(UIS_ERR_UNSUPPORTED, "look_ahead >= 2 supports kcap <= 255");
+  pl->P = pl->B * pl->Kcap + pl->B + 1;
+  pl->rows = U > 0 ? off[U] : 0;
+  int maxN = 0;
+  for (int u = 0; u < U; ++u) {
+    const long long n = off[u + 1] - off[u];
+    if (n < 0) return fail(UIS_ERR_INVALID, "frame_offsets not monotone");
+    if (n * pl->T > (1ll << 30)) return fail(UIS_ERR_INVALID, "utterance too long");
+    maxN = std::max<long long>(maxN, n);
+  }
+  pl->maxN = std::max(maxN, 1);
+  const long long J = (long long)U * configs;  // jobs
+  int ctas = o->n_ctas > 0 ? o->n_ctas : m->num_sms;
+  // lanes (utterances advanced together by one CTA, sharing each weight pass): 2 when there is
+  // enough work to keep every CTA's lanes busy, else 1 (latency mode); opts->lanes overrides.
+  int G = o->lanes > 0 ? std::min(o->lanes, 4) : (J >= 2ll * ctas ? 2 : 1);
+  if (tree) {
+    // look-ahead tree kernel: one utterance per CTA; size the on-chip node / leaf arrays to what
+    // shared memory allows (internal nodes : leaves ~ 1 : 8, the typical fan-out K+2)
+    G = 1;
+    long long tn = 0;
+    for (int u = 0; u < U; ++u) tn = std::max<long long>(tn, (off[u + 1] - off[u]) * pl->T);
+    pl->maxTN = (int)std::max<long long>(tn, 1);
+    pl->maxSteps = (pl->maxTN + pl->L - 1) / pl->L;
+    int ni = 64;
+    auto fits = [&](int n) {
+      uis::BeamParams q = beam_sizes(pl->B, pl->Kcap, 1);
+      q.L = pl->L; q.node_cap = n; q.leaf_cap = 8 * n; q.P = pl->B * pl->Kcap + n + pl->B + 1;
+      return kernel_smem(m, uis::Kernel::Tree, q) <= uis::kSmemCap;
+    };
+    if (!fits(ni)) return fail(UIS_ERR_UNSUPPORTED, "look_ahead=%d beam_size=%d kcap=%d does not fit in shared memory", pl->L, pl->B, pl->Kcap);
+    while (ni < 4096 && fits(ni + 32)) ni += 32;
+    pl->node_cap = ni;
+    pl->leaf_cap = 8 * ni;
+    pl->P = pl->B * pl->Kcap + ni + pl->B + 1;
+    pl->kernel = uis::Kernel::Tree;
+  } else {
+    // Tensor-core engine (look_ahead 1, depth 1, 128-row-tileable shapes): the cost of a weight pass does not depend on
+    // the number of columns, so a CTA advances up to N / 8 utterances together (a lane needs ~6 columns per step,
+    // at most beam_size + 1).  Chosen automatically when some CTA gets more than one utterance; below that the
+    // one-lane FFMA kernel or the cluster (latency) mode is faster.  Its device tables default to 16 clusters per
+    // hypothesis (UIS_ERR_OVERFLOW asks the caller for more, as always).
+    if (o->engine != 1 && m->tc_ready && o->cluster <= 0) {
+      int N = 48;
+      if (const char* env = std::getenv("UISRNN_B200_TC_N")) N = std::atoi(env);
+      const int kc = o->kcap > 0 ? o->kcap : 16;
+      auto tc_smem = [&](int g) { return kernel_smem(m, uis::Kernel::TensorCore, beam_sizes(pl->B, kc, g), N); };
+      if (tc_smem(1) != uis::kNoKernel) {
+        int Gt = o->lanes > 0 ? std::min(o->lanes, (int)uis::kMaxLanes)
+                              : (int)std::min<long long>(N / 8, (J + ctas - 1) / std::max(ctas, 1));
+        Gt = std::max(Gt, 1);
+        while (Gt > 1 && (tc_smem(Gt) > uis::kSmemCap || Gt * pl->B > 256)) --Gt;
+        const bool fits = tc_smem(Gt) <= uis::kSmemCap && pl->B * kc + pl->B + 1 <= 65535;
+        if (fits && (o->engine == 2 || J > ctas)) {
+          pl->kernel = uis::Kernel::TensorCore;
+          pl->tcn = N;
+          pl->Kcap = kc;
+          pl->P = pl->B * kc + pl->B + 1;
+          G = Gt;
+        } else if (o->engine == 2) {
+          return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: beam_size=%d kcap=%d does not fit in shared memory", pl->B, kc);
+        }
+      } else if (o->engine == 2) {
+        return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: no kernel for hidden=%d dim=%d columns=%d", m->H, m->D, N);
+      }
+    } else if (o->engine == 2) {
+      return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine needs look_ahead 1, depth 1, hidden/dim multiples of 128, no "
+                                       "cluster mode and weights its fp16 split holds (uis_model_create)");
+    }
+    if (!pl->tcn)
+      while (G > 1 && kernel_smem(m, uis::Kernel::Beam, beam_sizes(pl->B, pl->Kcap, G)) > uis::kSmemCap) --G;
+    while (G > 1 && G * pl->B > 256) --G;  // at most 256 (lane, winner) pairs per CTA step
+  }
+  if (tree && o->engine == 2) return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: look_ahead must be 1");
+  pl->G = G;
+  pl->ctas = (int)std::max(1ll, std::min<long long>(ctas, std::max((J + G - 1) / G, 1ll)));
+  if (tree) plan_tree_spill(m, pl);
+  // Cluster (latency) mode: with fewer utterances than SMs, a thread-block cluster of 2/4/8 CTAs works on
+  // each utterance (k-split of every weight matrix, uis_beam.cuh).  opts->cluster: 0 = auto (largest of 4, 2
+  // that still gives every utterance its own cluster), -1 = off, 2/4/8 = forced; UISRNN_B200_CLUSTER=0 disables
+  // the automatic choice.
+  // Stationary-weights mode (uis_beam_stat.cuh): 32 CTAs per utterance keep the weights in shared memory.  The fastest
+  // way to decode up to #SMs / 32 utterances at a time; opts->cluster = 32 forces it, 0 picks it automatically,
+  // UISRNN_B200_STAT=0 disables the automatic choice.
+  if (!tree && U >= 1 && (o->cluster == 0 || o->cluster == uis::kStatGroup) && m->depth == 1 &&
+      o->lanes <= 1 && o->engine != 2) {
+    const char* env = std::getenv("UISRNN_B200_STAT");
+    const bool want = o->cluster == uis::kStatGroup ||
+                      (!(env && env[0] == '0') && J * uis::kStatGroup <= ctas && o->engine == 0 && o->n_ctas <= 0);
+    const int kc = o->kcap > 0 ? o->kcap : 32;
+    const bool can = ctas >= uis::kStatGroup && kernel_smem(m, uis::Kernel::Stat, beam_sizes(pl->B, kc, 1)) <= uis::kSmemCap &&
+                     pl->B * kc + pl->B + 1 <= 65535;
+    if (want && can) {
+      const int groups = (int)std::max(1ll, std::min<long long>(ctas / uis::kStatGroup, J));
+      pl->kernel = uis::Kernel::Stat;
+      pl->forced = o->cluster == uis::kStatGroup;
+      pl->tcn = 0;
+      pl->Kcap = kc;
+      pl->P = pl->B * kc + pl->B + 1;
+      pl->G = 1;
+      pl->ctas = groups * uis::kStatGroup;
+      return 0;
+    }
+    if (o->cluster == uis::kStatGroup)
+      return fail(UIS_ERR_UNSUPPORTED, "stationary-weights mode needs hidden=512 dim=256 depth=1, >= 32 CTAs and beam_size/kcap that fit in shared memory");
+  }
+  if (pl->kernel == uis::Kernel::Beam && U >= 1 && o->cluster >= 0 && m->depth == 1 && o->lanes <= 1) {
+    int cs = 0;
+    if (o->cluster == 2 || o->cluster == 4 || o->cluster == 8) {
+      cs = o->cluster;
+    } else if (o->cluster == 0) {
+      const char* env = std::getenv("UISRNN_B200_CLUSTER");
+      if (!(env && env[0] == '0'))
+        for (int c : {4, 2})
+          if (J * c <= ctas) { cs = c; break; }
+    } else {
+      return fail(UIS_ERR_INVALID, "cluster must be -1, 0, 2, 4, 8 or 32");
+    }
+    if (cs > 1 && kernel_smem(m, uis::Kernel::Cluster, beam_sizes(pl->B, pl->Kcap, 1)) <= uis::kSmemCap) {
+      const int clusters = (int)std::max(1ll, std::min<long long>(ctas / cs, J));
+      pl->kernel = uis::Kernel::Cluster;
+      pl->cluster = cs;
+      pl->forced = o->cluster > 0;
+      pl->G = 1;
+      pl->ctas = clusters * cs;
+    } else if (o->cluster > 0) {
+      return fail(UIS_ERR_UNSUPPORTED, "cluster mode needs hidden=512 dim=256 depth=1 and beam_size/kcap that fit in shared memory");
+    }
+  }
+  return 0;
+}
+
+size_t workspace_bytes(const uis_model* m, const Plan& pl, int U, int configs = 1) {
+  const size_t J = (size_t)U * configs;
+  size_t b = 0;
+  b += (size_t)pl.rows * 3 * m->H * 4;                                  // gi
+  b += pool_slots(pl) * (m->D + m->depth * m->H + 1) * 4;            // slot pools (+ Gaussian term per slot)
+  b += (size_t)pl.spill_ctas * pl.spill_arena;                          // look-ahead spill arenas
+  b += (size_t)pl.ctas * pl.G * (pl.L > 1 ? (size_t)pl.maxTN + pl.maxSteps : (size_t)pl.maxN) * pl.B * 4;  // back-pointers
+  b += (size_t)(U + 1) * 8 + J * 8 + 256;                               // offsets, order, status
+  if (configs > 1) b += (size_t)configs * (4096 + 3) * 8;               // log tables of the sweep (at least)
+  if (pl.tcn) b += (size_t)pl.ctas * pl.tcn * m->H * 4;                 // a = relu(W1 h' + b1) between two products
+  return b;
+}
+
+// Speaker bounds of a bounded call (host arrays, either may be NULL): 0 = no bound, max >= 1, 0 <= min <= max.
+struct SpeakerBounds {
+  const int32_t* max = nullptr;
+  const int32_t* min = nullptr;
+  int32_t* out_dev = nullptr;  // [U] device, may be NULL
+  SpeakerBounds at(int u0) const {
+    return SpeakerBounds{max ? max + u0 : nullptr, min ? min + u0 : nullptr, out_dev ? out_dev + u0 : nullptr};
+  }
+};
+
+// N-best outputs of a call (n_best = 1 with NULL pointers: a plain call).  Labels are n_best planes of the call's rows.
+struct NBestOut {
+  int k = 1;
+  float* scores = nullptr;     // [U][k]
+  int32_t* speakers = nullptr; // [U][k]
+  int32_t* count = nullptr;    // [U]
+};
+
+int check_bounds(int U, const int32_t* mx, const int32_t* mn) {
+  for (int u = 0; u < U; ++u) {
+    const int a = mx ? mx[u] : 0, b = mn ? mn[u] : 0;
+    if (a < 0 || b < 0 || (a > 0 && b > a))
+      return fail(UIS_ERR_INVALID, "utterance %d: max_speakers=%d min_speakers=%d (need max >= 1 or 0 = none, "
+                  "min >= 0, min <= max)", u, a, b);
+  }
+  return 0;
+}
+
+// n_best in [1, beam_size]; an N-best call needs its label and score buffers.
+int check_nbest(int n_best, const uis_predict_opts* opts, const uis_nbest_out* out) {
+  if (n_best < 1 || n_best > opts->beam_size)
+    return fail(UIS_ERR_INVALID, "n_best=%d (need 1 <= n_best <= beam_size=%d)", n_best, opts->beam_size);
+  if (!out->scores) return fail(UIS_ERR_INVALID, "n_best: null scores buffer");
+  return 0;
+}
+
+// ---- launch ------------------------------------------------------------------------------------------------------
+
+// What launch errors call each uis::Kernel: the missing instantiation, the kernel.
+const struct { const char *missing, *name; } kKernelNames[] = {
+    {"sm_90a kernel instantiated", "beam kernel"},
+    {"cluster-mode kernel", "cluster beam kernel"},
+    {"stationary-weights kernel", "stationary-weights beam kernel"},
+    {"tensor-core kernel", "tensor-core beam kernel"},
+    {"sm_90a kernel instantiated", "look-ahead kernel"},
+    {"sm_90a kernel instantiated", "look-ahead kernel"},
+};
+
+// Launches kernel k of plan `pl` on `ctas` CTAs and records its CTAs per utterance in stats.cluster.  A latency mode
+// that the planner chose on its own and whose launch is refused (e.g. a partitioned GPU that cannot co-schedule the
+// CTAs) gives way to the FFMA kernel on the same grid: its extra CTAs find the utterance queue empty.
+int launch(uis_model* m, const Plan& pl, uis::Kernel k, const uis::BeamParams& p, int ctas, cudaStream_t st) {
+  using uis::Kernel;
+  const unsigned smem = kernel_smem(m, k, p, pl.tcn);
+  if (smem > uis::kSmemCap) {
+    if (k == Kernel::Tree || k == Kernel::TreeSpill)
+      return fail(UIS_ERR_UNSUPPORTED, "look_ahead=%d beam_size=%d kcap=%d needs %u B of shared memory (> 227 KB)", p.L,
+                  p.B, p.Kcap, smem);
+    return fail(UIS_ERR_UNSUPPORTED, "beam_size=%d kcap=%d lanes=%d needs %u B of shared memory (> 227 KB); lower kcap",
+                p.B, p.Kcap, p.G, smem);
+  }
+  cudaError_t e = cudaSuccess;
+  const bool have = launch_kernel(m, k, p, ctas, pl.cluster, pl.tcn, smem, st, &e);
+  if (have && e == cudaSuccess) {
+    m->stats.cluster = k == Kernel::Stat ? uis::kStatGroup : k == Kernel::Cluster ? pl.cluster : 1;
+    return 0;
+  }
+  if ((k == Kernel::Cluster || k == Kernel::Stat) && !pl.forced) {
+    (void)cudaGetLastError();  // clear the launch error and fall back
+    return launch(m, pl, Kernel::Beam, p, ctas, st);
+  }
+  if (!have && k == Kernel::TensorCore)
+    return fail(UIS_ERR_UNSUPPORTED, "no tensor-core kernel for hidden=%d dim=%d columns=%d", m->H, m->D, pl.tcn);
+  if (!have)
+    return fail(UIS_ERR_UNSUPPORTED, "no %s for hidden=%d dim=%d", kKernelNames[(int)k].missing, m->H, m->D);
+  return fail(UIS_ERR_CUDA, "%s launch failed: %s", kKernelNames[(int)k].name, cudaGetErrorString(e));
+}
+
+// ---- run_device --------------------------------------------------------------------------------------------------
+
+// Log tables for decodes of up to max_tn frames under `dp`, built on the host with std::log so that a config's values
+// are those a model created with its pair uses.  Fills the table pointers of `p`.
+int ensure_log_tables(uis_model* m, int max_tn, const DecodeParams& dp, uis::BeamParams* p) {
+  const int need = max_tn + 2;
+  if (need > m->log_cap) {
+    const int cap = std::max(need, 4096);
+    std::vector<double> ln(cap);
+    ln[0] = -INFINITY;
+    for (int i = 1; i < cap; ++i) ln[i] = std::log((double)i);  // np.log(block_counts[c])
+    if (int rc = upload(m->logn, ln.data(), cap * sizeof(double))) return rc;
+    m->log_cap = cap;
+  }
+  // the model's own pair (by value: the Python binding passes it as a one-pair sweep) keeps its own tables, so that
+  // alternating plain calls with a sweep does not rebuild a table on every call
+  const bool own = dp.count == 1 && std::memcmp(dp.alpha, &m->alpha, sizeof(double)) == 0 &&
+                   std::memcmp(dp.p0, &m->p0, sizeof(double)) == 0;
+  uis_model::LogTables& t = own ? m->own_logs : m->sweep_logs;
+  std::vector<double> key;
+  for (int c = 0; c < dp.count; ++c) { key.push_back(dp.alpha[c]); key.push_back(dp.p0[c]); }
+  if (need > t.cap || key != t.key) {
+    const int cap = std::max({need, 4096, t.cap});
+    if (t.cap) CU(cudaDeviceSynchronize());  // the tables are rewritten in place: no earlier call may still read them
+    std::vector<double> lt((size_t)dp.count * cap), cv((size_t)dp.count * 3);
+    for (int c = 0; c < dp.count; ++c) {
+      for (int i = 0; i < cap; ++i) lt[(size_t)c * cap + i] = std::log((double)i + dp.alpha[c]);  // np.log(sum(block_counts) + alpha)
+      cv[3 * c] = std::log(dp.p0[c]);            // np.log(self.transition_bias)      uisrnn.py:418
+      cv[3 * c + 1] = std::log(1.0 - dp.p0[c]);  // np.log(1 - self.transition_bias)  uisrnn.py:416
+      cv[3 * c + 2] = std::log(dp.alpha[c]);     // np.log(self.crp_alpha)            uisrnn.py:445
+    }
+    t.cap = 0;
+    t.key.clear();
+    if (int rc = upload(t.tot, lt.data(), lt.size() * sizeof(double))) return rc;
+    if (int rc = upload(t.cfg, cv.data(), cv.size() * sizeof(double))) return rc;
+    t.cap = cap;
+    t.key = key;
+  }
+  p->logn = m->logn.as<double>();
+  p->logtot = t.tot.as<double>();
+  p->cfg_log = t.cfg.as<double>();
+  p->logtot_stride = t.cap;
+  return 0;
+}
+
+// The model's part of the kernel parameters: weights and constants (ensure_log_tables adds the log terms).
+uis::BeamParams model_params(const uis_model* m) {
+  const int H = m->H;
+  uis::BeamParams p{};
+  p.whh_t = m->whh_t.as<float>(); p.w1_t = m->w1_t.as<float>(); p.w2_t = m->w2_t.as<float>();
+  p.depth = m->depth;
+  for (int l = 1; l < m->depth; ++l) {
+    p.wih_up_t[l - 1] = m->wih_up_t.as<float>() + (size_t)(l - 1) * H * 3 * H;
+    p.whh_up_t[l - 1] = m->whh_t.as<float>() + (size_t)l * H * 3 * H;
+  }
+  p.bih_up = m->bih.as<float>() + 3 * H;   // layers >= 1
+  p.bhh_up = m->bhh.as<float>() + 3 * H;
+  p.bhh = m->bhh.as<float>(); p.b1 = m->b1.as<float>(); p.b2 = m->b2.as<float>();
+  p.wvec = m->wvec.as<float>(); p.mean0 = m->mean0.as<float>(); p.hidden0 = m->hidden0.as<float>();
+  return p;
+}
+
+// Decodes U utterances under dp.count configs: J = U * dp.count jobs, job j = utterance j % U under config j / U.
+// Per-job outputs (status, N-best scores / speakers / counts, taps) are [J]; labels_dev holds dp.count * nb.k planes
+// of the call's rows (plane c * nb.k + j: config c, hypothesis j).
+int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, const Plan& pl, int32_t* labels_dev,
+               const uis_debug_taps* taps, cudaStream_t st, const SpeakerBounds& sb, const NBestOut& nb,
+               const DecodeParams& dp, bool gi_ready = false) {
+  const int H = m->H, D = m->D;
+  const int J = U * dp.count;
+  if (sb.out_dev && U > 0) CU(cudaMemsetAsync(sb.out_dev, 0, (size_t)J * sizeof(int32_t), st));  // empty inputs: 0
+  if (U > 0 && pl.rows == 0) {  // no kernel runs: every utterance is empty and returns no hypothesis
+    if (nb.count) CU(cudaMemsetAsync(nb.count, 0, (size_t)J * sizeof(int32_t), st));
+    if (nb.speakers) CU(cudaMemsetAsync(nb.speakers, 0, (size_t)J * nb.k * sizeof(int32_t), st));
+    if (nb.scores) {
+      const std::vector<float> inf((size_t)J * nb.k, std::numeric_limits<float>::infinity());
+      CU(cudaMemcpyAsync(nb.scores, inf.data(), inf.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+      CU(cudaStreamSynchronize(st));  // (inf is about to go out of scope)
+    }
+  }
+  m->stats = uis_stats{};
+  m->stats.utterances = J;
+  m->stats.frames = pl.rows;
+  m->stats.ctas = pl.ctas;
+  m->stats.lanes = pl.G;
+  m->stats.cluster = pl.cluster;
+  m->last_U = J;
+  m->last_score = false;
+  m->last_tree_spill = pl.spill_ctas > 0;
+  m->last_spill_ni = pl.spill_ni; m->last_spill_nlf = pl.spill_nlf; m->last_spill_budget = pl.spill_budget;
+  m->last_stream = st;
+  m->stats_pending = false;
+  if (U == 0 || pl.rows == 0) {
+    return 0;
+  }
+  uis::BeamParams p = model_params(m);
+  long long max_tn = 0;
+  for (int u = 0; u < U; ++u) max_tn = std::max<long long>(max_tn, (off[u + 1] - off[u]) * pl.T);
+  if (int rc = ensure_log_tables(m, (int)max_tn, dp, &p)) return rc;
+
+  // schedule: longest utterance first (LPT) -- steps are strictly sequential per utterance.  The configs of one
+  // utterance follow each other, so that they read the same input rows at about the same time.
+  std::vector<int> by_len(U), order((size_t)J);
+  std::iota(by_len.begin(), by_len.end(), 0);
+  std::stable_sort(by_len.begin(), by_len.end(),
+                   [&](int a, int b) { return off[a + 1] - off[a] > off[b + 1] - off[b]; });
+  for (int i = 0; i < U; ++i)
+    for (int c = 0; c < dp.count; ++c) order[(size_t)i * dp.count + c] = c * U + by_len[i];
+  std::vector<long long> off_ll(off, off + U + 1);
+
+  if (int rc = m->row_off.ensure((U + 1) * sizeof(long long))) return rc;
+  if (int rc = m->order.ensure((size_t)J * sizeof(int))) return rc;
+  if (int rc = m->status.ensure((size_t)J * sizeof(int))) return rc;
+  if (int rc = m->queue_stats.ensure(40 * sizeof(unsigned long long))) return rc;
+  if (int rc = m->gi.ensure((size_t)pl.rows * 3 * H * sizeof(float))) return rc;
+  if (int rc = m->pool_mean.ensure(pool_slots(pl) * D * sizeof(float))) return rc;
+  if (int rc = m->pool_hidden.ensure(pool_slots(pl) * m->depth * H * sizeof(float))) return rc;
+  if (int rc = m->pool_mse.ensure(pool_slots(pl) * sizeof(float))) return rc;
+  if (int rc = m->tree_arena.ensure((size_t)pl.spill_ctas * pl.spill_arena)) return rc;
+  if (int rc = m->bp.ensure((size_t)pl.ctas * pl.G * (pl.L > 1 ? (size_t)pl.maxTN + pl.maxSteps : (size_t)pl.maxN) * pl.B *
+                            sizeof(unsigned)))
+    return rc;
+
+  if (pl.tcn)
+    if (int rc = m->tc_scratch.ensure((size_t)pl.ctas * pl.tcn * H * sizeof(float))) return rc;
+  if (pl.kernel == uis::Kernel::Stat) {  // pl.ctas / kStatGroup groups
+    if (int rc = m->stat_bar.ensure((size_t)pl.ctas * sizeof(unsigned))) return rc;
+    if (int rc = m->stat_scratch.ensure((size_t)(pl.ctas / uis::kStatGroup) * uis::kCPCluster * H * sizeof(float))) return rc;
+    CU(cudaMemsetAsync(m->stat_bar.p, 0, (size_t)pl.ctas * sizeof(unsigned), st));
+  }
+
+  CU(cudaMemcpyAsync(m->row_off.p, off_ll.data(), (U + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(m->order.p, order.data(), (size_t)J * sizeof(int), cudaMemcpyHostToDevice, st));
+  CU(cudaMemsetAsync(m->queue_stats.p, 0, 40 * sizeof(unsigned long long), st));
+  CU(cudaMemsetAsync(m->status.p, 0xff, (size_t)J * sizeof(int), st));
+
+  p.x = x_dev; p.gi = m->gi.as<float>();
+  p.row_off = m->row_off.as<long long>(); p.order = m->order.as<int>();
+  p.U = J; p.n_utt = U; p.B = pl.B; p.Kcap = pl.Kcap; p.T = pl.T; p.P = pl.P; p.maxN = pl.maxN; p.G = pl.G;
+  p.L = pl.L; p.node_cap = pl.node_cap; p.leaf_cap = pl.leaf_cap; p.maxTN = pl.maxTN; p.maxSteps = pl.maxSteps;
+  { const char* e = getenv("UIS_DBG_MODE"); p.dbg_mode = e ? atoi(e) : 0; }
+  p.pool_mean = m->pool_mean.as<float>(); p.pool_hidden = m->pool_hidden.as<float>(); p.pool_mse = m->pool_mse.as<float>();
+  p.bp = m->bp.as<unsigned>();
+  p.queue = m->queue_stats.as<int>();
+  p.stats = m->queue_stats.as<unsigned long long>() + 8;
+  p.labels = labels_dev; p.status = m->status.as<int>();
+  if (sb.max || sb.min) {
+    std::vector<int32_t> kb(2 * (size_t)U);
+    for (int u = 0; u < U; ++u) { kb[2 * u] = sb.max ? sb.max[u] : 0; kb[2 * u + 1] = sb.min ? sb.min[u] : 0; }
+    if (int rc = m->spk_bound.ensure(kb.size() * sizeof(int32_t))) return rc;
+    CU(cudaMemcpyAsync(m->spk_bound.p, kb.data(), kb.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    p.spk_bound = m->spk_bound.as<int>();
+  }
+  p.spk_out = sb.out_dev;
+  p.n_best = nb.k; p.label_plane = pl.rows;
+  p.nbest_scores = nb.scores; p.nbest_speakers = nb.speakers; p.nbest_count = nb.count;
+  p.trace_utt = -1;
+  if (pl.kernel == uis::Kernel::Stat) {
+    p.stat_bar = m->stat_bar.as<unsigned>();
+    p.stat_scratch = m->stat_scratch.as<float>();
+  }
+  if (pl.tcn) {
+    p.tc_wmap = m->tc_map;
+    p.tc_sh = m->tc_sh; p.tc_sa = m->tc_sa;
+    p.tc_inv_hh = m->tc_inv_hh; p.tc_inv_1 = m->tc_inv_1; p.tc_inv_2 = m->tc_inv_2;
+    p.tc_scratch = m->tc_scratch.as<float>();
+  }
+
+  long long trace_steps = 0;
+  if (taps) {
+    if (taps->final_scores) {
+      if (int rc = m->dbg_final_scores.ensure((size_t)J * pl.B * 4)) return rc;
+      p.dbg_final_scores = m->dbg_final_scores.as<float>();
+      if (int rc = m->dbg_final_k.ensure((size_t)J * 4)) return rc;
+      p.dbg_final_k = m->dbg_final_k.as<int>();
+    }
+    if (taps->trace_utt >= 0 && taps->trace_utt < J) {  // a job: utterance trace_utt % U under config trace_utt / U
+      p.trace_utt = taps->trace_utt;
+      p.trace_capacity = std::max(taps->trace_capacity, 0);
+      const int tu = p.trace_utt % U;
+      trace_steps = ((off[tu + 1] - off[tu]) * pl.T + pl.L - 1) / pl.L;
+      if (taps->step_winners && p.trace_capacity > 0) {
+        if (int rc = m->dbg_win.ensure((size_t)p.trace_capacity * 4 * (1 + pl.L))) return rc;
+        if (int rc = m->dbg_score.ensure((size_t)p.trace_capacity * 4)) return rc;
+        if (int rc = m->dbg_off.ensure((size_t)(trace_steps + 1) * 8)) return rc;
+        p.dbg_win = m->dbg_win.as<int>(); p.dbg_score = m->dbg_score.as<float>();
+        p.dbg_off = m->dbg_off.as<long long>();
+      }
+      if (taps->best_mean) {
+        if (int rc = m->dbg_best_mean.ensure((size_t)pl.Kcap * D * 4)) return rc;
+        if (int rc = m->dbg_best_hidden.ensure((size_t)pl.Kcap * m->depth * H * 4)) return rc;
+        if (int rc = m->dbg_best_blocks.ensure((size_t)pl.Kcap * 4)) return rc;
+        p.dbg_best_mean = m->dbg_best_mean.as<float>(); p.dbg_best_hidden = m->dbg_best_hidden.as<float>();
+        p.dbg_best_blocks = m->dbg_best_blocks.as<int>();
+      }
+    }
+  }
+
   for (auto& e : m->ev)
-    if (e) cudaEventDestroy(e);
-  for (auto& e : m->ev_copied)
-    if (e) cudaEventDestroy(e);
-  for (auto& e : m->ev_free)
-    if (e) cudaEventDestroy(e);
-  for (auto& e : m->ev_h2d)
-    if (e) cudaEventDestroy(e);
-  if (m->ev_pipe) cudaEventDestroy(m->ev_pipe);
-  if (m->copy_stream) cudaStreamDestroy(m->copy_stream);
-  if (m->labels_pin) cudaFreeHost(m->labels_pin);
-  for (auto& e : m->ev_dma)
-    if (e) cudaEventDestroy(e);
-  if (m->pin_stage) cudaFreeHost(m->pin_stage);
-  delete m->copy_pool;
-  delete m;
+    if (!e) CU(cudaEventCreate(&e));
+  CU(cudaEventRecord(m->ev[0], st));
+  // kernel 1: input projection GEMM (the host-buffer path has already run it chunk by chunk, under the H2D copies)
+  if (!gi_ready) {
+    dim3 grid((3 * H + uis::PBN - 1) / uis::PBN, (unsigned)((pl.rows + uis::PBM - 1) / uis::PBM));
+    uis::input_proj_kernel<<<grid, 256, 0, st>>>(x_dev, m->wih_t.as<float>(), m->bih.as<float>(), m->gi.as<float>(),
+                                                (int)pl.rows, 3 * H, D);
+    CU(cudaGetLastError());
+  }
+  CU(cudaEventRecord(m->ev[1], st));
+  // kernel 2: the planned persistent beam search.  Look-ahead: the spill kernel right behind it on the same stream
+  // decodes the utterances it left at status -5 (every one under Kernel::TreeSpill) from a second queue; its CTAs find
+  // nothing to do and exit when every tree fitted.
+  if (pl.kernel != uis::Kernel::TreeSpill)
+    if (int rc = launch(m, pl, pl.kernel, p, pl.ctas, st)) return rc;
+  if (pl.spill_ctas) {
+    uis::BeamParams ps = p;
+    ps.node_cap = pl.spill_ni; ps.leaf_cap = pl.spill_nlf; ps.P = pl.spill_P;
+    ps.queue = p.queue + 1;
+    ps.tree_arena = m->tree_arena.as<unsigned char>();
+    ps.tree_spill_all = pl.kernel == uis::Kernel::TreeSpill;
+    if (int rc = launch(m, pl, uis::Kernel::TreeSpill, ps, pl.spill_ctas, st)) return rc;
+  }
+  m->stats.engine = pl.tcn ? 2 : 1;
+  m->stats.tc_columns = pl.tcn;
+  CU(cudaEventRecord(m->ev[2], st));
+  m->stats.kernel_launches = 2 + (pl.kernel == uis::Kernel::Tree && pl.spill_ctas ? 1 : 0);
+  m->stats_pending = true;
+
+  if (taps) {
+    CU(cudaStreamSynchronize(st));
+    if (p.dbg_final_scores) {
+      CU(cudaMemcpy(taps->final_scores, p.dbg_final_scores, (size_t)J * pl.B * 4, cudaMemcpyDeviceToHost));
+      if (taps->final_k) CU(cudaMemcpy(taps->final_k, p.dbg_final_k, (size_t)J * 4, cudaMemcpyDeviceToHost));
+    }
+    if (p.dbg_win) {
+      CU(cudaMemcpy(taps->step_winners, p.dbg_win, (size_t)p.trace_capacity * 4 * (1 + pl.L), cudaMemcpyDeviceToHost));
+      CU(cudaMemcpy(taps->step_scores, p.dbg_score, (size_t)p.trace_capacity * 4, cudaMemcpyDeviceToHost));
+      if (taps->step_offsets)
+        CU(cudaMemcpy(taps->step_offsets, p.dbg_off, (size_t)(trace_steps + 1) * 8, cudaMemcpyDeviceToHost));
+    }
+    if (p.dbg_best_mean) {
+      CU(cudaMemcpy2D(taps->best_mean, (size_t)m->D_user * 4, p.dbg_best_mean, (size_t)D * 4, (size_t)m->D_user * 4, pl.Kcap,
+                      cudaMemcpyDeviceToHost));
+      if (taps->best_hidden)
+        CU(cudaMemcpy2D(taps->best_hidden, (size_t)m->H_user * 4, p.dbg_best_hidden, (size_t)H * 4, (size_t)m->H_user * 4,
+                        (size_t)pl.Kcap * m->depth, cudaMemcpyDeviceToHost));
+      if (taps->best_blocks)
+        CU(cudaMemcpy(taps->best_blocks, p.dbg_best_blocks, (size_t)pl.Kcap * 4, cudaMemcpyDeviceToHost));
+    }
+  }
   return 0;
 }
 
-int uis_model_constants(uis_model* m, float* mean0, float* hidden0) {
-  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
-  uis::DeviceGuard device_guard_(m->device);
-  CU(device_guard_.status);
-  if (mean0) CU(cudaMemcpy(mean0, m->mean0.p, m->D_user * 4, cudaMemcpyDeviceToHost));
-  if (hidden0)
-    CU(cudaMemcpy2D(hidden0, (size_t)m->H_user * 4, m->hidden0.p, (size_t)m->H * 4, (size_t)m->H_user * 4, m->depth,
-                    cudaMemcpyDeviceToHost));
+// Pull the device-side counters and per-utterance status of the last call (synchronises).
+int collect(uis_model* m) {
+  if (!m->stats_pending) return 0;
+  CU(cudaStreamSynchronize(m->last_stream));
+  unsigned long long s[24];
+  CU(cudaMemcpy(s, m->queue_stats.as<unsigned long long>() + 8, sizeof s, cudaMemcpyDeviceToHost));
+  if (m->last_score) {  // the chain kernel's columns and passes; max_k came from the labels
+    m->stats.gru_columns = (int64_t)s[0];
+    m->stats.weight_passes = (int64_t)s[1];
+    CU(cudaEventElapsedTime(&m->stats.prepass_ms, m->ev[0], m->ev[1]));
+    CU(cudaEventElapsedTime(&m->stats.beam_ms, m->ev[1], m->ev[2]));
+    m->stats_pending = false;
+    return 0;
+  }
+  for (int i = 0; i < 10; ++i) m->stats.phase_cycles[i] = (int64_t)s[8 + i];
+  for (int i = 0; i < 4; ++i) m->stats.tc_cycles[i] = (int64_t)s[18 + i];
+  m->stats.gru_columns = (int64_t)s[0];
+  m->stats.weight_passes = (int64_t)s[1];
+  m->stats.candidates = (int64_t)s[2];
+  m->stats.beam_steps = (int64_t)s[3];
+  m->stats.max_k = (int32_t)s[4];
+  CU(cudaEventElapsedTime(&m->stats.prepass_ms, m->ev[0], m->ev[1]));
+  CU(cudaEventElapsedTime(&m->stats.beam_ms, m->ev[1], m->ev[2]));
+  m->stats_pending = false;
+  std::vector<int> status(m->last_U);
+  CU(cudaMemcpy(status.data(), m->status.p, (size_t)m->last_U * sizeof(int), cudaMemcpyDeviceToHost));
+  int overflow = 0, bad = 0, capacity = 0;
+  for (int v : status) {
+    if (v == -4) ++overflow;
+    else if (v == -5) ++capacity;
+    else if (v != 0) ++bad;
+  }
+  if (capacity && m->last_tree_spill)
+    return fail(UIS_ERR_CAPACITY, "%d utterance(s): the look-ahead tree of one beam step exhausted the device-memory arena "
+                "(%d nodes / %d leaves per CTA from a budget of %zu MiB; raise UISRNN_B200_TREE_SPILL_MB or lower "
+                "beam_size / look_ahead / kcap)", capacity, m->last_spill_ni, m->last_spill_nlf, m->last_spill_budget >> 20);
+  if (capacity)
+    return fail(UIS_ERR_CAPACITY, "%d utterance(s): the look-ahead tree of one beam step outgrew the on-chip node arrays "
+                "(lower beam_size / look_ahead / kcap)", capacity);
+  if (overflow)
+    return fail(UIS_ERR_OVERFLOW, "%d utterance(s) opened more clusters than kcap; retry with a larger kcap", overflow);
+  if (bad) return fail(UIS_ERR_INVALID, "%d utterance(s) ended with no finite hypothesis", bad);
   return 0;
 }
-
-size_t uis_predict_workspace_bytes(uis_model* m, const int64_t* frame_offsets, int U, const uis_predict_opts* opts) {
-  Plan pl;
-  if (make_plan(m, frame_offsets, U, opts, &pl)) return 0;
-  return workspace_bytes(m, pl, U);
-}
-
-int uis_predict_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
-                       const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream) {
-  return uis_predict_device_bounded(m, x_dev, frame_offsets, U, opts, labels_dev, taps, stream, nullptr, nullptr, nullptr);
-}
-
-int uis_predict_device_bounded(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
-                               const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
-                               const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev) {
-  return predict_device_impl(m, x_dev, frame_offsets, U, opts, labels_dev, taps, stream, max_speakers, min_speakers,
-                             speakers_dev, NBestOut{});
-}
-
-int uis_predict_device_nbest(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
-                             const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
-                             const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
-                             const uis_nbest_out* out) {
-  if (!opts || !out) return fail(UIS_ERR_INVALID, "null argument");
-  if (int rc = check_nbest(n_best, opts, out)) return rc;
-  return predict_device_impl(m, x_dev, frame_offsets, U, opts, out->labels_dev, taps, stream, max_speakers, min_speakers,
-                             nullptr, NBestOut{n_best, out->scores, out->speakers, out->count});
-}
-
-int uis_predict_device_sweep(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
-                             const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
-                             const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
-                             const uis_nbest_out* out, const uis_decode_params* params) {
-  if (!m || !opts || !out) return fail(UIS_ERR_INVALID, "null argument");
-  if (int rc = check_nbest(n_best, opts, out)) return rc;
-  DecodeParams dp;
-  if (int rc = check_decode(params, U, &dp)) return rc;
-  return predict_device_impl(m, x_dev, frame_offsets, U, opts, out->labels_dev, taps, stream, max_speakers, min_speakers,
-                             nullptr, NBestOut{n_best, out->scores, out->speakers, out->count}, &dp);
-}
-
-}  // extern "C"
-
-namespace {
 
 // Zero-pads the caller's `rows` device rows (D_user wide) to the kernel's row length D in m->x32 and points *x_dev
 // there; a model whose D_user is the kernel's D is left alone.
@@ -1300,7 +1148,7 @@ void drain_after_failure(uis_model* m, cudaStream_t st) {
 int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
                         const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
                         const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev,
-                        const NBestOut& nb, const DecodeParams* dpp) {
+                        const NBestOut& nb, const DecodeParams* dpp = nullptr) {
   if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
   const DecodeParams dp = dpp ? *dpp : model_decode(m);
   Plan pl;
@@ -1314,6 +1162,8 @@ int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_o
   return run_device(m, x_dev, frame_offsets, U, pl, labels_dev, taps, st,
                     SpeakerBounds{max_speakers, min_speakers, speakers_dev}, nb, dp);
 }
+
+// ---- host input pipeline -----------------------------------------------------------------------------------------
 
 int ensure_host_path(uis_model* m) {
   if (!m->copy_stream) CU(cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
@@ -1335,99 +1185,6 @@ size_t staging_chunk_rows(int d_user) {
   long long mb = 32;
   if (const char* env = std::getenv("UISRNN_B200_CHUNK_MB")) mb = std::max(0ll, std::atoll(env));  // 0 = the 256-row floor
   return std::max<size_t>(256, (size_t)mb * (1u << 20) / ((size_t)d_user * 8));
-}
-
-// One group of utterances, host buffers in, host buffers out: chunked H2D on the copy stream || cast + input
-// projection on `st`, then the beam kernel, then one D2H copy of all labels.
-int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
-                            const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
-                            const SpeakerBounds& sb, int32_t* speakers_out, const NBestOut& nb, int u0, int U_all,
-                            const DecodeParams& dp);
-
-int stage_host_rows(uis_model* m, const double* const* seqs, int U, const int64_t* off, size_t rows, cudaStream_t st,
-                    int* n_chunks_out, bool* staged_out);
-
-// Utterances [u0, u0 + U) of a list of U_all; `nb` holds the whole list's [configs][U_all][k] outputs.
-int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
-                       const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
-                       const SpeakerBounds& sb, int32_t* speakers_out, const NBestOut& nb, int u0, int U_all,
-                       const DecodeParams& dp) {
-  const int rc = predict_host_group_impl(m, seqs, n_frames, U, off, pl, labels_out, taps, st, sb, speakers_out, nb, u0,
-                                         U_all, dp);
-  if (rc != 0 && rc != UIS_ERR_OVERFLOW && rc != UIS_ERR_CAPACITY) drain_after_failure(m, st);
-  return rc;
-}
-
-int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
-                            const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
-                            const SpeakerBounds& sb_host, int32_t* speakers_out, const NBestOut& nb_host, int u0,
-                            int U_all, const DecodeParams& dp) {
-  const size_t rows = (size_t)pl.rows;
-  const int C = dp.count, J = U * C;
-  if (rows == 0) {
-    m->stats = uis_stats{};
-    m->stats.utterances = J;
-    return 0;
-  }
-  const int K = nb_host.k;
-  const size_t planes = (size_t)K * C;  // label planes: [config][hypothesis]
-  if (int rc = m->labels.ensure(rows * 4 * planes)) return rc;
-  SpeakerBounds sb = sb_host;  // speaker counts land in the handle's device buffer, then in `speakers_out`
-  if (speakers_out) {
-    if (int rc = m->spk_out.ensure((size_t)U * 4)) return rc;
-    sb.out_dev = m->spk_out.as<int32_t>();
-  }
-  NBestOut nb{K};  // likewise the N-best scores, cluster counts and hypothesis counts
-  if (nb_host.scores) {
-    if (int rc = m->nb_scores.ensure((size_t)J * K * 4)) return rc;
-    nb.scores = m->nb_scores.as<float>();
-  }
-  if (nb_host.speakers) {
-    if (int rc = m->nb_speakers.ensure((size_t)J * K * 4)) return rc;
-    nb.speakers = m->nb_speakers.as<int32_t>();
-  }
-  if (nb_host.count) {
-    if (int rc = m->nb_count.ensure((size_t)J * 4)) return rc;
-    nb.count = m->nb_count.as<int32_t>();
-  }
-  if (rows * 4 * planes > m->labels_pin_cap) {
-    if (m->labels_pin) cudaFreeHost(m->labels_pin);
-    m->labels_pin = nullptr;
-    m->labels_pin_cap = 0;
-    const size_t want = rows * 4 * planes + rows / 2 + 4096;
-    if (cudaMallocHost(&m->labels_pin, want) != cudaSuccess) {
-      (void)cudaGetLastError();
-      return fail(UIS_ERR_NOMEM, "cudaMallocHost(%zu) for the label staging buffer failed", want);
-    }
-    m->labels_pin_cap = want;
-  }
-  int n_chunks = 0;
-  bool staged = false;
-  if (int rc = stage_host_rows(m, seqs, U, off, rows, st, &n_chunks, &staged)) return rc;
-  if (int rc = run_device(m, m->x32.as<float>(), off, U, pl, m->labels.as<int32_t>(), taps, st, sb, nb, dp,
-                         /*gi_ready=*/true))
-    return rc;
-  m->stats.kernel_launches = 1 + 2 * (int64_t)n_chunks + (pl.L > 1 && pl.spill == 1 ? 1 : 0);
-  m->stats.chunks = n_chunks;
-  m->stats.staged = staged ? 1 : 0;
-  CU(cudaMemcpyAsync(m->labels_pin, m->labels.p, rows * 4 * planes, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  for (size_t j = 0; j < planes; ++j)  // plane j of the device rows -> rows j of the caller's [C][K][n_frames[q]] buffers
-    for (int q = 0; q < U; ++q)
-      if (n_frames[q] > 0)
-        std::memcpy(labels_out[q] + j * n_frames[q], m->labels_pin + j * rows + off[q], (size_t)n_frames[q] * 4);
-  if (speakers_out) CU(cudaMemcpy(speakers_out, sb.out_dev, (size_t)U * 4, cudaMemcpyDeviceToHost));
-  for (int c = 0; c < C; ++c) {  // config c's block of this group -> [c][u0 ..][K] of the whole list's outputs
-    const size_t dst = (size_t)c * U_all + u0, src = (size_t)c * U;
-    if (nb.scores) CU(cudaMemcpy(nb_host.scores + dst * K, nb.scores + src * K, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
-    if (nb.speakers)
-      CU(cudaMemcpy(nb_host.speakers + dst * K, nb.speakers + src * K, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
-    if (nb.count) CU(cudaMemcpy(nb_host.count + dst, nb.count + src, (size_t)U * 4, cudaMemcpyDeviceToHost));
-  }
-  if (int rc = collect(m)) return rc;
-  CU(cudaEventElapsedTime(&m->stats.h2d_ms, m->ev_h2d[0], m->ev_h2d[1]));
-  CU(cudaEventElapsedTime(&m->stats.pipeline_ms, m->ev_pipe, m->ev[1]));  // first cast -> beam kernel start
-  return 0;
 }
 
 // Input pipeline of the host-buffer entry points (uis_predict*, uis_score): the float64 rows of utterances [0, U)
@@ -1536,6 +1293,91 @@ int stage_host_rows(uis_model* m, const double* const* seqs, int U, const int64_
   return 0;
 }
 
+// One group of utterances, host buffers in, host buffers out: chunked H2D on the copy stream || cast + input
+// projection on `st`, then the beam kernel, then one D2H copy of all labels.
+int predict_host_group_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
+                            const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
+                            const SpeakerBounds& sb_host, int32_t* speakers_out, const NBestOut& nb_host, int u0,
+                            int U_all, const DecodeParams& dp) {
+  const size_t rows = (size_t)pl.rows;
+  const int C = dp.count, J = U * C;
+  if (rows == 0) {
+    m->stats = uis_stats{};
+    m->stats.utterances = J;
+    return 0;
+  }
+  const int K = nb_host.k;
+  const size_t planes = (size_t)K * C;  // label planes: [config][hypothesis]
+  if (int rc = m->labels.ensure(rows * 4 * planes)) return rc;
+  SpeakerBounds sb = sb_host;  // speaker counts land in the handle's device buffer, then in `speakers_out`
+  if (speakers_out) {
+    if (int rc = m->spk_out.ensure((size_t)U * 4)) return rc;
+    sb.out_dev = m->spk_out.as<int32_t>();
+  }
+  NBestOut nb{K};  // likewise the N-best scores, cluster counts and hypothesis counts
+  if (nb_host.scores) {
+    if (int rc = m->nb_scores.ensure((size_t)J * K * 4)) return rc;
+    nb.scores = m->nb_scores.as<float>();
+  }
+  if (nb_host.speakers) {
+    if (int rc = m->nb_speakers.ensure((size_t)J * K * 4)) return rc;
+    nb.speakers = m->nb_speakers.as<int32_t>();
+  }
+  if (nb_host.count) {
+    if (int rc = m->nb_count.ensure((size_t)J * 4)) return rc;
+    nb.count = m->nb_count.as<int32_t>();
+  }
+  if (rows * 4 * planes > m->labels_pin_cap) {
+    if (m->labels_pin) cudaFreeHost(m->labels_pin);
+    m->labels_pin = nullptr;
+    m->labels_pin_cap = 0;
+    const size_t want = rows * 4 * planes + rows / 2 + 4096;
+    if (cudaMallocHost(&m->labels_pin, want) != cudaSuccess) {
+      (void)cudaGetLastError();
+      return fail(UIS_ERR_NOMEM, "cudaMallocHost(%zu) for the label staging buffer failed", want);
+    }
+    m->labels_pin_cap = want;
+  }
+  int n_chunks = 0;
+  bool staged = false;
+  if (int rc = stage_host_rows(m, seqs, U, off, rows, st, &n_chunks, &staged)) return rc;
+  if (int rc = run_device(m, m->x32.as<float>(), off, U, pl, m->labels.as<int32_t>(), taps, st, sb, nb, dp,
+                         /*gi_ready=*/true))
+    return rc;
+  m->stats.kernel_launches = 1 + 2 * (int64_t)n_chunks + (pl.kernel == uis::Kernel::Tree && pl.spill_ctas ? 1 : 0);
+  m->stats.chunks = n_chunks;
+  m->stats.staged = staged ? 1 : 0;
+  CU(cudaMemcpyAsync(m->labels_pin, m->labels.p, rows * 4 * planes, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  for (size_t j = 0; j < planes; ++j)  // plane j of the device rows -> rows j of the caller's [C][K][n_frames[q]] buffers
+    for (int q = 0; q < U; ++q)
+      if (n_frames[q] > 0)
+        std::memcpy(labels_out[q] + j * n_frames[q], m->labels_pin + j * rows + off[q], (size_t)n_frames[q] * 4);
+  if (speakers_out) CU(cudaMemcpy(speakers_out, sb.out_dev, (size_t)U * 4, cudaMemcpyDeviceToHost));
+  for (int c = 0; c < C; ++c) {  // config c's block of this group -> [c][u0 ..][K] of the whole list's outputs
+    const size_t dst = (size_t)c * U_all + u0, src = (size_t)c * U;
+    if (nb.scores) CU(cudaMemcpy(nb_host.scores + dst * K, nb.scores + src * K, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
+    if (nb.speakers)
+      CU(cudaMemcpy(nb_host.speakers + dst * K, nb.speakers + src * K, (size_t)U * K * 4, cudaMemcpyDeviceToHost));
+    if (nb.count) CU(cudaMemcpy(nb_host.count + dst, nb.count + src, (size_t)U * 4, cudaMemcpyDeviceToHost));
+  }
+  if (int rc = collect(m)) return rc;
+  CU(cudaEventElapsedTime(&m->stats.h2d_ms, m->ev_h2d[0], m->ev_h2d[1]));
+  CU(cudaEventElapsedTime(&m->stats.pipeline_ms, m->ev_pipe, m->ev[1]));  // first cast -> beam kernel start
+  return 0;
+}
+
+// Utterances [u0, u0 + U) of a list of U_all; `nb` holds the whole list's [configs][U_all][k] outputs.
+int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int64_t* off,
+                       const Plan& pl, int32_t* const* labels_out, const uis_debug_taps* taps, cudaStream_t st,
+                       const SpeakerBounds& sb, int32_t* speakers_out, const NBestOut& nb, int u0, int U_all,
+                       const DecodeParams& dp) {
+  const int rc = predict_host_group_impl(m, seqs, n_frames, U, off, pl, labels_out, taps, st, sb, speakers_out, nb, u0,
+                                         U_all, dp);
+  if (rc != 0 && rc != UIS_ERR_OVERFLOW && rc != UIS_ERR_CAPACITY) drain_after_failure(m, st);
+  return rc;
+}
+
 void add_stats(uis_stats* a, const uis_stats& b) {
   a->utterances += b.utterances; a->frames += b.frames; a->beam_steps += b.beam_steps; a->gru_columns += b.gru_columns;
   a->weight_passes += b.weight_passes; a->candidates += b.candidates; a->kernel_launches += b.kernel_launches;
@@ -1548,52 +1390,10 @@ void add_stats(uis_stats* a, const uis_stats& b) {
   a->chunks += b.chunks; a->groups += b.groups; a->staged = std::max(a->staged, b.staged);
 }
 
-}  // namespace
-
-extern "C" {
-
-int uis_predict(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const uis_predict_opts* opts,
-                int32_t* const* labels_out, const uis_debug_taps* taps, void* stream) {
-  return uis_predict_bounded(m, seqs, n_frames, U, opts, labels_out, taps, stream, nullptr, nullptr, nullptr);
-}
-
-int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
-                        const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
-                        const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out) {
-  return predict_host_impl(m, seqs, n_frames, U, opts, labels_out, taps, stream, max_speakers, min_speakers,
-                           speakers_out, NBestOut{});
-}
-
-int uis_predict_nbest(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
-                      const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
-                      const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
-                      const uis_nbest_out* out) {
-  if (!opts || !out) return fail(UIS_ERR_INVALID, "null argument");
-  if (int rc = check_nbest(n_best, opts, out)) return rc;
-  return predict_host_impl(m, seqs, n_frames, U, opts, out->labels_out, taps, stream, max_speakers, min_speakers,
-                           nullptr, NBestOut{n_best, out->scores, out->speakers, out->count});
-}
-
-int uis_predict_sweep(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
-                      const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
-                      const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
-                      const uis_nbest_out* out, const uis_decode_params* params) {
-  if (!m || !opts || !out) return fail(UIS_ERR_INVALID, "null argument");
-  if (int rc = check_nbest(n_best, opts, out)) return rc;
-  DecodeParams dp;
-  if (int rc = check_decode(params, U, &dp)) return rc;
-  return predict_host_impl(m, seqs, n_frames, U, opts, out->labels_out, taps, stream, max_speakers, min_speakers,
-                           nullptr, NBestOut{n_best, out->scores, out->speakers, out->count}, &dp);
-}
-
-}  // extern "C"
-
-namespace {
-
 int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
                       const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
                       const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out,
-                      const NBestOut& nb, const DecodeParams* dpp) {
+                      const NBestOut& nb, const DecodeParams* dpp = nullptr) {
   if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
   if (U < 0 || (U > 0 && (!seqs || !n_frames || !labels_out))) return fail(UIS_ERR_INVALID, "null argument");
   if (int rc = check_bounds(U, max_speakers, min_speakers)) return rc;
@@ -1662,24 +1462,7 @@ int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_
   return 0;
 }
 
-}  // namespace
-
-extern "C" {
-
-int uis_get_stats(uis_model* m, uis_stats* out) {
-  if (!m || !out) return fail(UIS_ERR_INVALID, "null argument");
-  uis::DeviceGuard device_guard_(m->device);
-  CU(device_guard_.status);
-  const int rc = collect(m);
-  *out = m->stats;
-  return rc;
-}
-
-}  // extern "C"
-
-// ---------------------------------------------------------------------------------------------------------------------
-// score(): the neg_likelihood of given labellings (uis_kernels_score.cu)
-namespace {
+// ---- score(): the neg_likelihood of given labellings (uis_kernels_score.cu) ----------------------------------------
 
 // Chains of a score call, one per (utterance, cluster), longest first, with their frame rows in frame order.  The
 // labels must be canonical: 0, 1, 2, ... in order of first appearance (the ids a trace holds).
@@ -1737,9 +1520,10 @@ int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const
   uis::ScoreParams sp{};
   sp.b = model_params(m);
   if (int rc = ensure_log_tables(m, (int)maxN, dp, &sp.b)) return rc;  // block counts and totals reach N
-  const int CP = uis::score_cp(H);
+  if (uis::score_smem(H, D) > uis::kSmemCap) return fail(UIS_ERR_UNSUPPORTED, "no score kernel for hidden=%d dim=%d", H, D);
+  int CP = 0;  // columns per pass: the FFMA beam kernel's
+  uis::with_shape(uis::AllShapes{}, H, D, [&](auto s) { CP = uis::beam_cp<decltype(s)::H>(); });
   const int ctas = (int)std::max(1ll, std::min<long long>(m->num_sms, (cp.queued + CP - 1) / CP));
-  if (uis::score_smem(H, D) > 227u * 1024u) return fail(UIS_ERR_UNSUPPORTED, "no score kernel for hidden=%d dim=%d", H, D);
   if (int rc = m->row_off.ensure((U + 1) * sizeof(long long))) return rc;
   if (int rc = m->queue_stats.ensure(40 * sizeof(unsigned long long))) return rc;
   if (int rc = m->gi.ensure((size_t)rows * 3 * H * sizeof(float))) return rc;
@@ -1783,7 +1567,7 @@ int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const
     if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score chain kernel launch failed: %s", cudaGetErrorString(e));
   }
   CU(cudaEventRecord(m->ev[2], st));
-  if (!uis::launch_score_first(D, sp, st, &e)) return fail(UIS_ERR_UNSUPPORTED, "no score kernel for dim=%d", D);
+  if (!uis::launch_score_first(H, D, sp, st, &e)) return fail(UIS_ERR_UNSUPPORTED, "no score kernel for dim=%d", D);
   if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score first-visit kernel launch failed: %s", cudaGetErrorString(e));
   for (int c = 0; c < dp.count; ++c) {  // the Gaussian terms in sc_mse serve every config
     e = uis::launch_score_reduce(sp, c, st);
@@ -1863,48 +1647,6 @@ int score_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_fr
 }
 
 int score_host(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int32_t* const* labels,
-               float* scores_out, float* const* frame_out, void* stream, const DecodeParams& dp);
-int score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U, const int32_t* labels_dev,
-                 float* scores_dev, float* frame_dev, void* stream, const DecodeParams& dp);
-
-}  // namespace
-
-extern "C" {
-
-int uis_score(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int32_t* const* labels,
-              float* scores_out, float* const* frame_out, void* stream) {
-  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
-  return score_host(m, seqs, n_frames, U, labels, scores_out, frame_out, stream, model_decode(m));
-}
-
-int uis_score_sweep(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int32_t* const* labels,
-                    float* scores_out, float* const* frame_out, void* stream, const uis_decode_params* params) {
-  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
-  DecodeParams dp;
-  if (int rc = check_decode(params, U, &dp)) return rc;
-  return score_host(m, seqs, n_frames, U, labels, scores_out, frame_out, stream, dp);
-}
-
-int uis_score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U, const int32_t* labels_dev,
-                     float* scores_dev, float* frame_dev, void* stream) {
-  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
-  return score_device(m, x_dev, frame_offsets, U, labels_dev, scores_dev, frame_dev, stream, model_decode(m));
-}
-
-int uis_score_device_sweep(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
-                           const int32_t* labels_dev, float* scores_dev, float* frame_dev, void* stream,
-                           const uis_decode_params* params) {
-  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
-  DecodeParams dp;
-  if (int rc = check_decode(params, U, &dp)) return rc;
-  return score_device(m, x_dev, frame_offsets, U, labels_dev, scores_dev, frame_dev, stream, dp);
-}
-
-}  // extern "C"
-
-namespace {
-
-int score_host(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int32_t* const* labels,
                float* scores_out, float* const* frame_out, void* stream, const DecodeParams& dp) {
   if (U < 0 || (U > 0 && (!seqs || !n_frames || !labels || !scores_out))) return fail(UIS_ERR_INVALID, "null argument");
   uis::DeviceGuard device_guard_(m->device);
@@ -1944,3 +1686,234 @@ int score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets,
 }
 
 }  // namespace
+
+extern "C" {
+
+int uis_version(void) { return UIS_ABI_VERSION; }
+const char* uis_last_error(void) { return g_err.c_str(); }
+
+// Any (hidden <= 1024, dim <= 512) runs in the smallest instantiated kernel shape that holds it, zero-padded: a padded
+// hidden unit has zero weights and biases (r = z = 1/2, n = 0, so it stays at its initial 0) and feeds nothing; a
+// padded observation dimension has x = mean = 0 and adds (0 - 0)^2 * w = 0 to every Gaussian term.  Adding exact
+// zeros does not change an fp32 sum, so the results are those of a kernel instantiated for the caller's shape.
+int uis_model_create(uis_model** out, int device, int D, int H, int depth, const float* w_ih, const float* w_hh,
+                     const float* b_ih, const float* b_hh, const float* w1, const float* b1, const float* w2,
+                     const float* b2, const float* h0, const float* sigma2, double transition_bias,
+                     double crp_alpha) {
+  if (!out) return fail(UIS_ERR_INVALID, "out is NULL");
+  *out = nullptr;
+  if (!w_ih || !w_hh || !b_ih || !b_hh || !w1 || !b1 || !w2 || !b2 || !h0 || !sigma2)
+    return fail(UIS_ERR_INVALID, "NULL weight pointer");
+  if (depth < 1 || depth > uis::kMaxDepth)
+    return fail(UIS_ERR_UNSUPPORTED, "rnn_depth=%d: the sm_90a kernels support 1..%d stacked GRU layers", depth, uis::kMaxDepth);
+  if (D < 1 || H < 1) return fail(UIS_ERR_INVALID, "observation_dim and rnn_hidden_size must be >= 1");
+  int Hp = 0, Dp = 0;
+  for (auto& sh : uis::kShapes)
+    if (!Hp && H <= sh[0] && D <= sh[1]) { Hp = sh[0]; Dp = sh[1]; }
+  if (!Hp)
+    return fail(UIS_ERR_UNSUPPORTED, "hidden=%d dim=%d: the sm_90a kernels hold models up to hidden=1024 dim=512", H, D);
+  if (Hp == H && Dp == D)
+    return model_create_impl(out, device, D, H, depth, w_ih, w_hh, b_ih, b_hh, w1, b1, w2, b2, h0, sigma2,
+                             transition_bias, crp_alpha, D, H);
+  uis::DeviceGuard device_guard_(device);
+  CU(device_guard_.status);
+  std::vector<float> v, p_wih((size_t)3 * Hp * Dp + (size_t)(depth - 1) * 3 * Hp * Hp, 0.f), p_whh((size_t)depth * 3 * Hp * Hp, 0.f),
+      p_bih((size_t)depth * 3 * Hp, 0.f), p_bhh((size_t)depth * 3 * Hp, 0.f), p_w1((size_t)Hp * Hp, 0.f), p_b1(Hp, 0.f),
+      p_w2((size_t)Dp * Hp, 0.f), p_b2(Dp, 0.f), p_h0((size_t)depth * Hp, 0.f), p_s2(Dp, 1.f);
+  // gate blocks (r, z, n) keep their own row ranges: row g * H + j -> g * Hp + j
+  if (int r = fetch(v, w_ih, (size_t)3 * H * D + (size_t)(depth - 1) * 3 * H * H)) return r;
+  for (int g = 0; g < 3; ++g)
+    for (int j = 0; j < H; ++j)
+      std::copy(v.begin() + ((size_t)g * H + j) * D, v.begin() + ((size_t)g * H + j + 1) * D,
+                p_wih.begin() + ((size_t)g * Hp + j) * Dp);
+  for (int l = 1; l < depth; ++l)
+    for (int g = 0; g < 3; ++g)
+      for (int j = 0; j < H; ++j) {
+        const float* src = v.data() + (size_t)3 * H * D + (size_t)(l - 1) * 3 * H * H + ((size_t)g * H + j) * H;
+        std::copy(src, src + H, p_wih.begin() + (size_t)3 * Hp * Dp + (size_t)(l - 1) * 3 * Hp * Hp + ((size_t)g * Hp + j) * Hp);
+      }
+  if (int r = fetch(v, w_hh, (size_t)depth * 3 * H * H)) return r;
+  for (int l = 0; l < depth; ++l)
+    for (int g = 0; g < 3; ++g)
+      for (int j = 0; j < H; ++j) {
+        const float* src = v.data() + (size_t)l * 3 * H * H + ((size_t)g * H + j) * H;
+        std::copy(src, src + H, p_whh.begin() + (size_t)l * 3 * Hp * Hp + ((size_t)g * Hp + j) * Hp);
+      }
+  for (int which = 0; which < 2; ++which) {
+    if (int r = fetch(v, which ? b_hh : b_ih, (size_t)depth * 3 * H)) return r;
+    std::vector<float>& dst = which ? p_bhh : p_bih;
+    for (int l = 0; l < depth; ++l)
+      for (int g = 0; g < 3; ++g)
+        std::copy(v.begin() + ((size_t)l * 3 + g) * H, v.begin() + ((size_t)l * 3 + g + 1) * H,
+                  dst.begin() + ((size_t)l * 3 + g) * Hp);
+  }
+  if (int r = fetch(v, w1, (size_t)H * H)) return r;
+  for (int j = 0; j < H; ++j) std::copy(v.begin() + (size_t)j * H, v.begin() + (size_t)(j + 1) * H, p_w1.begin() + (size_t)j * Hp);
+  if (int r = fetch(v, b1, H)) return r;
+  std::copy(v.begin(), v.end(), p_b1.begin());
+  if (int r = fetch(v, w2, (size_t)D * H)) return r;
+  for (int d = 0; d < D; ++d) std::copy(v.begin() + (size_t)d * H, v.begin() + (size_t)(d + 1) * H, p_w2.begin() + (size_t)d * Hp);
+  if (int r = fetch(v, b2, D)) return r;
+  std::copy(v.begin(), v.end(), p_b2.begin());
+  if (int r = fetch(v, h0, (size_t)depth * H)) return r;
+  for (int l = 0; l < depth; ++l) std::copy(v.begin() + (size_t)l * H, v.begin() + (size_t)(l + 1) * H, p_h0.begin() + (size_t)l * Hp);
+  if (int r = fetch(v, sigma2, D)) return r;
+  std::copy(v.begin(), v.end(), p_s2.begin());
+  return model_create_impl(out, device, Dp, Hp, depth, p_wih.data(), p_whh.data(), p_bih.data(), p_bhh.data(), p_w1.data(),
+                           p_b1.data(), p_w2.data(), p_b2.data(), p_h0.data(), p_s2.data(), transition_bias, crp_alpha, D, H);
+}
+
+int uis_model_destroy(uis_model* m) {
+  if (!m) return 0;
+  uis::DeviceGuard device_guard_(m->device);
+  DevBuf* bufs[] = {&m->wih_t, &m->whh_t, &m->w1_t, &m->w2_t, &m->bih, &m->bhh, &m->b1, &m->b2, &m->wvec, &m->mean0,
+                    &m->hidden0, &m->wih_up_t, &m->logn, &m->own_logs.tot, &m->own_logs.cfg, &m->sweep_logs.tot, &m->sweep_logs.cfg, &m->x64, &m->x32, &m->gi, &m->row_off, &m->order,
+                    &m->pool_mean, &m->pool_hidden, &m->bp, &m->queue_stats, &m->labels, &m->status, &m->dbg_win,
+                    &m->dbg_score, &m->dbg_off, &m->dbg_final_scores, &m->dbg_final_k, &m->dbg_best_mean,
+                    &m->dbg_best_hidden, &m->dbg_best_blocks, &m->tc_planes, &m->tc_scratch, &m->pool_mse, &m->stat_bar, &m->stat_scratch,
+                    &m->tree_arena, &m->nb_scores, &m->nb_speakers, &m->nb_count, &m->sc_chain_off,
+                    &m->sc_chain_rows, &m->sc_mse, &m->sc_blocks, &m->sc_out};
+  for (DevBuf* b : bufs) b->release();
+  for (auto& e : m->ev)
+    if (e) cudaEventDestroy(e);
+  for (auto& e : m->ev_copied)
+    if (e) cudaEventDestroy(e);
+  for (auto& e : m->ev_free)
+    if (e) cudaEventDestroy(e);
+  for (auto& e : m->ev_h2d)
+    if (e) cudaEventDestroy(e);
+  if (m->ev_pipe) cudaEventDestroy(m->ev_pipe);
+  if (m->copy_stream) cudaStreamDestroy(m->copy_stream);
+  if (m->labels_pin) cudaFreeHost(m->labels_pin);
+  for (auto& e : m->ev_dma)
+    if (e) cudaEventDestroy(e);
+  if (m->pin_stage) cudaFreeHost(m->pin_stage);
+  delete m->copy_pool;
+  delete m;
+  return 0;
+}
+
+int uis_model_constants(uis_model* m, float* mean0, float* hidden0) {
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  uis::DeviceGuard device_guard_(m->device);
+  CU(device_guard_.status);
+  if (mean0) CU(cudaMemcpy(mean0, m->mean0.p, m->D_user * 4, cudaMemcpyDeviceToHost));
+  if (hidden0)
+    CU(cudaMemcpy2D(hidden0, (size_t)m->H_user * 4, m->hidden0.p, (size_t)m->H * 4, (size_t)m->H_user * 4, m->depth,
+                    cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+size_t uis_predict_workspace_bytes(uis_model* m, const int64_t* frame_offsets, int U, const uis_predict_opts* opts) {
+  Plan pl;
+  if (make_plan(m, frame_offsets, U, opts, &pl)) return 0;
+  return workspace_bytes(m, pl, U);
+}
+
+int uis_predict_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                       const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream) {
+  return uis_predict_device_bounded(m, x_dev, frame_offsets, U, opts, labels_dev, taps, stream, nullptr, nullptr, nullptr);
+}
+
+int uis_predict_device_bounded(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                               const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
+                               const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev) {
+  return predict_device_impl(m, x_dev, frame_offsets, U, opts, labels_dev, taps, stream, max_speakers, min_speakers,
+                             speakers_dev, NBestOut{});
+}
+
+int uis_predict_device_nbest(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                             const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                             const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                             const uis_nbest_out* out) {
+  if (!opts || !out) return fail(UIS_ERR_INVALID, "null argument");
+  if (int rc = check_nbest(n_best, opts, out)) return rc;
+  return predict_device_impl(m, x_dev, frame_offsets, U, opts, out->labels_dev, taps, stream, max_speakers, min_speakers,
+                             nullptr, NBestOut{n_best, out->scores, out->speakers, out->count});
+}
+
+int uis_predict_device_sweep(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                             const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                             const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                             const uis_nbest_out* out, const uis_decode_params* params) {
+  if (!m || !opts || !out) return fail(UIS_ERR_INVALID, "null argument");
+  if (int rc = check_nbest(n_best, opts, out)) return rc;
+  DecodeParams dp;
+  if (int rc = check_decode(params, U, &dp)) return rc;
+  return predict_device_impl(m, x_dev, frame_offsets, U, opts, out->labels_dev, taps, stream, max_speakers, min_speakers,
+                             nullptr, NBestOut{n_best, out->scores, out->speakers, out->count}, &dp);
+}
+
+int uis_predict(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const uis_predict_opts* opts,
+                int32_t* const* labels_out, const uis_debug_taps* taps, void* stream) {
+  return uis_predict_bounded(m, seqs, n_frames, U, opts, labels_out, taps, stream, nullptr, nullptr, nullptr);
+}
+
+int uis_predict_bounded(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                        const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
+                        const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out) {
+  return predict_host_impl(m, seqs, n_frames, U, opts, labels_out, taps, stream, max_speakers, min_speakers,
+                           speakers_out, NBestOut{});
+}
+
+int uis_predict_nbest(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                      const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                      const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                      const uis_nbest_out* out) {
+  if (!opts || !out) return fail(UIS_ERR_INVALID, "null argument");
+  if (int rc = check_nbest(n_best, opts, out)) return rc;
+  return predict_host_impl(m, seqs, n_frames, U, opts, out->labels_out, taps, stream, max_speakers, min_speakers,
+                           nullptr, NBestOut{n_best, out->scores, out->speakers, out->count});
+}
+
+int uis_predict_sweep(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
+                      const uis_predict_opts* opts, const uis_debug_taps* taps, void* stream,
+                      const int32_t* max_speakers, const int32_t* min_speakers, int32_t n_best,
+                      const uis_nbest_out* out, const uis_decode_params* params) {
+  if (!m || !opts || !out) return fail(UIS_ERR_INVALID, "null argument");
+  if (int rc = check_nbest(n_best, opts, out)) return rc;
+  DecodeParams dp;
+  if (int rc = check_decode(params, U, &dp)) return rc;
+  return predict_host_impl(m, seqs, n_frames, U, opts, out->labels_out, taps, stream, max_speakers, min_speakers,
+                           nullptr, NBestOut{n_best, out->scores, out->speakers, out->count}, &dp);
+}
+
+int uis_get_stats(uis_model* m, uis_stats* out) {
+  if (!m || !out) return fail(UIS_ERR_INVALID, "null argument");
+  uis::DeviceGuard device_guard_(m->device);
+  CU(device_guard_.status);
+  const int rc = collect(m);
+  *out = m->stats;
+  return rc;
+}
+
+int uis_score(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int32_t* const* labels,
+              float* scores_out, float* const* frame_out, void* stream) {
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  return score_host(m, seqs, n_frames, U, labels, scores_out, frame_out, stream, model_decode(m));
+}
+
+int uis_score_sweep(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U, const int32_t* const* labels,
+                    float* scores_out, float* const* frame_out, void* stream, const uis_decode_params* params) {
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  DecodeParams dp;
+  if (int rc = check_decode(params, U, &dp)) return rc;
+  return score_host(m, seqs, n_frames, U, labels, scores_out, frame_out, stream, dp);
+}
+
+int uis_score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U, const int32_t* labels_dev,
+                     float* scores_dev, float* frame_dev, void* stream) {
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  return score_device(m, x_dev, frame_offsets, U, labels_dev, scores_dev, frame_dev, stream, model_decode(m));
+}
+
+int uis_score_device_sweep(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                           const int32_t* labels_dev, float* scores_dev, float* frame_dev, void* stream,
+                           const uis_decode_params* params) {
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  DecodeParams dp;
+  if (int rc = check_decode(params, U, &dp)) return rc;
+  return score_device(m, x_dev, frame_offsets, U, labels_dev, scores_dev, frame_dev, stream, dp);
+}
+
+}  // extern "C"

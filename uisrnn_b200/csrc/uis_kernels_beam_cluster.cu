@@ -1,29 +1,18 @@
-// Cluster (latency) mode of the beam kernel: default model shape only, depth 1.
+// Cluster (latency) mode of the beam kernel: depth 1.
 #include "uis_launch.cuh"
 namespace uis {
 bool launch_beam_cluster(int H, int D, const BeamParams& p, int ctas, int cluster, unsigned smem, cudaStream_t st,
                          cudaError_t* err) {
-  if (!(H == 512 && D == 256) || p.depth != 1) return false;
-  auto kern = uis_beam_kernel<512, 256, false, true>;
-  *err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (*err != cudaSuccess) return true;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)ctas);
-  cfg.blockDim = dim3(Cfg<512, 256, kCPCluster>::BLOCK);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr{};
-  attr.id = cudaLaunchAttributeClusterDimension;
-  attr.val.clusterDim.x = (unsigned)cluster;
-  attr.val.clusterDim.y = 1;
-  attr.val.clusterDim.z = 1;
-  cfg.attrs = &attr;
-  cfg.numAttrs = 1;
-  *err = cudaLaunchKernelEx(&cfg, kern, p);
-  return true;
-}
-unsigned beam_cluster_smem(int H, int D, int B, int Kcap) {
-  if (H == 512 && D == 256) return make_layout<512, 256, kCPCluster, true>(B, Kcap, 1).total;
-  return 0xffffffffu;
+  if (p.depth != 1) return false;
+  return with_shape(LatencyShapes{}, H, D, [&](auto s) {
+    using S = decltype(s);
+    cudaLaunchAttribute attr{};
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = (unsigned)cluster;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    *err = launch_with_attr(uis_beam_kernel<S::H, S::D, false, 1>, p, ctas, Cfg<S::H, S::D, kCPCluster>::BLOCK, smem, st,
+                            attr);
+  });
 }
 }  // namespace uis

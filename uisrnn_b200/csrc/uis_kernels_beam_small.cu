@@ -1,16 +1,10 @@
 #include "uis_launch.cuh"
 namespace uis {
 bool launch_beam_small(int H, int D, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st, cudaError_t* err) {
-  if (H == 256 && D == 128) {
-    *err = p.depth > 1 ? launch_with_smem(uis_beam_kernel<256, 128, true>, p, ctas, Cfg<256, 128>::BLOCK, smem, st)
-                       : launch_with_smem(uis_beam_kernel<256, 128, false>, p, ctas, Cfg<256, 128>::BLOCK, smem, st);
-    return true;
-  }
-  if (H == 128 && D == 64) {
-    *err = p.depth > 1 ? launch_with_smem(uis_beam_kernel<128, 64, true>, p, ctas, Cfg<128, 64>::BLOCK, smem, st)
-                       : launch_with_smem(uis_beam_kernel<128, 64, false>, p, ctas, Cfg<128, 64>::BLOCK, smem, st);
-    return true;
-  }
-  return false;
+  return with_shape(SmallShapes{}, H, D, [&](auto s) {
+    using S = decltype(s);
+    *err = p.depth > 1 ? launch_with_smem(uis_beam_kernel<S::H, S::D, true>, p, ctas, Cfg<S::H, S::D>::BLOCK, smem, st)
+                       : launch_with_smem(uis_beam_kernel<S::H, S::D, false>, p, ctas, Cfg<S::H, S::D>::BLOCK, smem, st);
+  });
 }
 }  // namespace uis

@@ -1,26 +1,15 @@
-// Stationary-weights (latency) mode of the beam kernel (uis_beam_stat.cuh): default model shape only, depth 1.
+// Stationary-weights (latency) mode of the beam kernel (uis_beam_stat.cuh): depth 1.
 #include "uis_launch.cuh"
 namespace uis {
 bool launch_beam_stat(int H, int D, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st, cudaError_t* err) {
-  if (!(H == 512 && D == 256) || p.depth != 1) return false;
-  auto kern = uis_beam_kernel<512, 256, false, 2>;
-  *err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (*err != cudaSuccess) return true;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)ctas);
-  cfg.blockDim = dim3(Cfg<512, 256, kCPCluster>::BLOCK);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr{};
-  attr.id = cudaLaunchAttributeCooperative;  // the groups synchronise through global memory: all CTAs must be co-resident
-  attr.val.cooperative = 1;
-  cfg.attrs = &attr;
-  cfg.numAttrs = 1;
-  *err = cudaLaunchKernelEx(&cfg, kern, p);
-  return true;
-}
-unsigned beam_stat_smem(int H, int D, int B, int Kcap) {
-  if (H == 512 && D == 256) return make_layout<512, 256, kCPCluster, false, 0, true>(B, Kcap, 1).total;
-  return 0xffffffffu;
+  if (p.depth != 1) return false;
+  return with_shape(LatencyShapes{}, H, D, [&](auto s) {
+    using S = decltype(s);
+    cudaLaunchAttribute attr{};
+    attr.id = cudaLaunchAttributeCooperative;  // the groups synchronise through global memory: all CTAs must be co-resident
+    attr.val.cooperative = 1;
+    *err = launch_with_attr(uis_beam_kernel<S::H, S::D, false, 2>, p, ctas, Cfg<S::H, S::D, kCPCluster>::BLOCK, smem, st,
+                            attr);
+  });
 }
 }  // namespace uis

@@ -238,41 +238,25 @@ __global__ void __launch_bounds__(128) score_reduce_kernel(const __grid_constant
 }
 
 unsigned score_smem(int H, int D) {
-  if (H == 128 && D == 64) return ScoreLayout<128, 64>::total;
-  if (H == 256 && D == 128) return ScoreLayout<256, 128>::total;
-  if (H == 512 && D == 256) return ScoreLayout<512, 256>::total;
-  if (H == 1024 && D == 512) return ScoreLayout<1024, 512>::total;
-  return 0xffffffffu;
-}
-
-template <int H, int D>
-static cudaError_t launch_chains(const ScoreParams& sp, int ctas, cudaStream_t st) {
-  auto kern = sp.b.depth > 1 ? uis_score_kernel<H, D, true> : uis_score_kernel<H, D, false>;
-  const unsigned smem = ScoreLayout<H, D>::total;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  kern<<<ctas, Cfg<H, D>::BLOCK, smem, st>>>(sp);
-  return cudaGetLastError();
+  unsigned smem = kNoKernel;
+  with_shape(AllShapes{}, H, D, [&](auto s) { smem = ScoreLayout<decltype(s)::H, decltype(s)::D>::total; });
+  return smem;
 }
 
 bool launch_score_chains(int H, int D, const ScoreParams& sp, int ctas, cudaStream_t st, cudaError_t* err) {
-  if (H == 128 && D == 64) *err = launch_chains<128, 64>(sp, ctas, st);
-  else if (H == 256 && D == 128) *err = launch_chains<256, 128>(sp, ctas, st);
-  else if (H == 512 && D == 256) *err = launch_chains<512, 256>(sp, ctas, st);
-  else if (H == 1024 && D == 512) *err = launch_chains<1024, 512>(sp, ctas, st);
-  else return false;
-  return true;
+  return with_shape(AllShapes{}, H, D, [&](auto s) {
+    using S = decltype(s);
+    auto kern = sp.b.depth > 1 ? uis_score_kernel<S::H, S::D, true> : uis_score_kernel<S::H, S::D, false>;
+    *err = launch_with_smem(kern, sp, ctas, Cfg<S::H, S::D>::BLOCK, ScoreLayout<S::H, S::D>::total, st);
+  });
 }
 
-bool launch_score_first(int D, const ScoreParams& sp, cudaStream_t st, cudaError_t* err) {
+bool launch_score_first(int H, int D, const ScoreParams& sp, cudaStream_t st, cudaError_t* err) {
   const unsigned blocks = (unsigned)(((long long)sp.chains * 32 + 255) / 256);
-  if (D == 64) score_first_kernel<64><<<blocks, 256, 0, st>>>(sp);
-  else if (D == 128) score_first_kernel<128><<<blocks, 256, 0, st>>>(sp);
-  else if (D == 256) score_first_kernel<256><<<blocks, 256, 0, st>>>(sp);
-  else if (D == 512) score_first_kernel<512><<<blocks, 256, 0, st>>>(sp);
-  else return false;
-  *err = cudaGetLastError();
-  return true;
+  return with_shape(AllShapes{}, H, D, [&](auto s) {
+    score_first_kernel<decltype(s)::D><<<blocks, 256, 0, st>>>(sp);
+    *err = cudaGetLastError();
+  });
 }
 
 cudaError_t launch_score_reduce(const ScoreParams& sp, int cfg, cudaStream_t st) {
