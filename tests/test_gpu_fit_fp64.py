@@ -13,11 +13,11 @@ the unmodified kernels show over this whole file on an H100 (the measured figure
 
 The cases reach every host-side path choice of the trainer: the persistent cooperative recurrence at 32, 64, 96 and
 128 CTAs and the per-step launches (H not a multiple of 128, H = 1024 whose backward kernel outgrows shared
-memory, UISRNN_B200_TRAIN_STEPWISE=1); 64x64 and 128x128 GEMM tiles with and without split-K
-(UISRNN_B200_TRAIN_GEMM=64 forces the small tiles); the sliced column sum of the d h_{-1} carry (B >= 256); both grid
-barriers (UISRNN_B200_TRAIN_BARRIER=spin); rnn_depth 1..4 with and without inter-layer dropout.  The optimiser tests
-feed the trainer's own parameters and unclipped gradients of every step to the oracle's clip + Adam + clamp, so that
-they see the optimiser's arithmetic alone."""
+memory, UISRNN_B200_TRAIN_STEPWISE=1); 64x64 and 128x128 GEMM tiles, each of their three operand layouts with and
+without split-K (the small tiles serve products with M < 128 or N < 128: D = 2, 40, 64 and 65, H = 8 and 100, and
+the one-column 'min' batches); the sliced column sum of the d h_{-1} carry (B >= 256); rnn_depth 1..4 with and without
+inter-layer dropout.  The optimiser tests feed the trainer's own parameters and unclipped gradients of every step to
+the oracle's clip + Adam + clamp, so that they see the optimiser's arithmetic alone."""
 import numpy as np
 import pytest
 
@@ -88,7 +88,7 @@ _ORACLE = {}
 
 
 def oracle(shape, layout):
-  """Float64 losses and gradients of a case (cached: the switch tests rerun cases)."""
+  """Float64 losses and gradients of a case (cached: the STEPWISE tests rerun cases)."""
   key = (shape, layout)
   if key not in _ORACLE:
     params, x, lengths = case_inputs(shape, layout)
@@ -170,23 +170,14 @@ def test_losses_and_gradients_match_fp64(case):
   run_case(*case)
 
 
-SWITCH_CASES = [
-    ('UISRNN_B200_TRAIN_STEPWISE', '1', ((256, 512, 2), 'b33')),
-    ('UISRNN_B200_TRAIN_STEPWISE', '1', ((64, 128, 1), 'b64')),
-    ('UISRNN_B200_TRAIN_STEPWISE', '1', ((256, 384, 1), 'extreme')),
-    ('UISRNN_B200_TRAIN_GEMM', '64', ((256, 512, 2), 'b33')),
-    ('UISRNN_B200_TRAIN_GEMM', '64', ((512, 1024, 1), 'b33')),
-    ('UISRNN_B200_TRAIN_GEMM', '64', ((256, 512, 2), 'b300')),
-    ('UISRNN_B200_TRAIN_BARRIER', 'spin', ((256, 512, 2), 'b33')),
-    ('UISRNN_B200_TRAIN_BARRIER', 'spin', ((256, 384, 1), 'b64')),
-]
+STEPWISE_CASES = [((256, 512, 2), 'b33'), ((64, 128, 1), 'b64'), ((256, 384, 1), 'extreme')]
 
 
-@pytest.mark.parametrize('var,value,case', SWITCH_CASES,
-                         ids=['{}={}-{}'.format(v.rsplit('_', 1)[1], x, _id(c)) for v, x, c in SWITCH_CASES])
-def test_switches_match_fp64(monkeypatch, var, value, case):
-  """The documented A/B switches, read when the trainer is created / first steps: same oracle, same bounds."""
-  monkeypatch.setenv(var, value)
+@pytest.mark.parametrize('case', STEPWISE_CASES, ids=['STEPWISE=1-' + _id(c) for c in STEPWISE_CASES])
+def test_switches_match_fp64(monkeypatch, case):
+  """UISRNN_B200_TRAIN_STEPWISE=1 (read when the trainer first steps) forces the per-step recurrence launches on
+  shapes whose persistent kernels would run: same oracle, same bounds."""
+  monkeypatch.setenv('UISRNN_B200_TRAIN_STEPWISE', '1')
   run_case(*case)
 
 

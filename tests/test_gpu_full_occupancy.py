@@ -13,9 +13,9 @@ a. Traced utterances inside such calls, checked per beam step by beam_replay.che
    groups: decode-in-groups is covered by (b) and (c).)
 b. Every utterance and every rank (n_best = beam_size) bit-identical across call composition, per engine: the list
    permuted, 61 and 7 CTAs, 4 and 1 lanes, 256-row staging chunks, pageable inputs staged by the driver instead of the
-   pinned ring, decode in groups, 32-column tensor-core passes, and predict_device_nbest on a non-default stream (what
-   bench.py times); plane 0 equals the call without n_best.  A column's arithmetic does not depend on the lane, pass
-   position or CTA it lands in, nor the input projection on a row's position in its tile.  Engines and the
+   pinned ring, decode in groups, and predict_device_nbest on a non-default stream (what bench.py times); plane 0
+   equals the call without n_best.  A column's arithmetic does not depend on the lane, pass position or CTA it lands
+   in, nor the input projection on a row's position in its tile.  Engines and the
    cluster / stationary-weights modes are not compared with each other: they split k differently.  That includes a
    group of a decode-in-groups call: each group is planned on its own, and a group of no more utterances than SMs
    runs a latency-mode kernel under the automatic plan (a split of the rows in thirds left the last 3 utterances to
@@ -118,8 +118,8 @@ def traced_calls(native, xs, kw, expect, trace, max_speakers=None, min_speakers=
   return plain
 
 
-def tc_plan(sms, U=U_FULL, lanes=6, columns=48):
-  return dict(engine=2, lanes=lanes, tc_columns=columns, cluster=1, ctas=sms, utterances=U)
+def tc_plan(sms, U=U_FULL, lanes=6):
+  return dict(engine=2, lanes=lanes, tc_columns=48, cluster=1, ctas=sms, utterances=U)
 
 
 def ffma_plan(sms, lanes, U=U_FULL, ctas=None):
@@ -293,11 +293,6 @@ def test_call_composition_bit_identical(native, monkeypatch, batch, sms, variant
   same(ref, run(), 'decode in groups')
   assert nm.stats()['groups'] == 3
   monkeypatch.delenv('UISRNN_B200_MAX_ROWS')
-  if variant == 'tc':
-    monkeypatch.setenv('UISRNN_B200_TC_N', '32')
-    same(ref, run(), '32-column tensor-core passes')
-    check_stats(nm, tc_plan(sms, lanes=3, columns=32), '32-column passes')
-    monkeypatch.delenv('UISRNN_B200_TC_N')
   # the device entry point on a non-default stream
   same(ref, device_nbest(nm, xs, k, kw), 'predict_device_nbest')
   check_stats(nm, plan, 'predict_device_nbest')

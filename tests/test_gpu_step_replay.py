@@ -125,13 +125,12 @@ def test_ffma_one_and_two_lanes(native):
          dict(engine=1, lanes=2, tc_columns=0, cluster=1, ctas=1))
 
 
-@pytest.mark.parametrize('tc_n,lanes', [('48', 6), ('32', 3)])
-def test_tensor_cores_several_lanes(native, monkeypatch, tc_n, lanes):
-  """48-column passes with 6 lanes per CTA; 32-column passes with 3, the most their shared memory holds."""
-  xs = toy_batch(lanes, 200 + int(tc_n))
+@pytest.mark.parametrize('lanes', [6, 3])
+def test_tensor_cores_several_lanes(native, lanes):
+  """48-column passes shared by 6 lanes per CTA, the most one pass serves, and by 3."""
+  xs = toy_batch(lanes, 248)
   traced(native, TOY, xs, dict(engine=2, lanes=lanes, n_ctas=1),
-         dict(engine=2, lanes=lanes, tc_columns=int(tc_n), cluster=1, ctas=1),
-         monkeypatch=monkeypatch, env={'UISRNN_B200_TC_N': tc_n})
+         dict(engine=2, lanes=lanes, tc_columns=48, cluster=1, ctas=1))
 
 
 def test_tensor_cores_beam_64_two_passes(native):

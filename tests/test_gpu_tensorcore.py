@@ -37,7 +37,7 @@ def test_toy_testing_data_labels_identical_to_reference(toy_model):
   xs, labs = toy_utterances()
   got = toy_model.predict(xs, engine=2)
   st = toy_model.stats()
-  assert st['engine'] == 2 and st['tc_columns'] in (32, 48) and st['cluster'] == 1
+  assert st['engine'] == 2 and st['tc_columns'] == 48 and st['cluster'] == 1
   for i, (g, want) in enumerate(zip(got, labs)):
     assert g.tolist() == want.tolist(), 'utterance %d' % i
   assert st['frames'] == sum(len(x) for x in xs) and st['beam_steps'] == 2 * st['frames']
@@ -56,18 +56,17 @@ def test_toy_trace_matches_reference(toy_model, idx):
   assert np.max(np.abs(dbg['best_mean'] - g['u%d_final_mean' % idx])) < STATE_ATOL
 
 
-@pytest.mark.parametrize('lanes,n_ctas,columns', [(0, 0, 48), (6, 2, 48), (2, 0, 48), (8, 1, 48), (4, 3, 32), (1, 0, 32)])
-def test_default_shape_500_frames_reference_labels(toy_model, monkeypatch, lanes, n_ctas, columns):
+@pytest.mark.parametrize('lanes,n_ctas', [(0, 0), (6, 2), (2, 0), (8, 1), (4, 3), (1, 0)])
+def test_default_shape_500_frames_reference_labels(toy_model, lanes, n_ctas):
   """(512, 256), 1000 beam steps per utterance, lanes sharing one pass (incl. more columns than one pass holds)."""
   from uisrnn_b200.synth import synth_utt
-  monkeypatch.setenv('UISRNN_B200_TC_N', str(columns))
   _, xs, want = _bench_golden()
   g2 = np.load(GOLDEN + '/synth500.npz')
   xs = xs + [synth_utt(int(s))[0] for s in g2['seeds']]
   want = want + [lab.tolist() for lab in g2['labels']]
   got = toy_model.predict(xs, engine=2, lanes=lanes, n_ctas=n_ctas)
   st = toy_model.stats()
-  assert st['engine'] == 2 and st['tc_columns'] == columns
+  assert st['engine'] == 2 and st['tc_columns'] == 48
   if lanes:
     assert st['lanes'] <= lanes
   for i, (g, w) in enumerate(zip(got, want)):

@@ -1,6 +1,5 @@
 """A/B of the beam-kernel engines on bench.py's workload (device-resident): frames/s, kernel ms, phase shares.
-  python tools/tc_bench.py [U ...]      e.g.  python tools/tc_bench.py 264 792
-Environment: UISRNN_B200_TC_N=32|48 selects the columns per tensor-core pass."""
+  python tools/tc_bench.py [U ...]      e.g.  python tools/tc_bench.py 264 792"""
 import json
 import os
 import sys

@@ -220,8 +220,8 @@ namespace {
 // ---- the kernel variants (uis::Kernel, uis_launch.cuh): shared memory and launch ----------------------------------
 
 // Shared memory of kernel k at the model's shape for the sizes in p (B, Kcap, G; the tree kernels: L, node_cap,
-// leaf_cap, P); tcn = columns per tensor-core pass.  uis::kNoKernel if the shape has no such kernel.
-unsigned kernel_smem(const uis_model* m, uis::Kernel k, const uis::BeamParams& p, int tcn = 0) {
+// leaf_cap, P).  uis::kNoKernel if the shape has no such kernel.
+unsigned kernel_smem(const uis_model* m, uis::Kernel k, const uis::BeamParams& p) {
   using namespace uis;
   unsigned smem = kNoKernel;
   switch (k) {
@@ -245,10 +245,8 @@ unsigned kernel_smem(const uis_model* m, uis::Kernel k, const uis::BeamParams& p
       break;
     case Kernel::TensorCore:
       with_shape(TcShapes{}, m->H, m->D, [&](auto s) {
-        with_tc_columns(tcn, [&](auto n) {
-          using S = decltype(s);
-          smem = make_layout<S::H, S::D, kCPBeam, false, decltype(n)::value>(p.B, p.Kcap, p.G).total;
-        });
+        using S = decltype(s);
+        smem = make_layout<S::H, S::D, kCPBeam, false, kTcColumns>(p.B, p.Kcap, p.G).total;
       });
       break;
     case Kernel::Tree:
@@ -273,17 +271,17 @@ uis::BeamParams beam_sizes(int B, int Kcap, int G) {
   return p;
 }
 
-// Launches kernel k at the model's shape on `ctas` CTAs (Kernel::Cluster: `cluster` CTAs per cluster;
-// Kernel::TensorCore: `tcn` columns per pass).  false if the shape has no such kernel; *err = the launch status otherwise.
-bool launch_kernel(const uis_model* m, uis::Kernel k, const uis::BeamParams& p, int ctas, int cluster, int tcn,
-                   unsigned smem, cudaStream_t st, cudaError_t* err) {
+// Launches kernel k at the model's shape on `ctas` CTAs (Kernel::Cluster: `cluster` CTAs per cluster).  false if the
+// shape has no such kernel; *err = the launch status otherwise.
+bool launch_kernel(const uis_model* m, uis::Kernel k, const uis::BeamParams& p, int ctas, int cluster, unsigned smem,
+                   cudaStream_t st, cudaError_t* err) {
   const int H = m->H, D = m->D;
   switch (k) {
     case uis::Kernel::Beam:
       return uis::launch_beam_large(H, D, p, ctas, smem, st, err) || uis::launch_beam_small(H, D, p, ctas, smem, st, err);
     case uis::Kernel::Cluster: return uis::launch_beam_cluster(H, D, p, ctas, cluster, smem, st, err);
     case uis::Kernel::Stat: return uis::launch_beam_stat(H, D, p, ctas, smem, st, err);
-    case uis::Kernel::TensorCore: return uis::launch_beam_tc(H, D, tcn, p, ctas, smem, st, err);
+    case uis::Kernel::TensorCore: return uis::launch_beam_tc(H, D, p, ctas, smem, st, err);
     case uis::Kernel::Tree:
     case uis::Kernel::TreeSpill: {
       const bool spill = k == uis::Kernel::TreeSpill;
@@ -343,7 +341,7 @@ int tc_prepare(uis_model* m, const std::vector<float>& w_hh, const std::vector<f
                const std::vector<float>& w2, const std::vector<float>& hidden0) {
   const int H = m->H, D = m->D;
   m->tc_ready = false;
-  if (m->depth != 1 || kernel_smem(m, uis::Kernel::TensorCore, uis::BeamParams{}, 48) == uis::kNoKernel) return 0;
+  if (m->depth != 1 || kernel_smem(m, uis::Kernel::TensorCore, uis::BeamParams{}) == uis::kNoKernel) return 0;
   auto maxabs = [](const std::vector<float>& v) { double a = 0; for (float x : v) a = std::max(a, (double)std::fabs(x)); return a; };
   // |h'| <= max(1, |h|) by induction (h' is a convex combination of h and tanh(.)), starting from hidden0
   const double hmax = std::max(1.0, maxabs(hidden0));
@@ -523,7 +521,6 @@ struct Plan {
   uis::Kernel kernel = uis::Kernel::Beam;
   bool forced = false;  // the caller asked for this latency mode: a refused launch is an error, not a fallback
   int cluster = 1;      // Kernel::Cluster: CTAs per utterance (thread-block cluster size)
-  int tcn = 0;          // Kernel::TensorCore: columns per pass (uis_beam_tc.cuh)
   int node_cap = 0, leaf_cap = 0, maxTN = 0, maxSteps = 0;  // look_ahead >= 2 only
   // look_ahead >= 2: the spill kernel that decodes, from a device-memory arena, what outgrew shared memory.  It runs
   // after Kernel::Tree, or instead of it as Kernel::TreeSpill (UISRNN_B200_TREE_SPILL=force); spill_ctas = 0: off.
@@ -639,24 +636,21 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
     pl->kernel = uis::Kernel::Tree;
   } else {
     // Tensor-core engine (look_ahead 1, depth 1, 128-row-tileable shapes): the cost of a weight pass does not depend on
-    // the number of columns, so a CTA advances up to N / 8 utterances together (a lane needs ~6 columns per step,
+    // the number of columns, so a CTA advances up to kTcColumns / 8 utterances together (a lane needs ~6 columns per step,
     // at most beam_size + 1).  Chosen automatically when some CTA gets more than one utterance; below that the
     // one-lane FFMA kernel or the cluster (latency) mode is faster.  Its device tables default to 16 clusters per
     // hypothesis (UIS_ERR_OVERFLOW asks the caller for more, as always).
     if (o->engine != 1 && m->tc_ready && o->cluster <= 0) {
-      int N = 48;
-      if (const char* env = std::getenv("UISRNN_B200_TC_N")) N = std::atoi(env);
       const int kc = o->kcap > 0 ? o->kcap : 16;
-      auto tc_smem = [&](int g) { return kernel_smem(m, uis::Kernel::TensorCore, beam_sizes(pl->B, kc, g), N); };
+      auto tc_smem = [&](int g) { return kernel_smem(m, uis::Kernel::TensorCore, beam_sizes(pl->B, kc, g)); };
       if (tc_smem(1) != uis::kNoKernel) {
         int Gt = o->lanes > 0 ? std::min(o->lanes, (int)uis::kMaxLanes)
-                              : (int)std::min<long long>(N / 8, (J + ctas - 1) / std::max(ctas, 1));
+                              : (int)std::min<long long>(uis::kTcColumns / 8, (J + ctas - 1) / std::max(ctas, 1));
         Gt = std::max(Gt, 1);
         while (Gt > 1 && (tc_smem(Gt) > uis::kSmemCap || Gt * pl->B > 256)) --Gt;
         const bool fits = tc_smem(Gt) <= uis::kSmemCap && pl->B * kc + pl->B + 1 <= 65535;
         if (fits && (o->engine == 2 || J > ctas)) {
           pl->kernel = uis::Kernel::TensorCore;
-          pl->tcn = N;
           pl->Kcap = kc;
           pl->P = pl->B * kc + pl->B + 1;
           G = Gt;
@@ -664,13 +658,13 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
           return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: beam_size=%d kcap=%d does not fit in shared memory", pl->B, kc);
         }
       } else if (o->engine == 2) {
-        return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: no kernel for hidden=%d dim=%d columns=%d", m->H, m->D, N);
+        return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine: no kernel for hidden=%d dim=%d", m->H, m->D);
       }
     } else if (o->engine == 2) {
       return fail(UIS_ERR_UNSUPPORTED, "tensor-core engine needs look_ahead 1, depth 1, hidden/dim multiples of 128, no "
                                        "cluster mode and weights its fp16 split holds (uis_model_create)");
     }
-    if (!pl->tcn)
+    if (pl->kernel != uis::Kernel::TensorCore)
       while (G > 1 && kernel_smem(m, uis::Kernel::Beam, beam_sizes(pl->B, pl->Kcap, G)) > uis::kSmemCap) --G;
     while (G > 1 && G * pl->B > 256) --G;  // at most 256 (lane, winner) pairs per CTA step
   }
@@ -680,16 +674,12 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
   if (tree) plan_tree_spill(m, pl);
   // Cluster (latency) mode: with fewer utterances than SMs, a thread-block cluster of 2/4/8 CTAs works on
   // each utterance (k-split of every weight matrix, uis_beam.cuh).  opts->cluster: 0 = auto (largest of 4, 2
-  // that still gives every utterance its own cluster), -1 = off, 2/4/8 = forced; UISRNN_B200_CLUSTER=0 disables
-  // the automatic choice.
+  // that still gives every utterance its own cluster), -1 = off, 2/4/8 = forced.
   // Stationary-weights mode (uis_beam_stat.cuh): 32 CTAs per utterance keep the weights in shared memory.  The fastest
-  // way to decode up to #SMs / 32 utterances at a time; opts->cluster = 32 forces it, 0 picks it automatically,
-  // UISRNN_B200_STAT=0 disables the automatic choice.
+  // way to decode up to #SMs / 32 utterances at a time; opts->cluster = 32 forces it, 0 picks it automatically.
   if (!tree && U >= 1 && (o->cluster == 0 || o->cluster == uis::kStatGroup) && m->depth == 1 &&
       o->lanes <= 1 && o->engine != 2) {
-    const char* env = std::getenv("UISRNN_B200_STAT");
-    const bool want = o->cluster == uis::kStatGroup ||
-                      (!(env && env[0] == '0') && J * uis::kStatGroup <= ctas && o->engine == 0 && o->n_ctas <= 0);
+    const bool want = o->cluster == uis::kStatGroup || (J * uis::kStatGroup <= ctas && o->engine == 0 && o->n_ctas <= 0);
     const int kc = o->kcap > 0 ? o->kcap : 32;
     const bool can = ctas >= uis::kStatGroup && kernel_smem(m, uis::Kernel::Stat, beam_sizes(pl->B, kc, 1)) <= uis::kSmemCap &&
                      pl->B * kc + pl->B + 1 <= 65535;
@@ -697,7 +687,6 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
       const int groups = (int)std::max(1ll, std::min<long long>(ctas / uis::kStatGroup, J));
       pl->kernel = uis::Kernel::Stat;
       pl->forced = o->cluster == uis::kStatGroup;
-      pl->tcn = 0;
       pl->Kcap = kc;
       pl->P = pl->B * kc + pl->B + 1;
       pl->G = 1;
@@ -712,10 +701,8 @@ int make_plan(uis_model* m, const int64_t* off, int U, const uis_predict_opts* o
     if (o->cluster == 2 || o->cluster == 4 || o->cluster == 8) {
       cs = o->cluster;
     } else if (o->cluster == 0) {
-      const char* env = std::getenv("UISRNN_B200_CLUSTER");
-      if (!(env && env[0] == '0'))
-        for (int c : {4, 2})
-          if (J * c <= ctas) { cs = c; break; }
+      for (int c : {4, 2})
+        if (J * c <= ctas) { cs = c; break; }
     } else {
       return fail(UIS_ERR_INVALID, "cluster must be -1, 0, 2, 4, 8 or 32");
     }
@@ -742,7 +729,8 @@ size_t workspace_bytes(const uis_model* m, const Plan& pl, int U, int configs = 
   b += (size_t)pl.ctas * pl.G * (pl.L > 1 ? (size_t)pl.maxTN + pl.maxSteps : (size_t)pl.maxN) * pl.B * 4;  // back-pointers
   b += (size_t)(U + 1) * 8 + J * 8 + 256;                               // offsets, order, status
   if (configs > 1) b += (size_t)configs * (4096 + 3) * 8;               // log tables of the sweep (at least)
-  if (pl.tcn) b += (size_t)pl.ctas * pl.tcn * m->H * 4;                 // a = relu(W1 h' + b1) between two products
+  if (pl.kernel == uis::Kernel::TensorCore)                             // a = relu(W1 h' + b1) between two products
+    b += (size_t)pl.ctas * uis::kTcColumns * m->H * 4;
   return b;
 }
 
@@ -799,7 +787,7 @@ const struct { const char *missing, *name; } kKernelNames[] = {
 // CTAs) gives way to the FFMA kernel on the same grid: its extra CTAs find the utterance queue empty.
 int launch(uis_model* m, const Plan& pl, uis::Kernel k, const uis::BeamParams& p, int ctas, cudaStream_t st) {
   using uis::Kernel;
-  const unsigned smem = kernel_smem(m, k, p, pl.tcn);
+  const unsigned smem = kernel_smem(m, k, p);
   if (smem > uis::kSmemCap) {
     if (k == Kernel::Tree || k == Kernel::TreeSpill)
       return fail(UIS_ERR_UNSUPPORTED, "look_ahead=%d beam_size=%d kcap=%d needs %u B of shared memory (> 227 KB)", p.L,
@@ -808,7 +796,7 @@ int launch(uis_model* m, const Plan& pl, uis::Kernel k, const uis::BeamParams& p
                 p.B, p.Kcap, p.G, smem);
   }
   cudaError_t e = cudaSuccess;
-  const bool have = launch_kernel(m, k, p, ctas, pl.cluster, pl.tcn, smem, st, &e);
+  const bool have = launch_kernel(m, k, p, ctas, pl.cluster, smem, st, &e);
   if (have && e == cudaSuccess) {
     m->stats.cluster = k == Kernel::Stat ? uis::kStatGroup : k == Kernel::Cluster ? pl.cluster : 1;
     return 0;
@@ -817,8 +805,6 @@ int launch(uis_model* m, const Plan& pl, uis::Kernel k, const uis::BeamParams& p
     (void)cudaGetLastError();  // clear the launch error and fall back
     return launch(m, pl, Kernel::Beam, p, ctas, st);
   }
-  if (!have && k == Kernel::TensorCore)
-    return fail(UIS_ERR_UNSUPPORTED, "no tensor-core kernel for hidden=%d dim=%d columns=%d", m->H, m->D, pl.tcn);
   if (!have)
     return fail(UIS_ERR_UNSUPPORTED, "no %s for hidden=%d dim=%d", kKernelNames[(int)k].missing, m->H, m->D);
   return fail(UIS_ERR_CUDA, "%s launch failed: %s", kKernelNames[(int)k].name, cudaGetErrorString(e));
@@ -947,8 +933,9 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
                             sizeof(unsigned)))
     return rc;
 
-  if (pl.tcn)
-    if (int rc = m->tc_scratch.ensure((size_t)pl.ctas * pl.tcn * H * sizeof(float))) return rc;
+  const bool tc = pl.kernel == uis::Kernel::TensorCore;
+  if (tc)
+    if (int rc = m->tc_scratch.ensure((size_t)pl.ctas * uis::kTcColumns * H * sizeof(float))) return rc;
   if (pl.kernel == uis::Kernel::Stat) {  // pl.ctas / kStatGroup groups
     if (int rc = m->stat_bar.ensure((size_t)pl.ctas * sizeof(unsigned))) return rc;
     if (int rc = m->stat_scratch.ensure((size_t)(pl.ctas / uis::kStatGroup) * uis::kCPCluster * H * sizeof(float))) return rc;
@@ -964,7 +951,6 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   p.row_off = m->row_off.as<long long>(); p.order = m->order.as<int>();
   p.U = J; p.n_utt = U; p.B = pl.B; p.Kcap = pl.Kcap; p.T = pl.T; p.P = pl.P; p.maxN = pl.maxN; p.G = pl.G;
   p.L = pl.L; p.node_cap = pl.node_cap; p.leaf_cap = pl.leaf_cap; p.maxTN = pl.maxTN; p.maxSteps = pl.maxSteps;
-  { const char* e = getenv("UIS_DBG_MODE"); p.dbg_mode = e ? atoi(e) : 0; }
   p.pool_mean = m->pool_mean.as<float>(); p.pool_hidden = m->pool_hidden.as<float>(); p.pool_mse = m->pool_mse.as<float>();
   p.bp = m->bp.as<unsigned>();
   p.queue = m->queue_stats.as<int>();
@@ -985,7 +971,7 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
     p.stat_bar = m->stat_bar.as<unsigned>();
     p.stat_scratch = m->stat_scratch.as<float>();
   }
-  if (pl.tcn) {
+  if (tc) {
     p.tc_wmap = m->tc_map;
     p.tc_sh = m->tc_sh; p.tc_sa = m->tc_sa;
     p.tc_inv_hh = m->tc_inv_hh; p.tc_inv_1 = m->tc_inv_1; p.tc_inv_2 = m->tc_inv_2;
@@ -1046,8 +1032,8 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
     ps.tree_spill_all = pl.kernel == uis::Kernel::TreeSpill;
     if (int rc = launch(m, pl, uis::Kernel::TreeSpill, ps, pl.spill_ctas, st)) return rc;
   }
-  m->stats.engine = pl.tcn ? 2 : 1;
-  m->stats.tc_columns = pl.tcn;
+  m->stats.engine = tc ? 2 : 1;
+  m->stats.tc_columns = tc ? uis::kTcColumns : 0;
   CU(cudaEventRecord(m->ev[2], st));
   m->stats.kernel_launches = 2 + (pl.kernel == uis::Kernel::Tree && pl.spill_ctas ? 1 : 0);
   m->stats_pending = true;

@@ -100,7 +100,6 @@ struct BeamParams {
   const int* order;         // [U] job ids, longest utterance first, the configs of one utterance side by side
   int U, B, Kcap, T, P, maxN, G;
   int L, node_cap, leaf_cap, maxTN, maxSteps;  // look_ahead >= 2 (uis_beam_tree.cuh) only
-  int dbg_mode;  // 0 normal; 1 = stream the weights but skip the math (timing experiment, results invalid)
   // tensor-core pass (uis_beam_tc.cuh): fp16 hi/lo weight planes [2 * (3H + H + D)][H] behind a tensor map
   alignas(64) CUtensorMap tc_wmap;
   float tc_sh, tc_sa;                  // power-of-two scales of the hidden columns and of a = relu(W1 h' + b1)
@@ -871,7 +870,7 @@ __device__ __forceinline__ void tc_run_pass(const BeamParams& p, const unsigned 
   using TC = TcCfg<H, D, N>;
   constexpr int NT = 256, NI = N / 8;
   // batch sizes of the GRU (KB columns) and running-mean (WB groups of 8 columns) epilogues: larger batches spill
-  constexpr int KB = (NI == 6) ? 2 : 4, WB = (NI == 6) ? 3 : NI;
+  constexpr int KB = 2, WB = 3;
   // slot s of lane g in the CTA's pools (g * P + s is small: 32-bit index arithmetic, no 64-bit strides held)
   auto hslot = [&](int g, int s) { return pool_hidden_cta + (size_t)(g * p.P + s) * H; };
   auto mslot = [&](int g, int s) { return pool_mean_cta + (size_t)(g * p.P + s) * D; };
@@ -1055,7 +1054,7 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
   const SmemLayout L_ = make_layout<H, D, C::CP, XCL, TCN, STAT>(B, Kcap, G);
   const SmemLayout& L = TC ? p.tc_layout : L_;  // tensor-core engine: read from the parameter bank, no registers
   if constexpr (TC)
-    if (p.tc_layout.total == 0) __trap();  // a launcher that did not fill tc_layout (launch_tc does)
+    if (p.tc_layout.total == 0) __trap();  // a launcher that did not fill tc_layout (launch_beam_tc does)
   const int sq = STAT ? (int)(blockIdx.x % kStatGroup) : 0, sgroup = STAT ? (int)(blockIdx.x / kStatGroup) : 0;
   float* ring = reinterpret_cast<float*>(smem + L.ring);
   float* XA = reinterpret_cast<float*>(smem + L.xa);
@@ -1702,7 +1701,6 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_beam_kernel(const __g
       if constexpr (STAT)
         stat_pass<H, D, C::CP, NT>(p, ring, XA, XB, cc, m0, Mp, pool_mean_cta, pool_hidden_cta,
                                    p.stat_scratch + (size_t)sgroup * C::CP * H, p.stat_bar + (size_t)sgroup * kStatGroup, stat_epoch, sq, tid, ph, tmark);
-      else if (p.dbg_mode == 1) drain_pass<C>(full, empty, it, lane, p.depth, xsize);
       else run_pass_any<C, DEEP, XCL>(p, ring, full, empty, it, XA, XB, cc, m0, Mp, pool_mean_cta, pool_hidden_cta, bh, b1r, b2r, tid, lane, ph, tmark, &xc);
       named_bar_sync(1, NT);
       UIS_PHASE(4);

@@ -29,6 +29,7 @@
 namespace uis {
 
 constexpr int kTcBoxBytes = 16384;  // 128 rows x 64 k, fp16
+constexpr int kTcColumns = 48;      // columns per pass: the one instantiated N
 
 template <int H, int D, int N>
 struct TcCfg {
@@ -42,9 +43,9 @@ struct TcCfg {
   static constexpr int NV = N / 2;                        // folded (hi + lo) values per thread and tile
   static constexpr int ATOM_BYTES = NP * 128;             // one k atom of the B operand
   static constexpr int BOP_BYTES = KA * ATOM_BYTES;
-  static constexpr int STAGES = (N <= 32) ? 8 : 4;        // ring depth (boxes)
+  static constexpr int STAGES = 4;                        // ring depth (boxes)
   static_assert(H % 128 == 0 && D % 128 == 0, "tensor-core pass: 128-row tiles");
-  static_assert(NP == 64 || NP == 96, "wgmma instantiations: N = 32 or 48 columns");
+  static_assert(NP == 96, "wgmma instantiation: N = 48 columns");
 };
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------------------
@@ -71,16 +72,6 @@ template <> struct Wgmma<96> {
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-        : "l"(adesc), "l"(bdesc), "r"(acc)
-        : "memory");
-  }
-};
-template <> struct Wgmma<64> {
-  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
         : "l"(adesc), "l"(bdesc), "r"(acc)
         : "memory");
   }

@@ -39,7 +39,7 @@ enum class Kernel {
   Beam,        // FFMA weight pass, G lanes per CTA (uis_beam.cuh)
   Cluster,     // latency mode: a thread-block cluster of 2/4/8 CTAs per utterance, k-split weight passes
   Stat,        // latency mode: kStatGroup CTAs per utterance keep the weights in shared memory (uis_beam_stat.cuh)
-  TensorCore,  // wgmma weight pass over N columns (uis_beam_tc.cuh)
+  TensorCore,  // wgmma weight pass over kTcColumns columns (uis_beam_tc.cuh)
   Tree,        // look_ahead >= 2, the candidate tree in shared memory (uis_beam_tree.cuh)
   TreeSpill,   // look_ahead >= 2, the tree-sized arrays in a device-memory arena (p.tree_arena)
 };
@@ -53,21 +53,11 @@ bool launch_beam_cluster(int H, int D, const BeamParams& p, int ctas, int cluste
                          cudaError_t* err);
 // `ctas` = groups * kStatGroup, cooperative launch
 bool launch_beam_stat(int H, int D, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st, cudaError_t* err);
-// N = columns per pass (32 or 48)
-bool launch_beam_tc(int H, int D, int N, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st, cudaError_t* err);
+bool launch_beam_tc(int H, int D, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st, cudaError_t* err);
 bool launch_tree_small(int H, int D, bool spill, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st,
                        cudaError_t* err);
 bool launch_tree_large(int H, int D, bool spill, const BeamParams& p, int ctas, unsigned smem, cudaStream_t st,
                        cudaError_t* err);
-
-// The tensor-core kernel's instantiations: f(std::integral_constant<int, N>{}) for N = 32 or 48; false otherwise.
-template <class F>
-bool with_tc_columns(int N, F&& f) {
-  if (N == 48) f(std::integral_constant<int, 48>{});
-  else if (N == 32) f(std::integral_constant<int, 32>{});
-  else return false;
-  return true;
-}
 
 // score(): the neg_likelihood of given labellings (uis_kernels_score.cu).  With the labels fixed, every (utterance,
 // cluster) pair is an independent chain of GRU steps over that cluster's frames; the chain kernel packs the chains'

@@ -385,39 +385,17 @@ __global__ void gru_gate_fwd_kernel(const float* __restrict__ gh, const float* _
 // work per step for a launch each (a launch + drain costs more than the step's arithmetic).  Here CTA c owns
 // kUPC = 4 hidden units for the whole sequence -- the 12 rows (forward) / 4 columns (backward) of W_hh it
 // needs stay in its shared memory (24 KB) for all L steps -- and the CTAs exchange h_t (forward) / dGh_t
-// (backward) through L2 with one grid-wide barrier per step.  H % 128 == 0, H / 4 CTAs (128 at H = 512).
+// (backward) through L2 with one grid-wide barrier per step (cooperative_groups grid.sync(): the cooperative launch
+// makes all CTAs co-resident).  H % 128 == 0, H / 4 CTAs (128 at H = 512).
 constexpr int kUPC = 4;
 // One launch covers a group of <= 32 batch columns [b0, b0 + B) of a batch that is `stride` columns wide (the
 // pointers handed to the kernels are already offset to column b0); wider batches run group after group.
-struct SeqParams { int length[32]; int L, B, H, stride, spin_barrier; };
+struct SeqParams { int length[32]; int L, B, H, stride; };
 
 __device__ __forceinline__ int seq_rows_alive(const SeqParams& sp, int t) {
   int nb = 0;
   for (int b = 0; b < sp.B; ++b) nb += sp.length[b] > t ? 1 : 0;
   return nb;
-}
-
-// Grid-wide barrier of the persistent recurrence kernels (cooperative launch: all CTAs are co-resident).  Default:
-// cooperative_groups grid.sync().  UISRNN_B200_TRAIN_BARRIER=spin selects the earlier hand-rolled arrival counter
-// (kept for A/B timing; bounded spin, a lost CTA sets *err instead of hanging the device).
-__device__ __forceinline__ void seq_grid_sync(const SeqParams& sp, unsigned* bar, unsigned target, int* err) {
-  if (!sp.spin_barrier) {
-    cooperative_groups::this_grid().sync();
-    return;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    atomicAdd(bar, 1u);
-    unsigned v = 0;
-    long long spins = 0;
-    do {
-      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory");
-    } while (v < target && ++spins < (1ll << 24));
-    if (v < target) atomicExch(err, 1);
-    __threadfence();
-  }
-  __syncthreads();
 }
 
 // Forward: for t = 0..L-1, rows b < nb(t):  gh = W_hh h_{t-1};  (r, z, n, h_t) as gru_gate_fwd_kernel.
@@ -426,7 +404,7 @@ __global__ void __launch_bounds__(256) gru_seq_fwd_kernel(const float* __restric
                                                           const float* __restrict__ gi, float* hs,
                                                           float* __restrict__ r_o, float* __restrict__ z_o,
                                                           float* __restrict__ n_o, float* __restrict__ hn_o,
-                                                          SeqParams sp, unsigned* bar, int* err) {
+                                                          SeqParams sp) {
   extern __shared__ float4 seq_smem[];
   const int H = sp.H, B = sp.stride, S = H + 4, tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   float* sW = reinterpret_cast<float*>(seq_smem);  // [3 * kUPC][H]: row g * kUPC + u = W_hh[g * H + j0 + u][:]
@@ -449,6 +427,8 @@ __global__ void __launch_bounds__(256) gru_seq_fwd_kernel(const float* __restric
     }
   };
   fetch_gi(0);
+  // (the grid handle is taken once, before the loop: taken at the barrier, ptxas 12.9 spills 44 B in this kernel)
+  cooperative_groups::grid_group grid = cooperative_groups::this_grid();
   for (int t = 0; t < sp.L; ++t) {
     const int nb = seq_rows_alive(sp, t);
     if (nb == 0) break;
@@ -498,7 +478,7 @@ __global__ void __launch_bounds__(256) gru_seq_fwd_kernel(const float* __restric
       }
     }
     fetch_gi(t + 1);
-    seq_grid_sync(sp, bar, (unsigned)(t + 1) * gridDim.x, err);
+    grid.sync();
   }
 }
 
@@ -508,8 +488,7 @@ __global__ void __launch_bounds__(256) gru_seq_bwd_kernel(const float* __restric
                                                           const float* __restrict__ r_i, const float* __restrict__ z_i,
                                                           const float* __restrict__ n_i, const float* __restrict__ hn_i,
                                                           const float* __restrict__ hs, float* __restrict__ dgi,
-                                                          float* dgh, float* __restrict__ carry_out, SeqParams sp,
-                                                          unsigned* bar, int* err) {
+                                                          float* dgh, float* __restrict__ carry_out, SeqParams sp) {
   extern __shared__ float4 seq_smem[];
   const int H = sp.H, B = sp.stride, H3 = 3 * H, CH = H3 / 4, S = CH + 4, rpw = CH / 8;
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5, j0 = blockIdx.x * kUPC;
@@ -530,7 +509,7 @@ __global__ void __launch_bounds__(256) gru_seq_bwd_kernel(const float* __restric
     }
   };
   fetch_a(sp.L - 1);
-  unsigned epoch = 0;
+  cooperative_groups::grid_group grid = cooperative_groups::this_grid();
   for (int t = sp.L - 1; t >= 0; --t) {  // lengths[0] == L: every step has at least one live row
     const int nb = seq_rows_alive(sp, t);
     const size_t o = (size_t)t * B;
@@ -547,7 +526,7 @@ __global__ void __launch_bounds__(256) gru_seq_bwd_kernel(const float* __restric
       gh[aj] = dar; gh[H + aj] = daz; gh[2 * H + aj] = dan * r;
       scarry[tid] = dh * z;
     }
-    seq_grid_sync(sp, bar, ++epoch * gridDim.x, err);
+    grid.sync();
     fetch_a(t - 1);
     // dGh_t (written by every CTA before the barrier) streams through two staging buffers: L2 -> smem copies
     // (cp.async.cg: L2 only, never a stale L1 line) of chunk c + 1 run under the product with chunk c
@@ -844,7 +823,6 @@ struct SplitCtx {
   size_t partial_cap = 0;       // floats
   unsigned* tile_tickets = nullptr;
   int ticket_cap = 0;
-  bool force_small = false;     // UISRNN_B200_TRAIN_GEMM=64: the 64x64-tile kernel everywhere (A/B timing)
   float* colsum_partial = nullptr;  // [colsum_groups][kColsumSlices][32]
   unsigned* colsum_tickets = nullptr;
   int colsum_groups = 0;
@@ -861,7 +839,7 @@ template <bool TA, bool TB>
 int gemm(cudaStream_t st, const SplitCtx& sc, const float* A, const float* B, const float* bias, const float* mask,
          float* C, int M, int N, int K, bool relu = false, bool acc = false) {
   if (M <= 0 || N <= 0) return 0;
-  const bool big = M >= 128 && N >= 128 && !sc.force_small;  // 128x128 tiles; tiny models keep the 64x64 kernel
+  const bool big = M >= 128 && N >= 128;  // 128x128 tiles; tiny models keep the 64x64 kernel
   const int T = big ? 128 : 64;
   dim3 grid((N + T - 1) / T, (M + T - 1) / T, 1);
   const int tiles = grid.x * grid.y;
@@ -920,10 +898,8 @@ struct uis_trainer {
   size_t pin_cap = 0;
   cudaEvent_t pin_ev[2] = {nullptr, nullptr};
   int pin_idx = 0;
+  int seq_mode = -1;  // -1 unknown, 0 per-step launches, 1 persistent cooperative kernels
   // corpus path: training rows (fp32) + flat gather indices + per-sub-sequence offsets (host copy)
-  unsigned* seq_bar = nullptr;  // [2] arrival counters of the persistent recurrence kernels; [2] = error flag
-  int seq_mode = -1;            // -1 unknown, 0 per-step launches, 1 persistent cooperative kernels
-  int spin_barrier = 0;
   uis::DBuf corpus;
   int* corpus_index = nullptr;
   long long corpus_rows = 0;
@@ -1009,10 +985,6 @@ int uis_trainer_create(uis_trainer** out, int device, int D, int H, const float*
   t->total = t->seg_off_h[t->n_seg];
   t->rnn_end = t->seg_off_h[t->seg_h0()];
   t->sigma_begin = t->seg_off_h[t->seg_sigma2()];
-  {
-    const char* env = std::getenv("UISRNN_B200_TRAIN_BARRIER");
-    t->spin_barrier = (env && std::strcmp(env, "spin") == 0) ? 1 : 0;
-  }
   auto body = [&]() -> int {
     if (int rc = t->params.ensure(t->total)) return rc;
     if (int rc = t->grads.ensure(t->total)) return rc;
@@ -1033,10 +1005,6 @@ int uis_trainer_create(uis_trainer** out, int device, int D, int H, const float*
     CUT(cudaMemset(t->gemm_tickets, 0, 4096 * sizeof(unsigned)));
     if (int rc = t->gemm_partial.ensure((size_t)4096 * 4096)) return rc;  // 64 MB of split-K partial tiles
     t->sc.partial = t->gemm_partial.p; t->sc.partial_cap = t->gemm_partial.cap; t->sc.tile_tickets = t->gemm_tickets; t->sc.ticket_cap = 4096;
-    {
-      const char* env = std::getenv("UISRNN_B200_TRAIN_GEMM");
-      t->sc.force_small = env && std::strcmp(env, "64") == 0;
-    }
     t->sc.colsum_groups = (std::max(3 * H, D) + 31) / 32;
     CUT(cudaMalloc(&t->sc.colsum_partial, (size_t)t->sc.colsum_groups * uis::kColsumSlices * 32 * sizeof(float)));
     CUT(cudaMalloc(&t->sc.colsum_tickets, (size_t)t->sc.colsum_groups * sizeof(unsigned)));
@@ -1062,7 +1030,6 @@ int uis_trainer_destroy(uis_trainer* t) {
   if (t->sc.colsum_partial) cudaFree(t->sc.colsum_partial);
   if (t->sc.colsum_tickets) cudaFree(t->sc.colsum_tickets);
   if (t->corpus_index) cudaFree(t->corpus_index);
-  if (t->seq_bar) cudaFree(t->seq_bar);
   t->corpus.release();
   for (int i = 0; i < 2; ++i) {
     if (t->pin[i]) cudaFreeHost(t->pin[i]);
@@ -1095,18 +1062,7 @@ int seq_setup(uis_trainer* t) {
   CUT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, uis::gru_seq_fwd_kernel, 256, seq_fwd_smem(H)));
   CUT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, uis::gru_seq_bwd_kernel, 256, seq_bwd_smem(H)));
   if (occ_f * sms < H / uis::kUPC || occ_b * sms < H / uis::kUPC) return 0;
-  CUT(cudaMalloc(&t->seq_bar, 4 * sizeof(unsigned)));
-  CUT(cudaMemset(t->seq_bar, 0, 4 * sizeof(unsigned)));
   t->seq_mode = 1;
-  return 0;
-}
-
-// After a synchronisation: did a grid barrier of the persistent recurrence kernels ever time out?
-int seq_check(uis_trainer* t) {
-  if (!t->seq_bar) return 0;
-  int flag = 0;
-  CUT(cudaMemcpy(&flag, t->seq_bar + 2, sizeof(int), cudaMemcpyDeviceToHost));
-  if (flag) return uis::api_fail(UIS_ERR_CUDA, "persistent recurrence kernel: grid barrier timed out");
   return 0;
 }
 
@@ -1311,13 +1267,11 @@ int run_iteration(uis_trainer* t, const int32_t* lengths, int B, int L, int mode
       if (t->seq_mode == 1) {
         SeqParams sp{};
         for (int b = 0; b < 32; ++b) sp.length[b] = b < nbg ? lengths[b0 + b] : 0;
-        sp.L = Lg; sp.B = nbg; sp.H = H; sp.stride = B; sp.spin_barrier = t->spin_barrier;
-        CUT(cudaMemsetAsync(t->seq_bar, 0, 2 * sizeof(unsigned), st));
+        sp.L = Lg; sp.B = nbg; sp.H = H; sp.stride = B;
         const float* a_whh = whh; const float* a_bhh = bhh; const float* a_gi = gi_l + (size_t)b0 * 3 * H;
         float* a_hs = hs_l + (size_t)b0 * H; float* a_r = r_l + (size_t)b0 * H; float* a_z = z_l + (size_t)b0 * H;
         float* a_n = n_l + (size_t)b0 * H; float* a_hn = hn_l + (size_t)b0 * H;
-        unsigned* a_bar = t->seq_bar; int* a_err = reinterpret_cast<int*>(t->seq_bar + 2);
-        void* args[] = {&a_whh, &a_bhh, &a_gi, &a_hs, &a_r, &a_z, &a_n, &a_hn, &sp, &a_bar, &a_err};
+        void* args[] = {&a_whh, &a_bhh, &a_gi, &a_hs, &a_r, &a_z, &a_n, &a_hn, &sp};
         CUT(cudaLaunchCooperativeKernel((const void*)gru_seq_fwd_kernel, dim3(H / kUPC), dim3(256), args, seq_fwd_smem(H), st));
       } else {
         for (int tt = 0; tt < Lg; ++tt) {
@@ -1374,15 +1328,13 @@ int run_iteration(uis_trainer* t, const int32_t* lengths, int B, int L, int mode
       if (t->seq_mode == 1) {
         SeqParams sp{};
         for (int b = 0; b < 32; ++b) sp.length[b] = b < nbg ? lengths[b0 + b] : 0;
-        sp.L = Lg; sp.B = nbg; sp.H = H; sp.stride = B; sp.spin_barrier = t->spin_barrier;
-        CUT(cudaMemsetAsync(t->seq_bar, 0, 2 * sizeof(unsigned), st));
+        sp.L = Lg; sp.B = nbg; sp.H = H; sp.stride = B;
         const float* a_whh = whh; const float* a_dout = t->dout.p + (size_t)b0 * H; const float* a_r = r_l + (size_t)b0 * H;
         const float* a_z = z_l + (size_t)b0 * H; const float* a_n = n_l + (size_t)b0 * H; const float* a_hn = hn_l + (size_t)b0 * H;
         const float* a_hs = hs_l + (size_t)b0 * H;
         float* a_dgi = t->dgi.p + (size_t)b0 * 3 * H; float* a_dgh = t->dgh.p + (size_t)b0 * 3 * H;
         float* a_carry = t->carry.p + (size_t)b0 * H;
-        unsigned* a_bar = t->seq_bar + 1; int* a_err = reinterpret_cast<int*>(t->seq_bar + 2);
-        void* args[] = {&a_whh, &a_dout, &a_r, &a_z, &a_n, &a_hn, &a_hs, &a_dgi, &a_dgh, &a_carry, &sp, &a_bar, &a_err};
+        void* args[] = {&a_whh, &a_dout, &a_r, &a_z, &a_n, &a_hn, &a_hs, &a_dgi, &a_dgh, &a_carry, &sp};
         CUT(cudaLaunchCooperativeKernel((const void*)gru_seq_bwd_kernel, dim3(H / kUPC), dim3(256), args, seq_bwd_smem(H), st));
       } else {
         for (int tt = Lg - 1; tt >= 0; --tt) {
@@ -1428,7 +1380,6 @@ int uis_trainer_losses(uis_trainer* t, int count, float* out) {
   uis::DeviceGuard device_guard_(t->device);
   CUT(device_guard_.status);
   CUT(cudaDeviceSynchronize());
-  if (int rc = seq_check(t)) return rc;
   for (int i = 0; i < count; ++i) {
     const long long slot = (t->calls - count + i) % t->hist_cap;
     CUT(cudaMemcpy(out + 3 * i, t->loss_hist.p + 3 * slot, 3 * sizeof(float), cudaMemcpyDeviceToHost));
@@ -1473,7 +1424,6 @@ int uis_trainer_get(uis_trainer* t, int what, float* const* out) {
   uis::DeviceGuard device_guard_(t->device);
   CUT(device_guard_.status);
   CUT(cudaDeviceSynchronize());
-  if (int rc = seq_check(t)) return rc;
   const float* src = what == 0 ? t->params.p : t->grads.p;
   for (int s = 0; s < t->n_seg; ++s)
     if (out[s])

@@ -288,12 +288,9 @@ class UISRNN:
   def _native_fit_supported(self, args):
     """On a CUDA device fit() runs on the hand-written training kernels (csrc/uis_train.cu): 1..4 stacked GRU
     layers (inter-layer dropout in train mode), any mini-batch width including batch_size=None (one batch of
-    every sub-sequence).  UISRNN_B200_TORCH_FIT=1 selects PyTorch autograd instead (a developer switch for A/B
-    checks); the CPU device always trains with PyTorch, as the reference does."""
-    import os
+    every sub-sequence).  The CPU device always trains with PyTorch, as the reference does."""
     del args
-    return (self.device.type == 'cuda' and 1 <= self.rnn_init_hidden.shape[0] <= 4 and
-            os.environ.get('UISRNN_B200_TORCH_FIT', '0') != '1')
+    return self.device.type == 'cuda' and 1 <= self.rnn_init_hidden.shape[0] <= 4
 
   def _fit_native(self, train_sequence, index_lists, seq_lengths, args):
     """fit_concatenated's iteration loop (uisrnn.py:252-311) on libuisrnn_b200.so: the training set,
