@@ -308,6 +308,28 @@ int uis_score_device_sweep(uis_model* m, const float* x_dev, const int64_t* fram
                            const int32_t* labels_dev, float* scores_dev, float* frame_dev, void* stream,
                            const uis_decode_params* params);
 
+/*
+ * Scoring labellings held on the device as arbitrary ids (same ABI version 7; additive).  uis_score_device_sweep with
+ *   ids_dev      int64 [frame_offsets[U]] device memory: any values per frame.  A labelling is taken up to renaming:
+ *                frame t of utterance u belongs to cluster c, c = the number of distinct ids of u first seen before
+ *                ids_dev[t]'s first appearance (what canonical labels hold), so no input is an invalid labelling.
+ *   labels_dev   int32 [frame_offsets[U]] device memory, may be NULL: receives those canonical labels.
+ * The other arguments and the outputs are those of uis_score_device_sweep; frame_offsets[0] must be 0, the list
+ * holds fewer than 2^31 - 1 frames, x_dev is 16-byte aligned (the rows are read with 16-byte loads) and ids_dev 8-byte
+ * aligned; anything else is UIS_ERR_INVALID.  The renaming and the chain plan run on the device (sorts and scans on `stream`),
+ * so the call reads nothing back: it enqueues its work on `stream` and returns, except where a sweep rewrites its log
+ * tables (see above) or the handle's workspace grows (cudaMalloc / cudaFree).  The scores are those
+ * uis_score_device_sweep gives for the canonical labels, bit for bit.  uis_get_stats fills the fields a score call
+ * fills, max_k from the device plan.
+ *
+ * Every entry point of a handle orders its device work after the previous call's: each call records an event on its
+ * stream at its end, and the next call's stream waits for it (cudaStreamWaitEvent; the host does not block).  So calls
+ * on one handle from different streams do not overwrite the workspace under each other's kernels.
+ */
+int uis_score_device_ids(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
+                         const int64_t* ids_dev, float* scores_dev, float* frame_dev, int32_t* labels_dev,
+                         void* stream, const uis_decode_params* params);
+
 /* Device bytes uis_predict_device() will hold for this problem (workspace is cached in the handle). */
 size_t uis_predict_workspace_bytes(uis_model* m, const int64_t* frame_offsets, int U,
                                    const uis_predict_opts* opts);

@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libuisrnn_b200.so')
 STAMP = LIB + '.srchash'
 SOURCES = ['uis_api.cu', 'uis_train.cu', 'uis_kernels_beam_large.cu', 'uis_kernels_beam_small.cu', 'uis_kernels_beam_cluster.cu', 'uis_kernels_beam_stat.cu', 'uis_kernels_beam_tc.cu',
-           'uis_kernels_tree_large.cu', 'uis_kernels_tree_small.cu', 'uis_kernels_score.cu']
+           'uis_kernels_tree_large.cu', 'uis_kernels_tree_small.cu', 'uis_kernels_score.cu', 'uis_score_plan.cu']
 DEPS = SOURCES + ['uis_beam.cuh', 'uis_beam_tc.cuh', 'uis_beam_stat.cuh', 'uis_beam_tree.cuh', 'uis_prepass.cuh', 'uis_common.cuh', 'uis_launch.cuh',
         os.path.join('..', '..', 'include', 'uisrnn_b200.h')]
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',

@@ -186,6 +186,7 @@ struct uis_model {
   DevBuf tree_arena;  // look-ahead spill kernel: [spill CTAs][make_tree_arena(..).total]
   // score calls (uis_kernels_score.cu): chain plan, per-frame Gaussian terms, reduce scratch, host entry's outputs
   DevBuf sc_chain_off, sc_chain_rows, sc_mse, sc_blocks, sc_out;
+  DevBuf sc_counts, sc_plan;  // device-planned score calls: {chains, queued, max_k}; the plan kernels' scratch
   DevBuf dbg_win, dbg_score, dbg_off, dbg_final_scores, dbg_final_k, dbg_best_mean, dbg_best_hidden,
       dbg_best_blocks;
   // last call
@@ -193,6 +194,11 @@ struct uis_model {
   int last_U = 0;
   bool last_tree_spill = false;  // the last call ran the look-ahead spill kernel (its caps name the arena in errors)
   bool last_score = false;       // the last call was a score call (two counters, no per-utterance status)
+  bool last_score_counts = false;  // ... whose chains were planned on the device: max_k is in sc_counts
+  // every call records ev_done on its stream after its last work, and the next call's stream waits for it: a call on
+  // another stream must not overwrite the workspace while the previous call's kernels still read it
+  cudaEvent_t ev_done = nullptr;
+  bool done_recorded = false;
   int last_spill_ni = 0, last_spill_nlf = 0;
   size_t last_spill_budget = 0;
   cudaStream_t last_stream = nullptr;
@@ -1069,9 +1075,14 @@ int collect(uis_model* m) {
   CU(cudaStreamSynchronize(m->last_stream));
   unsigned long long s[24];
   CU(cudaMemcpy(s, m->queue_stats.as<unsigned long long>() + 8, sizeof s, cudaMemcpyDeviceToHost));
-  if (m->last_score) {  // the chain kernel's columns and passes; max_k came from the labels
+  if (m->last_score) {  // the chain kernel's columns and passes; max_k came from the labels (or the device plan)
     m->stats.gru_columns = (int64_t)s[0];
     m->stats.weight_passes = (int64_t)s[1];
+    if (m->last_score_counts) {
+      int counts[3];
+      CU(cudaMemcpy(counts, m->sc_counts.p, sizeof counts, cudaMemcpyDeviceToHost));
+      m->stats.max_k = counts[2];
+    }
     CU(cudaEventElapsedTime(&m->stats.prepass_ms, m->ev[0], m->ev[1]));
     CU(cudaEventElapsedTime(&m->stats.beam_ms, m->ev[1], m->ev[2]));
     m->stats_pending = false;
@@ -1131,6 +1142,27 @@ void drain_after_failure(uis_model* m, cudaStream_t st) {
   g_err = keep;
 }
 
+// Orders one call's device work after the previous call's on the same handle.  Every call shares the handle's
+// workspace (gi, slot pools, chain plans, ...), so a call on another stream could overwrite it while the previous
+// call's kernels still read it.  Constructed before the call's first enqueue: `st` waits for the event the previous
+// call recorded at its end (cudaStreamWaitEvent: the host does not block; on the previous call's own stream the wait
+// adds nothing).  Destroyed when the call returns: records that event on `st`.
+class CallOrder {
+ public:
+  CallOrder(uis_model* m, cudaStream_t st) : m_(m), st_(st) {
+    if (!m->ev_done) status = cudaEventCreateWithFlags(&m->ev_done, cudaEventDisableTiming);
+    else if (m->done_recorded) status = cudaStreamWaitEvent(st, m->ev_done, 0);
+  }
+  ~CallOrder() {
+    if (m_->ev_done) m_->done_recorded = cudaEventRecord(m_->ev_done, st_) == cudaSuccess;
+  }
+  cudaError_t status = cudaSuccess;
+
+ private:
+  uis_model* m_;
+  cudaStream_t st_;
+};
+
 int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
                         const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
                         const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev,
@@ -1144,6 +1176,8 @@ int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_o
   uis::DeviceGuard device_guard_(m->device);
   CU(device_guard_.status);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CallOrder order(m, st);
+  CU(order.status);
   if (int rc = pad_to_kernel_d(m, &x_dev, (size_t)pl.rows, st)) return rc;
   return run_device(m, x_dev, frame_offsets, U, pl, labels_dev, taps, st,
                     SpeakerBounds{max_speakers, min_speakers, speakers_dev}, nb, dp);
@@ -1404,6 +1438,8 @@ int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_
   CU(device_guard_.status);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (pl.rows == 0) return 0;
+  CallOrder order(m, st);
+  CU(order.status);
   // Memory: the per-frame workspace (gi 12H B + fp32 rows 4D B + labels) is the part that grows with the input.
   // A list that does not fit the device at once is decoded in groups of whole utterances, one after the other
   // (utterances are independent, uisrnn.py:587-589); UISRNN_B200_MAX_ROWS forces a limit (tests).
@@ -1496,8 +1532,9 @@ int plan_chains(const int32_t* labels, const int64_t* off, int U, ChainPlan* cp)
 
 // Enqueues a score call on `st`: input projection (unless gi_ready), chain kernel, first visits, then one reduce per
 // config of `dp` (scores_dev [configs][U], frame_dev [configs][rows]).  x_dev: the fp32 rows at the kernel shape (m->D);
-// labels_dev: the canonical labels the plan was made from.
-int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const ChainPlan& cp, const int32_t* labels_dev,
+// labels_dev: the canonical labels the plan was made from.  cp: a host plan, uploaded here; nullptr: the device plan
+// that score_plan wrote to sc_chain_off / sc_chain_rows / sc_counts earlier on `st` (row_off is on the device too).
+int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const ChainPlan* cp, const int32_t* labels_dev,
               float* scores_dev, float* frame_dev, cudaStream_t st, bool gi_ready, const DecodeParams& dp) {
   const int H = m->H, D = m->D;
   const long long rows = off[U];
@@ -1509,20 +1546,25 @@ int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const
   if (uis::score_smem(H, D) > uis::kSmemCap) return fail(UIS_ERR_UNSUPPORTED, "no score kernel for hidden=%d dim=%d", H, D);
   int CP = 0;  // columns per pass: the FFMA beam kernel's
   uis::with_shape(uis::AllShapes{}, H, D, [&](auto s) { CP = uis::beam_cp<decltype(s)::H>(); });
-  const int ctas = (int)std::max(1ll, std::min<long long>(m->num_sms, (cp.queued + CP - 1) / CP));
+  // a device plan's counts are not known here: the grids are sized from their bounds (every queued chain has two frames)
+  const long long queued = cp ? cp->queued : rows / 2;
+  const int ctas = (int)std::max(1ll, std::min<long long>(m->num_sms, (queued + CP - 1) / CP));
   if (int rc = m->row_off.ensure((U + 1) * sizeof(long long))) return rc;
   if (int rc = m->queue_stats.ensure(40 * sizeof(unsigned long long))) return rc;
   if (int rc = m->gi.ensure((size_t)rows * 3 * H * sizeof(float))) return rc;
   if (int rc = m->pool_mean.ensure((size_t)ctas * CP * 2 * D * sizeof(float))) return rc;
   if (int rc = m->pool_hidden.ensure((size_t)ctas * CP * 2 * m->depth * H * sizeof(float))) return rc;
-  if (int rc = m->sc_chain_off.ensure(cp.off.size() * sizeof(long long))) return rc;
-  if (int rc = m->sc_chain_rows.ensure(cp.rows.size() * sizeof(long long))) return rc;
   if (int rc = m->sc_mse.ensure((size_t)rows * sizeof(float))) return rc;
   if (int rc = m->sc_blocks.ensure((size_t)rows * sizeof(int))) return rc;
-  std::vector<long long> off_ll(off, off + U + 1);
-  CU(cudaMemcpyAsync(m->row_off.p, off_ll.data(), (U + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(m->sc_chain_off.p, cp.off.data(), cp.off.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(m->sc_chain_rows.p, cp.rows.data(), cp.rows.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+  if (cp) {
+    if (int rc = m->sc_chain_off.ensure(cp->off.size() * sizeof(long long))) return rc;
+    if (int rc = m->sc_chain_rows.ensure(cp->rows.size() * sizeof(long long))) return rc;
+    std::vector<long long> off_ll(off, off + U + 1);
+    CU(cudaMemcpyAsync(m->row_off.p, off_ll.data(), (U + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(m->sc_chain_off.p, cp->off.data(), cp->off.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(m->sc_chain_rows.p, cp->rows.data(), cp->rows.size() * sizeof(long long), cudaMemcpyHostToDevice,
+                       st));
+  }
   CU(cudaMemsetAsync(m->queue_stats.p, 0, 40 * sizeof(unsigned long long), st));
 
   sp.b.x = x_dev; sp.b.gi = m->gi.as<float>();
@@ -1532,7 +1574,8 @@ int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const
   sp.b.queue = m->queue_stats.as<int>();
   sp.b.stats = m->queue_stats.as<unsigned long long>() + 8;
   sp.chain_off = m->sc_chain_off.as<long long>(); sp.chain_rows = m->sc_chain_rows.as<long long>();
-  sp.chains = cp.chains; sp.queued = cp.queued;
+  sp.chains = cp ? cp->chains : (int)rows; sp.queued = (int)queued;
+  sp.counts = cp ? nullptr : m->sc_counts.as<int>();
   sp.mse = m->sc_mse.as<float>(); sp.labels = labels_dev; sp.scores = scores_dev; sp.frame_out = frame_dev;
   sp.blocks = m->sc_blocks.as<int>();
 
@@ -1547,7 +1590,7 @@ int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const
   }
   CU(cudaEventRecord(m->ev[1], st));
   cudaError_t e = cudaSuccess;
-  if (cp.queued > 0) {
+  if (queued > 0) {
     if (!uis::launch_score_chains(H, D, sp, ctas, st, &e))
       return fail(UIS_ERR_UNSUPPORTED, "no score kernel for hidden=%d dim=%d", H, D);
     if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score chain kernel launch failed: %s", cudaGetErrorString(e));
@@ -1559,8 +1602,8 @@ int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const
     e = uis::launch_score_reduce(sp, c, st);
     if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score reduce kernel launch failed: %s", cudaGetErrorString(e));
   }
-  m->stats.ctas = cp.queued > 0 ? ctas : 0;
-  m->stats.kernel_launches = (gi_ready ? 0 : 1) + (cp.queued > 0 ? 1 : 0) + 1 + dp.count;
+  m->stats.ctas = queued > 0 ? ctas : 0;
+  m->stats.kernel_launches = (gi_ready ? 0 : 1) + (queued > 0 ? 1 : 0) + 1 + dp.count;
   m->stats_pending = true;
   return 0;
 }
@@ -1574,6 +1617,7 @@ void begin_score_stats(uis_model* m, int jobs, long long rows, const ChainPlan& 
   m->stats.engine = 1;
   m->last_U = jobs;
   m->last_score = true;
+  m->last_score_counts = false;
   m->last_tree_spill = false;
   m->last_stream = st;
   m->stats_pending = false;
@@ -1607,7 +1651,7 @@ int score_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_fr
   CU(cudaMemcpyAsync(m->labels.p, lab.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, st));
   if (int rc = m->sc_out.ensure(((size_t)U + (frame_out ? (size_t)rows : 0)) * C * 4)) return rc;
   float* dev_frames = frame_out ? m->sc_out.as<float>() + (size_t)U * C : nullptr;
-  if (int rc = run_score(m, m->x32.as<float>(), off.data(), U, cp, m->labels.as<int32_t>(), m->sc_out.as<float>(),
+  if (int rc = run_score(m, m->x32.as<float>(), off.data(), U, &cp, m->labels.as<int32_t>(), m->sc_out.as<float>(),
                          dev_frames, st, /*gi_ready=*/true, dp))
     return rc;
   m->stats.kernel_launches += 2 * (int64_t)n_chunks;
@@ -1638,6 +1682,8 @@ int score_host(uis_model* m, const double* const* seqs, const int64_t* n_frames,
   uis::DeviceGuard device_guard_(m->device);
   CU(device_guard_.status);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CallOrder order(m, st);
+  CU(order.status);
   const int rc = score_host_impl(m, seqs, n_frames, U, labels, scores_out, frame_out, st, dp);
   if (rc != 0 && rc != UIS_ERR_INVALID) drain_after_failure(m, st);
   return rc;
@@ -1653,6 +1699,8 @@ int score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets,
   uis::DeviceGuard device_guard_(m->device);
   CU(device_guard_.status);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CallOrder order(m, st);
+  CU(order.status);
   // the chain plan is made on the host: the labels come back first (this synchronises `stream`)
   std::vector<int32_t> lab((size_t)std::max(rows, 0ll));
   if (rows > 0) {
@@ -1668,7 +1716,58 @@ int score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets,
     return 0;
   }
   if (int rc = pad_to_kernel_d(m, &x_dev, (size_t)rows, st)) return rc;
-  return run_score(m, x_dev, frame_offsets, U, cp, labels_dev, scores_dev, frame_dev, st, /*gi_ready=*/false, dp);
+  return run_score(m, x_dev, frame_offsets, U, &cp, labels_dev, scores_dev, frame_dev, st, /*gi_ready=*/false, dp);
+}
+
+// score_device with arbitrary int64 ids per frame: the renaming and the chain plan run on the device (score_plan), so
+// nothing is read back and the call only enqueues.
+// The arguments are checked before the handle, so that a bad call is rejected the same way with or without a device.
+int score_device_ids(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U, const int64_t* ids_dev,
+                     float* scores_dev, float* frame_dev, int32_t* labels_dev, void* stream,
+                     const uis_decode_params* params) {
+  if (U < 0 || (U > 0 && (!frame_offsets || !scores_dev))) return fail(UIS_ERR_INVALID, "null argument");
+  if (U > 0 && frame_offsets[0] != 0) return fail(UIS_ERR_INVALID, "frame_offsets[0] must be 0");
+  for (int u = 0; u < U; ++u)
+    if (frame_offsets[u + 1] < frame_offsets[u]) return fail(UIS_ERR_INVALID, "frame_offsets not monotone");
+  const long long rows = U > 0 ? frame_offsets[U] : 0;
+  if (rows > 0 && (!x_dev || !ids_dev)) return fail(UIS_ERR_INVALID, "null device buffer");
+  // the input projection reads the rows with float4 loads; the ids are read as int64
+  if (rows > 0 && (reinterpret_cast<uintptr_t>(x_dev) % 16 || reinterpret_cast<uintptr_t>(ids_dev) % 8))
+    return fail(UIS_ERR_INVALID, "x_dev must be 16-byte aligned and ids_dev 8-byte aligned");
+  if (rows >= 0x7fffffffll) return fail(UIS_ERR_UNSUPPORTED, "%lld frames: a device-planned score call holds < 2^31 - 1", rows);
+  if (!m) return fail(UIS_ERR_INVALID, "model is NULL");
+  DecodeParams dp;
+  if (int rc = check_decode(params, U, &dp)) return rc;
+  uis::DeviceGuard device_guard_(m->device);
+  CU(device_guard_.status);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CallOrder order(m, st);
+  CU(order.status);
+  begin_score_stats(m, U * dp.count, rows, ChainPlan{}, st);
+  if (U == 0) return 0;
+  if (rows == 0) {
+    CU(cudaMemsetAsync(scores_dev, 0, (size_t)U * dp.count * 4, st));  // empty utterances score 0
+    return 0;
+  }
+  if (int rc = pad_to_kernel_d(m, &x_dev, (size_t)rows, st)) return rc;
+  const size_t plan_bytes = uis::score_plan_bytes(rows, U);
+  if (int rc = m->row_off.ensure((U + 1) * sizeof(long long))) return rc;
+  if (int rc = m->labels.ensure((size_t)rows * 4)) return rc;
+  if (int rc = m->sc_chain_off.ensure((size_t)(rows + 1) * sizeof(long long))) return rc;
+  if (int rc = m->sc_chain_rows.ensure((size_t)rows * sizeof(long long))) return rc;
+  if (int rc = m->sc_counts.ensure(4 * sizeof(int))) return rc;
+  if (int rc = m->sc_plan.ensure(plan_bytes)) return rc;
+  std::vector<long long> off_ll(frame_offsets, frame_offsets + U + 1);
+  CU(cudaMemcpyAsync(m->row_off.p, off_ll.data(), (U + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+  CU(uis::score_plan(reinterpret_cast<const long long*>(ids_dev), m->row_off.as<long long>(), U, rows, m->sc_plan.p,
+                     m->sc_plan.cap, m->labels.as<int>(), labels_dev, m->sc_chain_off.as<long long>(),
+                     m->sc_chain_rows.as<long long>(), m->sc_counts.as<int>(), m->num_sms, st));
+  m->last_score_counts = true;
+  if (int rc = run_score(m, x_dev, frame_offsets, U, nullptr, m->labels.as<int32_t>(), scores_dev, frame_dev, st,
+                         /*gi_ready=*/false, dp))
+    return rc;
+  m->stats.kernel_launches += uis::kScorePlanLaunches;
+  return 0;
 }
 
 }  // namespace
@@ -1758,7 +1857,7 @@ int uis_model_destroy(uis_model* m) {
                     &m->dbg_score, &m->dbg_off, &m->dbg_final_scores, &m->dbg_final_k, &m->dbg_best_mean,
                     &m->dbg_best_hidden, &m->dbg_best_blocks, &m->tc_planes, &m->tc_scratch, &m->pool_mse, &m->stat_bar, &m->stat_scratch,
                     &m->tree_arena, &m->nb_scores, &m->nb_speakers, &m->nb_count, &m->sc_chain_off,
-                    &m->sc_chain_rows, &m->sc_mse, &m->sc_blocks, &m->sc_out};
+                    &m->sc_chain_rows, &m->sc_mse, &m->sc_blocks, &m->sc_out, &m->sc_counts, &m->sc_plan};
   for (DevBuf* b : bufs) b->release();
   for (auto& e : m->ev)
     if (e) cudaEventDestroy(e);
@@ -1769,6 +1868,7 @@ int uis_model_destroy(uis_model* m) {
   for (auto& e : m->ev_h2d)
     if (e) cudaEventDestroy(e);
   if (m->ev_pipe) cudaEventDestroy(m->ev_pipe);
+  if (m->ev_done) cudaEventDestroy(m->ev_done);
   if (m->copy_stream) cudaStreamDestroy(m->copy_stream);
   if (m->labels_pin) cudaFreeHost(m->labels_pin);
   for (auto& e : m->ev_dma)
@@ -1900,6 +2000,12 @@ int uis_score_device_sweep(uis_model* m, const float* x_dev, const int64_t* fram
   DecodeParams dp;
   if (int rc = check_decode(params, U, &dp)) return rc;
   return score_device(m, x_dev, frame_offsets, U, labels_dev, scores_dev, frame_dev, stream, dp);
+}
+
+int uis_score_device_ids(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U, const int64_t* ids_dev,
+                         float* scores_dev, float* frame_dev, int32_t* labels_dev, void* stream,
+                         const uis_decode_params* params) {
+  return score_device_ids(m, x_dev, frame_offsets, U, ids_dev, scores_dev, frame_dev, labels_dev, stream, params);
 }
 
 }  // extern "C"

@@ -93,11 +93,12 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_score_kernel(const __
   if (tid < D) wv[tid] = p.wvec[tid];
   long long st_cols = 0, st_pass = 0;  // thread 0's
 
-  // (thread 0) bind column m to the next queued chain, or retire it
+  // (thread 0) bind column m to the next queued chain, or retire it (a device plan's count is read here, where it is
+  // used: held across the loop it costs the larger shapes a spill; the surplus CTAs of its grid find the queue empty)
   auto bind = [&](int m) {
     const int q = atomicAdd(p.queue, 1);
     cchain[m] = -1;
-    if (q < sp.queued) {
+    if (q < (sp.counts ? __ldg(sp.counts + 1) : sp.queued)) {
       cchain[m] = q; cpos[m] = 0; ccur[m] = 0; cfresh[m] = 1;
       cstart[m] = sp.chain_off[q];
       clen[m] = (int)(sp.chain_off[q + 1] - sp.chain_off[q]);
@@ -189,13 +190,14 @@ __global__ void __launch_bounds__(Cfg<H, D>::BLOCK, 1) uis_score_kernel(const __
   }
 }
 
-// mean0 against the first frame of every chain: one warp per chain.
+// mean0 against the first frame of every chain: one warp per chain (a device plan: the grid covers `chains` = rows
+// warps, and those past the plan's chain count return).
 template <int D>
 __global__ void __launch_bounds__(256) score_first_kernel(const __grid_constant__ ScoreParams sp) {
   const BeamParams& p = sp.b;
   const int lane = threadIdx.x & 31;
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (w >= sp.chains) return;  // (whole warps)
+  if (w >= (sp.counts ? sp.counts[0] : sp.chains)) return;  // (whole warps)
   const long long row = sp.chain_rows[sp.chain_off[w]];
   float4 m4[1][(D + 127) / 128];
 #pragma unroll

@@ -73,6 +73,10 @@ struct ScoreParams {
   float* scores;                // [configs][U]    neg_likelihood
   float* frame_out;             // [configs][rows] per-frame increments (may be null)
   int* blocks;                  // [rows] reduce kernel scratch: block counts of utterance u's clusters at row_off[u]
+  // A plan made on the device (score_plan): {chains, queued, max_k} in device memory, written by the plan kernels
+  // earlier on the stream.  The kernels read `chains` / `queued` from here; the two fields above then only bound the
+  // launch grids (chains <= rows, queued <= rows / 2).  nullptr for a host plan.
+  const int* counts;
 };
 unsigned score_smem(int H, int D);  // kNoKernel if (H, D) is not an instantiated shape
 // the three kernels of a score call, in order: chains (Gaussian terms of every visit after the first, C::CP = beam_cp
@@ -81,6 +85,20 @@ unsigned score_smem(int H, int D);  // kNoKernel if (H, D) is not an instantiate
 bool launch_score_chains(int H, int D, const ScoreParams& sp, int ctas, cudaStream_t st, cudaError_t* err);
 bool launch_score_first(int H, int D, const ScoreParams& sp, cudaStream_t st, cudaError_t* err);
 cudaError_t launch_score_reduce(const ScoreParams& sp, int cfg, cudaStream_t st);
+
+// The chain plan of a score call with arbitrary int64 ids per frame (uis_score_device_ids), made on the device: the
+// plan plan_chains (uis_api.cu) makes from the canonical labels, with no read-back.  The (id, frame) pairs are sorted
+// stably by id, then by utterance, so each run of equal ids is one chain with its frames in order; the first frames of
+// the runs, scanned in frame order, give the canonical labels and the chain ids (utterance base + canonical label); the
+// chain ids are sorted stably by descending run length.  Outputs: labels [rows] (and labels_out, may be null) the
+// canonical labels; chain_off [rows + 1] (entries past the last chain hold rows); chain_rows [rows]; counts [3] =
+// {chains, queued (chains of length >= 2), max_k (most clusters in one utterance)}.  row_off: device [U + 1].
+// ws: score_plan_bytes(rows, U) bytes of device scratch.  Everything is enqueued on `st`.  rows <= INT_MAX - 1.
+size_t score_plan_bytes(long long rows, int U);
+constexpr int kScorePlanLaunches = 13;  // score_plan's kernels and CUB calls (uis_stats.kernel_launches counts each once)
+cudaError_t score_plan(const long long* ids, const long long* row_off, int U, long long rows, void* ws, size_t ws_bytes,
+                       int* labels, int* labels_out, long long* chain_off, long long* chain_rows, int* counts,
+                       int num_sms, cudaStream_t st);
 
 template <class Kern, class Params>
 inline cudaError_t launch_with_smem(Kern kern, const Params& p, int ctas, int block, unsigned smem, cudaStream_t st) {

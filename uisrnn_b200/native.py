@@ -74,7 +74,7 @@ EXPORTS = ('uis_version', 'uis_last_error', 'uis_model_create', 'uis_model_destr
            'uis_model_constants', 'uis_predict', 'uis_predict_device', 'uis_predict_bounded',
            'uis_predict_device_bounded', 'uis_predict_nbest', 'uis_predict_device_nbest',
            'uis_score', 'uis_score_device', 'uis_predict_sweep', 'uis_predict_device_sweep', 'uis_score_sweep',
-           'uis_score_device_sweep', 'uis_predict_workspace_bytes', 'uis_get_stats', 'uis_trainer_create',
+           'uis_score_device_sweep', 'uis_score_device_ids', 'uis_predict_workspace_bytes', 'uis_get_stats', 'uis_trainer_create',
            'uis_trainer_destroy', 'uis_trainer_step', 'uis_trainer_get', 'uis_trainer_losses',
            'uis_trainer_comm_size', 'uis_trainer_comm_export', 'uis_trainer_comm_apply',
            'uis_trainer_set_corpus', 'uis_trainer_step_corpus')
@@ -183,6 +183,9 @@ def load_library():
   lib.uis_score_sweep.argtypes = lib.uis_score.argtypes + [C.POINTER(DecodeParams)]
   lib.uis_score_device_sweep.restype = C.c_int
   lib.uis_score_device_sweep.argtypes = lib.uis_score_device.argtypes + [C.POINTER(DecodeParams)]
+  lib.uis_score_device_ids.restype = C.c_int
+  lib.uis_score_device_ids.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(DecodeParams)]
   lib.uis_predict_workspace_bytes.restype = C.c_size_t
   lib.uis_predict_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.c_int,
                                               C.POINTER(PredictOpts)]
@@ -555,6 +558,19 @@ class NativeModel:
     _check(self._lib, self._lib.uis_score_device_sweep(
         self._h, C.c_void_p(x_ptr), off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1, C.c_void_p(labels_ptr),
         C.c_void_p(scores_ptr), C.c_void_p(frame_ptr), C.c_void_p(stream), C.byref(dp)))
+    del keep_dp
+
+  def score_device_ids(self, x_ptr, frame_offsets, ids_ptr, scores_ptr, decode_params, frame_ptr=0, labels_ptr=0,
+                       stream=0):
+    """Device-resident score sweep of arbitrary ids (uis_score_device_ids): ids_ptr -> int64 [rows], any values per
+    frame, renamed in order of first appearance per utterance on the device; scores_ptr -> float32 [C][U], frame_ptr ->
+    float32 [C][rows] (0 = none), labels_ptr -> int32 [rows] receives the canonical labels (0 = none).  Enqueues on
+    `stream` without reading anything back.  decode_params=None is the model's own pair (C = 1)."""
+    off = np.ascontiguousarray(frame_offsets, dtype=np.int64)
+    dp, keep_dp, _ = self._sweep(decode_params)
+    _check(self._lib, self._lib.uis_score_device_ids(
+        self._h, C.c_void_p(x_ptr), off.ctypes.data_as(C.POINTER(C.c_int64)), len(off) - 1, C.c_void_p(ids_ptr),
+        C.c_void_p(scores_ptr), C.c_void_p(frame_ptr), C.c_void_p(labels_ptr), C.c_void_p(stream), C.byref(dp)))
     del keep_dp
 
   def score_device(self, x_ptr, frame_offsets, labels_ptr, scores_ptr, frame_ptr=0, stream=0):

@@ -89,6 +89,73 @@ def _check_test_sequence(test_sequence, observation_dim):
     raise ValueError('test_sequence does not match the dimension specified by args.observation_dim.')
 
 
+_TENSOR_DTYPES = (torch.float32, torch.float16, torch.bfloat16, torch.float64)
+
+
+def _tensor_sequences(sequences, observation_dim, device):
+  """Whether a list of test sequences holds torch tensors (True) or not (False: the ndarray rules apply).  Tensors are
+  checked here: one dtype for the whole call, one of _TENSOR_DTYPES (TypeError), 2-D [N, observation_dim] (the
+  ValueErrors of _check_test_sequence) and on `device` (ValueError).  A list mixing tensors with anything else is a
+  TypeError."""
+  is_tensor = [isinstance(s, torch.Tensor) for s in sequences]
+  if not any(is_tensor):
+    return False
+  if not all(is_tensor):
+    raise TypeError('test_sequences must be all numpy arrays or all torch tensors, not a mix of both.')
+  dtypes = sorted({str(s.dtype) for s in sequences})
+  if len(dtypes) > 1:
+    raise TypeError('all test_sequence tensors of one call must share a dtype, got {}.'.format(', '.join(dtypes)))
+  if sequences[0].dtype not in _TENSOR_DTYPES:
+    raise TypeError('test_sequence tensors must be float32, float16, bfloat16 or float64, got {}.'.format(
+        sequences[0].dtype))
+  for sequence in sequences:
+    if sequence.ndim != 2:
+      raise ValueError('test_sequence must be 2-dim array.')
+    if sequence.shape[1] != observation_dim:
+      raise ValueError('test_sequence does not match the dimension specified by args.observation_dim.')
+    if sequence.device != device:
+      raise ValueError('test_sequence tensors must be on the model\'s device {}, got {}.'.format(device, sequence.device))
+  return True
+
+
+def _device_rows(tensors):
+  """(x, offsets) of checked tensors: one contiguous fp32 [rows, D] CUDA tensor (the caller's own when a single
+  contiguous fp32 tensor starting on a 16-byte boundary is given, else one cat + cast, float64 rounded to nearest) and
+  int64 frame offsets [U + 1].  The input projection reads the rows with float4 loads, so a view at an element offset
+  that is not a multiple of 4 is copied."""
+  offsets = np.zeros(len(tensors) + 1, np.int64)
+  np.cumsum([t.shape[0] for t in tensors], out=offsets[1:])
+  with torch.no_grad():
+    t0 = tensors[0] if len(tensors) == 1 else None
+    if t0 is not None and t0.dtype == torch.float32 and t0.is_contiguous() and t0.data_ptr() % 16 == 0:
+      x = t0.detach()
+    else:
+      x = torch.cat([t.detach() for t in tensors]).to(torch.float32).contiguous()
+  return x, offsets
+
+
+def _device_ids(test_cluster_ids, lengths, device):
+  """One contiguous int64 CUDA tensor [rows] of the label sequences of a tensor score() call: an integer tensor on
+  `device` is taken with its values as they are (any strides: a strided one is copied), a host sequence is renamed on
+  the host (canonical_labels: any hashable values) and uploaded."""
+  parts = []
+  for u, (ids, n) in enumerate(zip(test_cluster_ids, lengths)):
+    if isinstance(ids, torch.Tensor):
+      if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
+        raise TypeError('utterance {}: a label tensor must have an integer dtype, got {}'.format(u, ids.dtype))
+      if ids.device != device:
+        raise ValueError('utterance {}: the label tensor is on {}, the sequences on {}'.format(u, ids.device, device))
+      if ids.ndim != 1:
+        raise ValueError('a label sequence must be a 1-D sequence of labels')
+      part = ids.detach().to(torch.int64).contiguous()  # (an int64 tensor comes back as itself, strides included)
+    else:
+      part = torch.from_numpy(canonical_labels(ids).astype(np.int64)).to(device, non_blocking=True)
+    if part.shape[0] != n:
+      raise ValueError('utterance {}: {} labels for {} frames'.format(u, part.shape[0], n))
+    parts.append(part)
+  return torch.cat(parts) if len(parts) > 1 else parts[0]
+
+
 class _Fingerprint:
   """Parameter tensors (copied, or the live ones) and scalars, compared exactly: per device, one fused difference and
   one fused max-norm of the tensors there, and one device -> host copy."""
@@ -431,12 +498,15 @@ class UISRNN:
         self._native = ((self._fingerprint(), index), native.NativeModel(self.export_weights(), device=index))
       return self._native[1]
 
-  def _decode(self, sequences, args, bounds, n_best, pairs, as_arrays=False):
+  def _decode(self, sequences, args, bounds, n_best, pairs, as_arrays=False, tensors=False):
     """The one decode behind every predict entry point, of checked `sequences` under speaker `bounds` ((max, min) int32
     arrays from native.speaker_bounds, None = absent), `n_best` and `pairs` (checked (crp_alpha, transition_bias) pairs,
     None = the model's own).  Returns (hypotheses, speakers): hypotheses[c][u] is the NBest of utterance u under pair c
     with n_best, else its hypothesis 0's labels (an int32 array on CUDA with as_arrays, else a list of ints; empty for
-    an empty utterance); speakers[c][u] is the cluster count of hypothesis 0 (0 for an empty utterance)."""
+    an empty utterance); speakers[c][u] is the cluster count of hypothesis 0 (0 for an empty utterance).  With
+    `tensors` the sequences are CUDA tensors and so are the labels, scores and cluster counts of the hypotheses."""
+    if tensors:
+      return _native_decode_tensors(self._native_model(), sequences, args, bounds, n_best, pairs)
     if self.device.type == 'cuda':
       return _native_decode(self._native_model(), sequences, args, bounds, n_best, pairs, as_arrays)
     mx, mn = bounds
@@ -452,17 +522,20 @@ class UISRNN:
 
   def _predict(self, test_sequences, args, max_speakers, min_speakers, n_best, pairs):
     """predict() of an ndarray or a list, after decode_params was checked (pairs, None = none given)."""
-    single = isinstance(test_sequences, np.ndarray)
+    on_cuda = self.device.type == 'cuda'
+    single = isinstance(test_sequences, np.ndarray) or (on_cuda and isinstance(test_sequences, torch.Tensor))
     if not single and not isinstance(test_sequences, list):
       raise TypeError('test_sequences should be either a list or numpy array.')
     sequences = [test_sequences] if single else test_sequences
-    for sequence in sequences:
-      _check_test_sequence(sequence, self.observation_dim)
+    tensors = on_cuda and _tensor_sequences(sequences, self.observation_dim, self.device)
+    if not tensors:
+      for sequence in sequences:
+        _check_test_sequence(sequence, self.observation_dim)
     if single and (np.ndim(max_speakers) or np.ndim(min_speakers)):
       raise ValueError('predict_single takes one int per bound')
     k = _check_n_best(n_best, args) if n_best is not None else None
     bounds = _speaker_bounds(len(sequences), max_speakers, min_speakers)
-    hyps, speakers = self._decode(sequences, args, bounds, k, pairs)
+    hyps, speakers = self._decode(sequences, args, bounds, k, pairs, tensors=tensors)
     _warn_min_speakers([len(s) for s in sequences], speakers, bounds[1], pairs is not None, stacklevel=4)
     out = [row[0] for row in hyps] if single else hyps
     return out if pairs is not None else out[0]
@@ -471,8 +544,9 @@ class UISRNN:
     """Labels (list of N ints) for one test sequence [N, D] float64 (uisrnn.py:479-562).
 
     max_speakers / min_speakers (ints, 0 or None = no bound) bound the number of speakers, and n_best returns
-    an NBest instead: see `predict`."""
-    _check_test_sequence(test_sequence, self.observation_dim)
+    an NBest instead; a CUDA model also takes a torch tensor: see `predict`."""
+    if not (self.device.type == 'cuda' and isinstance(test_sequence, torch.Tensor)):
+      _check_test_sequence(test_sequence, self.observation_dim)
     return self._predict(test_sequence, args, max_speakers, min_speakers, n_best, None)
 
   def predict(self, test_sequences, args, *, max_speakers=None, min_speakers=None, n_best=None, decode_params=None):
@@ -499,7 +573,17 @@ class UISRNN:
     with one entry per pair, entry c being exactly what this call returns without `decode_params` for a model whose
     crp_alpha / transition_bias are pair c (bounds and n_best apply to every pair).  The model is not changed.  On a
     CUDA device the whole grid is one native call: the inputs are copied and projected once.  Pick a pair by scoring
-    each entry on a labelled dev set (e.g. `evals.compute_sequence_match_accuracy`)."""
+    each entry on a labelled dev set (e.g. `evals.compute_sequence_match_accuracy`).
+
+    Inputs already on the GPU (not in the reference): a CUDA model also takes a torch tensor [N, D] or a list of them,
+    on the model's device, all float32, all float16, all bfloat16 or all float64 (any strides; requires_grad is
+    ignored).  A list mixing tensors with ndarrays, or mixing dtypes, is a TypeError.  The rows are cast to float32 on
+    the device (float64 rounds to nearest as the ndarray path's cast does, so the same values decode bit for bit either
+    way; float16 / bfloat16 decode as their exact float64 upcast would) and decoded on torch's current stream of the
+    device, with nothing crossing the bus but the per-utterance counts the call reads back when it ends.  Every
+    utterance then gives an int64 CUDA tensor [N] of labels instead of a list, and with n_best an NBest of CUDA tensors:
+    labels int64 [n, N], scores float32 [n], speakers int32 [n], for the n hypotheses returned.  Bounds and
+    decode_params behave as for ndarrays.  A CPU model raises the reference's TypeError for tensors."""
     pairs = _decode_params(decode_params) if decode_params is not None else None
     return self._predict(test_sequences, args, max_speakers, min_speakers, n_best, pairs)
 
@@ -518,8 +602,19 @@ class UISRNN:
 
     With `decode_params` (a non-empty sequence of (crp_alpha, transition_bias) pairs, validated as in `predict`) the
     result is a list with one entry per pair, each being what this call returns for a model with that pair.  On a CUDA
-    device the GRU work is done once for all pairs."""
+    device the GRU work is done once for all pairs.
+
+    Inputs already on the GPU: a CUDA model also takes torch tensors as `predict` does (same rules and casts).  Their
+    label sequences may be integer CUDA tensors [N] on the same device (any integer dtype and any values, negative and
+    beyond 32 bits included: they are renamed in order of first appearance on the device) or host label sequences as
+    above.  A list of tensors then gives a float32 CUDA tensor [U] of scores, a single tensor a 0-d one, and
+    decode_params a list of such tensors, one per pair; with per_frame every utterance gives a FrameScores of a 0-d total
+    and float32 [N] increments.  The scores equal those of the ndarray call bit for bit.  The call enqueues its work on
+    torch's current stream of the device and returns without waiting for it."""
     pairs = _decode_params(decode_params) if decode_params is not None else None
+    if self.device.type == 'cuda' and isinstance(test_sequences, torch.Tensor):
+      out = self.score([test_sequences], [test_cluster_ids], per_frame=per_frame, decode_params=pairs)
+      return out[0] if pairs is None else [entry[0] for entry in out]
     if isinstance(test_sequences, np.ndarray):
       out = self.score([test_sequences], [test_cluster_ids], per_frame=per_frame, decode_params=pairs)
       return out[0] if pairs is None else [entry[0] for entry in out]
@@ -529,6 +624,8 @@ class UISRNN:
       raise TypeError('test_cluster_ids should be a list with one label sequence per sequence.')
     if len(test_cluster_ids) != len(test_sequences):
       raise ValueError('{} sequences but {} label sequences'.format(len(test_sequences), len(test_cluster_ids)))
+    if self.device.type == 'cuda' and _tensor_sequences(test_sequences, self.observation_dim, self.device):
+      return self._score_tensors(test_sequences, test_cluster_ids, per_frame, pairs)
     for sequence in test_sequences:
       _check_test_sequence(sequence, self.observation_dim)
     labels = [canonical_labels(ids) for ids in test_cluster_ids]
@@ -548,6 +645,23 @@ class UISRNN:
         decoder = beam_cpu.CpuBeamSearch(self, crp_alpha=alpha, transition_bias=bias)
         out = [decoder.score(sequence, lab) for sequence, lab in zip(test_sequences, labels)]
         result.append([FrameScores(float(t), inc) for t, inc in out] if per_frame else [float(t) for t, _ in out])
+    return result if pairs is not None else result[0]
+
+  def _score_tensors(self, sequences, test_cluster_ids, per_frame, pairs):
+    """score() of a list of checked CUDA tensors: one uis_score_device_ids call on torch's current stream, outputs
+    allocated by torch on that stream, no synchronisation."""
+    x, offsets = _device_rows(sequences)
+    ids = _device_ids(test_cluster_ids, np.diff(offsets), self.device)
+    n, rows, configs = len(sequences), int(offsets[-1]), 1 if pairs is None else len(pairs)
+    scores = torch.empty((configs, n), dtype=torch.float32, device=self.device)
+    frames = torch.empty((configs, rows), dtype=torch.float32, device=self.device) if per_frame else None
+    model = self._native_model()
+    with model.lock:
+      model.score_device_ids(x.data_ptr(), offsets, ids.data_ptr(), scores.data_ptr(), pairs,
+                             frame_ptr=frames.data_ptr() if per_frame else 0,
+                             stream=torch.cuda.current_stream(self.device).cuda_stream)
+    result = [[FrameScores(scores[c, u], frames[c, offsets[u]:offsets[u + 1]]) for u in range(n)] if per_frame else
+              scores[c] for c in range(configs)]
     return result if pairs is not None else result[0]
 
 
@@ -594,26 +708,66 @@ def _check_n_best(n_best, args):
 def _native_decode(model, sequences, args, bounds, n_best, pairs, as_arrays=False):
   """UISRNN._decode on a NativeModel: one NativeModel.predict_sweep call, repeated with larger device tables (kcap)
   while a hypothesis opens more clusters than they hold (UIS_ERR_OVERFLOW)."""
-  from . import native
   mx, mn = bounds
-  kcap = _DEFAULT_KCAP
-  while True:
-    try:
-      with model.lock:  # a uis_model handle (one workspace) is not re-entrant
-        labels, scores, speakers, count = model.predict_sweep(
-            sequences, pairs, beam_size=args.beam_size, look_ahead=args.look_ahead,
-            test_iteration=args.test_iteration, kcap=kcap, max_speakers=mx, min_speakers=mn, n_best=n_best)
-      break
-    except native.NativeError as err:
-      if err.code != native.UIS_ERR_OVERFLOW or kcap >= 1024:
-        raise
-      kcap = 32 if kcap == 0 else kcap * 2
+  labels, scores, speakers, count = _grow_kcap(model, lambda kcap: model.predict_sweep(
+      sequences, pairs, beam_size=args.beam_size, look_ahead=args.look_ahead, test_iteration=args.test_iteration,
+      kcap=kcap, max_speakers=mx, min_speakers=mn, n_best=n_best))
   if n_best is None:  # hypothesis 0's labels: label plane 0, which an empty utterance leaves empty
     hyps = [[lab[c, 0] if as_arrays else lab[c, 0].tolist() for lab in labels] for c in range(len(count))]
   else:
     hyps = [[NBest(lab[c, :n].tolist(), s[:n], k[:n]) for lab, s, k, n in zip(labels, sc, sp, cn)]
             for c, (sc, sp, cn) in enumerate(zip(scores.tolist(), speakers.tolist(), count.tolist()))]
   return hyps, speakers[:, :, 0]
+
+
+def _grow_kcap(model, decode):
+  """decode(kcap) under the model's lock, repeated with larger device tables (kcap) while a hypothesis opens more
+  clusters than they hold (UIS_ERR_OVERFLOW)."""
+  from . import native
+  kcap = _DEFAULT_KCAP
+  while True:
+    try:
+      with model.lock:  # a uis_model handle (one workspace) is not re-entrant
+        return decode(kcap)
+    except native.NativeError as err:
+      if err.code != native.UIS_ERR_OVERFLOW or kcap >= 1024:
+        raise
+      kcap = 32 if kcap == 0 else kcap * 2
+
+
+def _native_decode_tensors(model, tensors, args, bounds, n_best, pairs):
+  """_native_decode of checked CUDA tensors: one uis_predict_device_sweep call on torch's current stream into outputs
+  torch allocates there, then one synchronisation (NativeModel.stats raises what a job's status reports, e.g. the
+  overflow that grows kcap).  Only the [C][U] hypothesis and cluster counts come back to the host."""
+  x, offsets = _device_rows(tensors)
+  device = x.device
+  n, rows, configs = len(tensors), int(offsets[-1]), 1 if pairs is None else len(pairs)
+  k = n_best or 1
+  labels = torch.empty((configs, k, rows), dtype=torch.int32, device=device)
+  scores = torch.empty((configs, max(n, 1), k), dtype=torch.float32, device=device)
+  speakers = torch.empty((configs, max(n, 1), k), dtype=torch.int32, device=device)
+  count = torch.empty((configs, max(n, 1)), dtype=torch.int32, device=device)
+  stream = torch.cuda.current_stream(device).cuda_stream
+  mx, mn = bounds
+
+  def decode(kcap):
+    model.predict_device_sweep(x.data_ptr(), offsets, labels.data_ptr(), scores.data_ptr(), pairs,
+                               beam_size=args.beam_size, look_ahead=args.look_ahead,
+                               test_iteration=args.test_iteration, kcap=kcap, stream=stream, max_speakers=mx,
+                               min_speakers=mn, n_best=k, speakers_ptr=speakers.data_ptr(), count_ptr=count.data_ptr())
+    model.stats()
+
+  _grow_kcap(model, decode)
+  labels = labels.to(torch.int64)
+  counts = count[:, :n].cpu().numpy()
+  spk0 = speakers[:, :n, 0].cpu().numpy()
+  spans = [(int(offsets[u]), int(offsets[u + 1])) for u in range(n)]
+  if n_best is None:
+    hyps = [[labels[c, 0, a:b] for a, b in spans] for c in range(configs)]
+  else:
+    hyps = [[NBest(labels[c, :m, a:b], scores[c, u, :m], speakers[c, u, :m])
+             for u, ((a, b), m) in enumerate(zip(spans, counts[c].tolist()))] for c in range(configs)]
+  return hyps, spk0
 
 
 def _decode_task(model, args, n_best, sequence, max_speakers, min_speakers):
