@@ -399,6 +399,33 @@ int uis_trainer_set_corpus(uis_trainer* t, const double* rows, int64_t n_rows, c
 int uis_trainer_step_corpus(uis_trainer* t, const int32_t* chosen, int B, int mode, float* losses_out, void* stream);
 
 /*
+ * Training set read in place from device memory (same ABI version 7; additive).  Instead of a float64 host copy,
+ *   row_addr  device array of n_rows row addresses: row r is D elements of `dtype` in unit element stride starting at
+ *             row_addr[r], aligned to the element size (no wider alignment is assumed; rows may overlap or repeat).
+ *   dtype     one of uis_dtype.
+ * index, offsets and n_sub are those of uis_trainer_set_corpus and are checked the same way on the host.  Null
+ * pointers, an unknown dtype, inconsistent sizes or an index out of range give UIS_ERR_INVALID before any device work.
+ * The trainer keeps no copy of the rows: every later uis_trainer_step_corpus gathers its batch from row_addr and
+ * the rows it points to, converting each element to fp32 (float64 rounds to nearest, as uis_trainer_set_corpus's
+ * cast does; float16 and bfloat16 convert exactly).  So the table and the rows must stay allocated and unchanged
+ * until the next uis_trainer_set_corpus* call or uis_trainer_destroy, and a step reads what they hold when its
+ * gather runs on its stream.  The trainer's initialisation (uis_trainer_create) and the index upload run on the legacy
+ * default stream; `stream` is made to wait for them on an event, so steps on any stream, non-blocking ones included,
+ * start after them, and the call does not wait for earlier work on `stream`.  An fp32 corpus of an earlier
+ * uis_trainer_set_corpus is freed (cudaFree, which may synchronise the device).
+ */
+typedef enum uis_dtype {
+  UIS_DTYPE_F32 = 0,
+  UIS_DTYPE_F16 = 1,
+  UIS_DTYPE_BF16 = 2,
+  UIS_DTYPE_F64 = 3
+} uis_dtype;
+
+int uis_trainer_set_corpus_device(uis_trainer* t, const void* const* row_addr, int32_t dtype, int64_t n_rows,
+                                  const int32_t* index, int64_t n_index, const int64_t* offsets, int32_t n_sub,
+                                  void* stream);
+
+/*
  * Data-parallel fit() (optional; SURVEY.md 8(e)): every rank runs uis_trainer_step(mode = 2) on its
  * shard of the mini-batch (forward + backward with UN-normalised gradients), exports
  *   [gradients of all parameters but sigma2 | per-dimension squared-residual sums | per-dimension counts | row count]

@@ -11,6 +11,8 @@
 // All arithmetic fp32.  The derivation of the backward pass is checked against torch autograd in
 // tools/fit_manual_check.py (CPU) and tests/test_gpu_fit.py (device).
 #include <cooperative_groups.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -756,18 +758,30 @@ __global__ void scale_by_inv_kernel(float* __restrict__ g, const float* __restri
   if (i < n) g[i] = g[i] / nz[0];
 }
 
-// Corpus path (fit() host data prep on the device, SURVEY 8(f) f1): the training set lives on the device as
-// fp32 rows; a mini-batch is a gather.  x[t][b][:] = 0 for t = 0 (the prepended zero frame, utils.py:243) and
-// for t >= length_b (padding), else rows[index[begin_b + t - 1]][:].
+// Corpus path (fit() host data prep on the device, SURVEY 8(f) f1): a mini-batch is a gather of training rows.
+// x[t][b][:] = 0 for t = 0 (the prepended zero frame, utils.py:243) and for t >= length_b (padding), else row
+// index[begin_b + t - 1] converted to fp32.  The rows are either the trainer's own fp32 corpus (T = float,
+// kTable = false: row r at rows + r * D) or the caller's rows read in place in their dtype (kTable = true: `rows` is
+// a device table of row addresses, row r at ((const T* const*)rows)[r]).  Elements are loaded one by one, so a row
+// needs only the alignment of T.
 struct GatherCols { long long begin[32]; int length[32]; };
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(double v) { return __double2float_rn(v); }  // = torch .float()
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }       // exact
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }  // exact
 // columns [b0, b0 + nbg) of a batch B columns wide; grid = L * nbg
-__global__ void gather_batch_kernel(const float* __restrict__ rows, const int* __restrict__ index, GatherCols cols,
+template <typename T, bool kTable>
+__global__ void gather_batch_kernel(const void* __restrict__ rows, const int* __restrict__ index, GatherCols cols,
                                     float* __restrict__ x, int nbg, int b0, int B, int D) {
   const int tt = blockIdx.x / nbg, bl = blockIdx.x % nbg;
   float* dst = x + ((size_t)tt * B + b0 + bl) * D;
   const bool live = tt >= 1 && tt < cols.length[bl];
-  const float* src = live ? rows + (size_t)index[cols.begin[bl] + tt - 1] * D : nullptr;
-  for (int i = threadIdx.x; i < D; i += blockDim.x) dst[i] = live ? src[i] : 0.f;
+  const T* src = nullptr;
+  if (live) {
+    const int r = index[cols.begin[bl] + tt - 1];
+    src = kTable ? static_cast<const T* const*>(rows)[r] : static_cast<const T*>(rows) + (size_t)r * D;
+  }
+  for (int i = threadIdx.x; i < D; i += blockDim.x) dst[i] = live ? to_f32(src[i]) : 0.f;
 }
 
 // Inter-layer dropout of the stacked GRU in train mode (nn.GRU(dropout=p), uisrnn.py:39-41): element i of the output
@@ -899,8 +913,13 @@ struct uis_trainer {
   cudaEvent_t pin_ev[2] = {nullptr, nullptr};
   int pin_idx = 0;
   int seq_mode = -1;  // -1 unknown, 0 per-step launches, 1 persistent cooperative kernels
-  // corpus path: training rows (fp32) + flat gather indices + per-sub-sequence offsets (host copy)
+  // corpus path: training rows (fp32) + flat gather indices + per-sub-sequence offsets (host copy).  After
+  // uis_trainer_set_corpus_device the rows are the caller's, read in place through the device table row_addr
+  // (corpus is then empty).
   uis::DBuf corpus;
+  const void* const* row_addr = nullptr;
+  int row_dtype = UIS_DTYPE_F32;
+  cudaEvent_t legacy_done = nullptr;  // set_corpus_device: the caller's stream waits for the legacy-stream work
   int* corpus_index = nullptr;
   long long corpus_rows = 0;
   std::vector<long long> sub_off;
@@ -1031,6 +1050,7 @@ int uis_trainer_destroy(uis_trainer* t) {
   if (t->sc.colsum_tickets) cudaFree(t->sc.colsum_tickets);
   if (t->corpus_index) cudaFree(t->corpus_index);
   t->corpus.release();
+  if (t->legacy_done) cudaEventDestroy(t->legacy_done);
   for (int i = 0; i < 2; ++i) {
     if (t->pin[i]) cudaFreeHost(t->pin[i]);
     if (t->pin_ev[i]) cudaEventDestroy(t->pin_ev[i]);
@@ -1093,15 +1113,23 @@ int uis_trainer_step(uis_trainer* t, const float* x_host, const int32_t* lengths
 // Training set on the device: rows [n_rows][D] float64 host (cast to fp32 on the device, as the reference's
 // torch.from_numpy(...).float() does per batch, utils.py:245), index = the concatenated row indices of every
 // sub-sequence of utils.resize_sequence, offsets[n_sub + 1] its prefix sums.
-int uis_trainer_set_corpus(uis_trainer* t, const double* rows, int64_t n_rows, const int32_t* index, int64_t n_index,
-                           const int64_t* offsets, int32_t n_sub) {
-  if (!t || !rows || !index || !offsets) return uis::api_fail(UIS_ERR_INVALID, "null argument");
+namespace {
+// The host-side checks both set_corpus entry points make of the gather plan.
+int check_corpus(int64_t n_rows, const int32_t* index, int64_t n_index, const int64_t* offsets, int32_t n_sub) {
   if (n_rows < 1 || n_sub < 1 || n_index < 0 || offsets[0] != 0 || offsets[n_sub] != n_index)
     return uis::api_fail(UIS_ERR_INVALID, "inconsistent corpus sizes");
   for (int64_t i = 0; i < n_index; ++i)
     if (index[i] < 0 || index[i] >= n_rows) return uis::api_fail(UIS_ERR_INVALID, "corpus index out of range");
   for (int32_t k = 0; k < n_sub; ++k)
     if (offsets[k + 1] < offsets[k]) return uis::api_fail(UIS_ERR_INVALID, "corpus offsets must be non-decreasing");
+  return 0;
+}
+}  // namespace
+
+int uis_trainer_set_corpus(uis_trainer* t, const double* rows, int64_t n_rows, const int32_t* index, int64_t n_index,
+                           const int64_t* offsets, int32_t n_sub) {
+  if (!t || !rows || !index || !offsets) return uis::api_fail(UIS_ERR_INVALID, "null argument");
+  if (int rc = check_corpus(n_rows, index, n_index, offsets, n_sub)) return rc;
   uis::DeviceGuard device_guard_(t->device);
   CUT(device_guard_.status);
   const size_t n = (size_t)n_rows * t->D;
@@ -1122,6 +1150,36 @@ int uis_trainer_set_corpus(uis_trainer* t, const double* rows, int64_t n_rows, c
   if (t->corpus_index) { cudaFree(t->corpus_index); t->corpus_index = nullptr; }
   CUT(cudaMalloc(&t->corpus_index, std::max<size_t>(1, (size_t)n_index) * sizeof(int)));
   CUT(cudaMemcpy(t->corpus_index, index, (size_t)n_index * sizeof(int), cudaMemcpyHostToDevice));
+  t->corpus_rows = n_rows;
+  t->row_addr = nullptr;
+  t->sub_off.assign(offsets, offsets + n_sub + 1);
+  return 0;
+}
+
+// Training set left where the caller holds it: row r is D elements of `dtype` at the device address row_addr[r]
+// (row_addr: a device table of n_rows addresses), read in place by every later uis_trainer_step_corpus.  index and
+// offsets as in uis_trainer_set_corpus.  uis_trainer_create initialises the trainer on the legacy default stream and
+// the index goes up there too; `stream` (which may be a non-blocking stream) waits for that work on an event, so
+// neither the host nor the legacy stream waits for earlier work on `stream`.
+int uis_trainer_set_corpus_device(uis_trainer* t, const void* const* row_addr, int32_t dtype, int64_t n_rows,
+                                  const int32_t* index, int64_t n_index, const int64_t* offsets, int32_t n_sub,
+                                  void* stream) {
+  if (!row_addr || !index || !offsets) return uis::api_fail(UIS_ERR_INVALID, "null argument");
+  if (dtype < UIS_DTYPE_F32 || dtype > UIS_DTYPE_F64) return uis::api_fail(UIS_ERR_INVALID, "unknown dtype %d", dtype);
+  if (int rc = check_corpus(n_rows, index, n_index, offsets, n_sub)) return rc;
+  if (!t) return uis::api_fail(UIS_ERR_INVALID, "trainer is NULL");
+  uis::DeviceGuard device_guard_(t->device);
+  CUT(device_guard_.status);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  t->corpus.release();  // (cudaFree waits for the steps that may still read an earlier corpus)
+  if (t->corpus_index) { cudaFree(t->corpus_index); t->corpus_index = nullptr; }
+  CUT(cudaMalloc(&t->corpus_index, std::max<size_t>(1, (size_t)n_index) * sizeof(int)));
+  CUT(cudaMemcpyAsync(t->corpus_index, index, (size_t)n_index * sizeof(int), cudaMemcpyHostToDevice, cudaStreamLegacy));
+  if (!t->legacy_done) CUT(cudaEventCreateWithFlags(&t->legacy_done, cudaEventDisableTiming));
+  CUT(cudaEventRecord(t->legacy_done, cudaStreamLegacy));
+  CUT(cudaStreamWaitEvent(st, t->legacy_done, 0));
+  t->row_addr = row_addr;
+  t->row_dtype = dtype;
   t->corpus_rows = n_rows;
   t->sub_off.assign(offsets, offsets + n_sub + 1);
   return 0;
@@ -1204,7 +1262,18 @@ int run_iteration(uis_trainer* t, const int32_t* lengths, int B, int L, int mode
       const int b0 = 32 * g, nbg = std::min(32, B - b0);
       GatherCols cols{};
       for (int b = 0; b < nbg; ++b) { cols.begin[b] = col_begin[b0 + b]; cols.length[b] = lengths[b0 + b]; }
-      gather_batch_kernel<<<(unsigned)(L * nbg), 128, 0, st>>>(t->corpus.p, t->corpus_index, cols, t->x.p, nbg, b0, B, D);
+      const dim3 grid((unsigned)(L * nbg));
+      const void* rows = t->row_addr;
+      if (!t->row_addr)
+        gather_batch_kernel<float, false><<<grid, 128, 0, st>>>(t->corpus.p, t->corpus_index, cols, t->x.p, nbg, b0, B, D);
+      else if (t->row_dtype == UIS_DTYPE_F32)
+        gather_batch_kernel<float, true><<<grid, 128, 0, st>>>(rows, t->corpus_index, cols, t->x.p, nbg, b0, B, D);
+      else if (t->row_dtype == UIS_DTYPE_F16)
+        gather_batch_kernel<__half, true><<<grid, 128, 0, st>>>(rows, t->corpus_index, cols, t->x.p, nbg, b0, B, D);
+      else if (t->row_dtype == UIS_DTYPE_BF16)
+        gather_batch_kernel<__nv_bfloat16, true><<<grid, 128, 0, st>>>(rows, t->corpus_index, cols, t->x.p, nbg, b0, B, D);
+      else
+        gather_batch_kernel<double, true><<<grid, 128, 0, st>>>(rows, t->corpus_index, cols, t->x.p, nbg, b0, B, D);
     }
     CUT(cudaGetLastError());
   } else {  // stage the batch in pinned memory: the H2D copy then overlaps the previous iteration's kernels

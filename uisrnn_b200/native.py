@@ -77,7 +77,10 @@ EXPORTS = ('uis_version', 'uis_last_error', 'uis_model_create', 'uis_model_destr
            'uis_score_device_sweep', 'uis_score_device_ids', 'uis_predict_workspace_bytes', 'uis_get_stats', 'uis_trainer_create',
            'uis_trainer_destroy', 'uis_trainer_step', 'uis_trainer_get', 'uis_trainer_losses',
            'uis_trainer_comm_size', 'uis_trainer_comm_export', 'uis_trainer_comm_apply',
-           'uis_trainer_set_corpus', 'uis_trainer_step_corpus')
+           'uis_trainer_set_corpus', 'uis_trainer_step_corpus', 'uis_trainer_set_corpus_device')
+
+# uis_dtype: the element types uis_trainer_set_corpus_device reads
+UIS_DTYPE_F32, UIS_DTYPE_F16, UIS_DTYPE_BF16, UIS_DTYPE_F64 = 0, 1, 2, 3
 
 
 class TrainHParams(C.Structure):
@@ -207,6 +210,9 @@ def load_library():
   lib.uis_trainer_set_corpus.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32]
   lib.uis_trainer_step_corpus.restype = C.c_int
   lib.uis_trainer_step_corpus.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, fp, C.c_void_p]
+  lib.uis_trainer_set_corpus_device.restype = C.c_int
+  lib.uis_trainer_set_corpus_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int64,
+                                                C.c_void_p, C.c_int32, C.c_void_p]
   lib.uis_trainer_comm_size.restype = C.c_int64
   lib.uis_trainer_comm_size.argtypes = [C.c_void_p]
   lib.uis_trainer_comm_export.restype = C.c_int
@@ -586,6 +592,14 @@ class NativeModel:
     return s.as_dict()
 
 
+def _gather_plan(index_lists):
+  """(flat int32 row indices of every sub-sequence back to back, int64 offsets [n_sub + 1]) for set_corpus*."""
+  offsets = np.zeros(len(index_lists) + 1, np.int64)
+  np.cumsum([len(ix) for ix in index_lists], out=offsets[1:])
+  flat = (np.concatenate(index_lists) if len(index_lists) else np.zeros(0)).astype(np.int32)
+  return flat, offsets
+
+
 class NativeTrainer:
   """Owns a `uis_trainer*`: parameters, gradients and Adam state of one fit_concatenated call live
   on the device; `step()` runs one iteration on a host batch.  `params`: dict name -> ndarray in
@@ -607,12 +621,14 @@ class NativeTrainer:
                       float(hparams['sigma_beta']), float(hparams['regularization_weight']),
                       float(hparams['grad_max_norm']), int(bool(hparams['train_sigma2'])), self.depth,
                       float(hparams.get('rnn_dropout', 0.0) or 0.0), int(hparams.get('dropout_seed', 0) or 0))
+    self._corpus = None
     _check(lib, lib.uis_trainer_create(C.byref(self._h), device, self.D, self.H, ptrs, C.byref(hp)))
 
   def close(self):
     if getattr(self, '_h', None) is not None and self._h:
       self._lib.uis_trainer_destroy(self._h)
       self._h = C.c_void_p()
+    self._corpus = None  # the rows a set_corpus_device left the trainer reading
 
   def __del__(self):
     try:
@@ -632,12 +648,37 @@ class NativeTrainer:
     sub-sequence (utils.resize_indices).  Everything is copied to the device once."""
     rows = np.ascontiguousarray(rows, dtype=np.float64)
     assert rows.ndim == 2 and rows.shape[1] == self.D
-    offsets = np.zeros(len(index_lists) + 1, np.int64)
-    np.cumsum([len(ix) for ix in index_lists], out=offsets[1:])
-    flat = (np.concatenate(index_lists) if len(index_lists) else np.zeros(0)).astype(np.int32)
+    flat, offsets = _gather_plan(index_lists)
     _check(self._lib, self._lib.uis_trainer_set_corpus(
         self._h, rows.ctypes.data_as(C.c_void_p), rows.shape[0], flat.ctypes.data_as(C.c_void_p), len(flat),
         offsets.ctypes.data_as(C.c_void_p), len(index_lists)))
+    self._corpus = None
+
+  def set_corpus_device(self, tensors, index_lists, stream=0):
+    """tensors: torch CUDA tensors [N_i, D] on the trainer's device, all float32, float16, bfloat16 or float64, any strides;
+    row indices refer to their rows back to back.  The trainer reads the rows in place at every step_corpus, so they
+    must not change until close() or the next set_corpus*.  The row-address table (8 bytes per row) is built by torch
+    on the current stream; a tensor whose elements are not in unit stride is made contiguous first.  This object keeps
+    the tensors, those copies and the table alive until then."""
+    import torch
+    code = {torch.float32: UIS_DTYPE_F32, torch.float16: UIS_DTYPE_F16, torch.bfloat16: UIS_DTYPE_BF16,
+            torch.float64: UIS_DTYPE_F64}[tensors[0].dtype]
+    with torch.no_grad():
+      rows = [t.detach() if t.shape[1] == 1 or t.stride(1) == 1 else t.detach().contiguous() for t in tensors]
+      device = rows[0].device
+      n = sum(r.shape[0] for r in rows)
+      # (from pinned memory, so the copy is ordered on the current stream without the host waiting for that stream)
+      meta = torch.tensor([[r.data_ptr(), r.stride(0) * r.element_size(), r.shape[0]] for r in rows],
+                          dtype=torch.int64).pin_memory().to(device, non_blocking=True)
+      # address of row j of utterance u = base_u + (j - first row of u) * row stride_u
+      utt = torch.repeat_interleave(torch.arange(len(rows), device=device), meta[:, 2], output_size=n)
+      first = torch.cumsum(meta[:, 2], 0) - meta[:, 2]
+      table = meta[utt, 0] + (torch.arange(n, device=device) - first[utt]) * meta[utt, 1]
+    flat, offsets = _gather_plan(index_lists)
+    _check(self._lib, self._lib.uis_trainer_set_corpus_device(
+        self._h, C.c_void_p(table.data_ptr()), code, n, flat.ctypes.data_as(C.c_void_p), len(flat),
+        offsets.ctypes.data_as(C.c_void_p), len(index_lists), C.c_void_p(stream)))
+    self._corpus = (rows, table, meta)
 
   def step_corpus(self, chosen, mode=0, want_losses=False, stream=0):
     """One iteration on sub-sequences `chosen` (ids in column order, lengths descending).  mode as in

@@ -92,30 +92,47 @@ def _check_test_sequence(test_sequence, observation_dim):
 _TENSOR_DTYPES = (torch.float32, torch.float16, torch.bfloat16, torch.float64)
 
 
-def _tensor_sequences(sequences, observation_dim, device):
-  """Whether a list of test sequences holds torch tensors (True) or not (False: the ndarray rules apply).  Tensors are
+def _tensor_sequences(sequences, observation_dim, device, name='test_sequence'):
+  """Whether a list of sequences holds torch tensors (True) or not (False: the ndarray rules apply).  Tensors are
   checked here: one dtype for the whole call, one of _TENSOR_DTYPES (TypeError), 2-D [N, observation_dim] (the
   ValueErrors of _check_test_sequence) and on `device` (ValueError).  A list mixing tensors with anything else is a
-  TypeError."""
+  TypeError.  `name` is the argument the messages name (test_sequence or train_sequence)."""
   is_tensor = [isinstance(s, torch.Tensor) for s in sequences]
   if not any(is_tensor):
     return False
   if not all(is_tensor):
-    raise TypeError('test_sequences must be all numpy arrays or all torch tensors, not a mix of both.')
+    raise TypeError('{}s must be all numpy arrays or all torch tensors, not a mix of both.'.format(name))
   dtypes = sorted({str(s.dtype) for s in sequences})
   if len(dtypes) > 1:
-    raise TypeError('all test_sequence tensors of one call must share a dtype, got {}.'.format(', '.join(dtypes)))
+    raise TypeError('all {} tensors of one call must share a dtype, got {}.'.format(name, ', '.join(dtypes)))
   if sequences[0].dtype not in _TENSOR_DTYPES:
-    raise TypeError('test_sequence tensors must be float32, float16, bfloat16 or float64, got {}.'.format(
-        sequences[0].dtype))
+    raise TypeError('{} tensors must be float32, float16, bfloat16 or float64, got {}.'.format(
+        name, sequences[0].dtype))
   for sequence in sequences:
     if sequence.ndim != 2:
-      raise ValueError('test_sequence must be 2-dim array.')
+      raise ValueError('{} must be 2-dim array.'.format(name))
     if sequence.shape[1] != observation_dim:
-      raise ValueError('test_sequence does not match the dimension specified by args.observation_dim.')
+      raise ValueError('{} does not match the dimension specified by args.observation_dim.'.format(name))
     if sequence.device != device:
-      raise ValueError('test_sequence tensors must be on the model\'s device {}, got {}.'.format(device, sequence.device))
+      raise ValueError('{} tensors must be on the model\'s device {}, got {}.'.format(name, device, sequence.device))
   return True
+
+
+def _fit_labels(train_cluster_ids, lengths, device):
+  """The label sequences of a fit from tensors, on the host: every integer tensor [N] on `device` (any integer dtype and
+  strides) becomes the list of str(v) of its values v (utils.host_labels, one read-back for all of them); host label
+  sequences are kept for utils.concatenate_training_data to check.  A label tensor of another dtype is a TypeError, of
+  another shape, length or device a ValueError."""
+  if not isinstance(train_cluster_ids, list):
+    return train_cluster_ids  # (concatenate_training_data raises the reference's TypeError)
+  for u, ids in enumerate(train_cluster_ids):
+    if isinstance(ids, torch.Tensor) and ids.device != device:
+      raise ValueError('utterance {}: the label tensor is on {}, the sequences on {}'.format(u, ids.device, device))
+  labels = utils.host_labels(train_cluster_ids)  # (dtype and shape checks)
+  for u, (ids, n) in enumerate(zip(train_cluster_ids, lengths)):
+    if isinstance(ids, torch.Tensor) and ids.shape[0] != n:
+      raise ValueError('utterance {}: {} labels for {} frames'.format(u, ids.shape[0], n))
+  return labels
 
 
 def _device_rows(tensors):
@@ -269,7 +286,25 @@ class UISRNN:
     """Trains on one concatenated sequence `train_sequence` [N, D] (float64) with string labels
     `train_cluster_id` [N] (uisrnn.py:172-313): per iteration a random batch of per-speaker
     sub-sequences, running-mean prediction, weighted-MSE + sigma^2 prior + norm regulariser,
-    clipped Adam step, sigma^2 >= 1e-6."""
+    clipped Adam step, sigma^2 >= 1e-6.
+
+    A CUDA model also takes a torch tensor [N, D] on its device with an integer label tensor [N] or host labels: see
+    `fit`."""
+    if self.device.type == 'cuda' and isinstance(train_sequence, torch.Tensor):
+      _tensor_sequences([train_sequence], self.observation_dim, self.device, 'train_sequence')
+      self._require_device_trainer(args)
+      train_cluster_id = _fit_labels([train_cluster_id], [train_sequence.shape[0]], self.device)[0]
+      if isinstance(train_cluster_id, list):
+        train_cluster_id = np.array(train_cluster_id)
+      if (not isinstance(train_cluster_id, np.ndarray) or
+          not train_cluster_id.dtype.name.startswith(('str', 'unicode'))):
+        raise TypeError('train_cluster_id type be a numpy array of strings.')
+      if train_cluster_id.ndim != 1:
+        raise ValueError('train_cluster_id must be 1-dim array.')
+      if train_sequence.shape[0] != len(train_cluster_id):
+        raise ValueError('train_sequence length is not equal to train_cluster_id length.')
+      self._fit_tensors([train_sequence], train_cluster_id, args)
+      return
     if not isinstance(train_sequence, np.ndarray) or train_sequence.dtype != float:
       raise TypeError('train_sequence should be a numpy array of float type.')
     if isinstance(train_cluster_id, list):
@@ -359,11 +394,26 @@ class UISRNN:
     del args
     return self.device.type == 'cuda' and 1 <= self.rnn_init_hidden.shape[0] <= 4
 
+  def _require_device_trainer(self, args):
+    if not self._native_fit_supported(args):
+      raise TypeError('train_sequence tensors train on the device trainer only (rnn_depth 1 to 4 on a CUDA device); '
+                      'this model trains with PyTorch: pass float64 numpy arrays.')
+
+  def _fit_tensors(self, sequences, train_cluster_id, args):
+    """fit_concatenated of checked CUDA tensors `sequences`, whose rows back to back are the concatenated sequence, and
+    their string labels: the steps of the ndarray path on the device trainer, reading the rows in place."""
+    self.rnn_model.train()
+    self._get_optimizer(optimizer=args.optimizer, learning_rate=args.learning_rate)
+    self._sync_replicas()
+    index_lists, seq_lengths = utils.resize_indices(train_cluster_id, args.num_permutations)
+    self._fit_native(sequences, index_lists, seq_lengths, args)
+
   def _fit_native(self, train_sequence, index_lists, seq_lengths, args):
     """fit_concatenated's iteration loop (uisrnn.py:252-311) on libuisrnn_b200.so: the training set,
     parameters, gradients and Adam state stay on the device; per iteration only the ids of the drawn
     sub-sequences go up (the batch is gathered on the device) and the loss scalars are read back
-    when they are logged."""
+    when they are logged.  `train_sequence` is a float64 ndarray (copied to the device as fp32, steps on stream 0) or a
+    list of CUDA tensors (read in place; every step on torch's current stream of the model's device)."""
     from . import native
     import torch.distributed as dist
     world = dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1
@@ -391,24 +441,29 @@ class UISRNN:
     self.last_fit_backend = 'native'
     comm = torch.zeros(trainer.comm_size(), dtype=torch.float32, device=self.device) if world > 1 else None
     sampler = utils.BatchSampler(seq_lengths, args.batch_size)
+    tensors = isinstance(train_sequence, list)
+    stream = torch.cuda.current_stream(self.device).cuda_stream if tensors else 0
     try:
-      trainer.set_corpus(train_sequence, index_lists)
+      if tensors:
+        trainer.set_corpus_device(train_sequence, index_lists, stream=stream)
+      else:
+        trainer.set_corpus(train_sequence, index_lists)
       pending = 0  # steps enqueued since the losses were last read back
       for num_iter in range(args.train_iteration):
         chosen, _ = sampler.draw()  # same np.random.choice call as utils.pack_sequence
         if world == 1:
-          trainer.step_corpus(chosen)  # asynchronous: the host runs ahead of the device
+          trainer.step_corpus(chosen, stream=stream)  # asynchronous: the host runs ahead of the device
         else:
           # local forward/backward on this rank's columns -> ONE all-reduce(sum) of [gradients | loss
           # statistics] over NCCL -> identical normalise / clip / Adam step on every rank
           mine = shard_columns(len(chosen), rank, world)
           if len(mine):
-            trainer.step_corpus(chosen[mine], mode=2)
-            trainer.comm_export(comm.data_ptr())
+            trainer.step_corpus(chosen[mine], mode=2, stream=stream)
+            trainer.comm_export(comm.data_ptr(), stream=stream)
           else:
             comm.zero_()
           dist.all_reduce(comm, op=dist.ReduceOp.SUM)
-          trainer.comm_apply(comm.data_ptr())
+          trainer.comm_apply(comm.data_ptr(), stream=stream)
         pending += 1
         log_now = num_iter % 10 == 0 or num_iter == args.train_iteration - 1
         if log_now or pending == 4096:
@@ -434,8 +489,27 @@ class UISRNN:
 
   def fit(self, train_sequences, train_cluster_ids, args):
     """Trains on a list of sequences (+ list of label sequences) or on one concatenated sequence
-    (uisrnn.py:315-386).  Estimates / running-averages `transition_bias` unless it was given."""
-    if isinstance(train_sequences, np.ndarray):
+    (uisrnn.py:315-386).  Estimates / running-averages `transition_bias` unless it was given.
+
+    Training sets already on the GPU (not in the reference): a CUDA model that trains on the device trainer (rnn_depth
+    1 to 4) also takes a list of torch tensors [N_i, D], or one tensor as the concatenated form, on the model's device,
+    all float32, all float16, all bfloat16 or all float64 (any strides; requires_grad is ignored).  A list mixing
+    tensors with ndarrays, or mixing dtypes, is a TypeError.  A label sequence may then be an integer tensor [N_i] on
+    the same device (any integer dtype and strides) or host labels as above, in any mix per utterance; an integer
+    label v is the string str(v), so it trains exactly as that string would, uniqueness prefixes included.  The label
+    tensors are read back to the host once: the shuffle, the sub-sequence permutations and the mini-batch draws stay
+    on the host and use the same random numbers as for ndarrays.  The trainer reads the rows in place, in their dtype,
+    on torch's current stream of the device, with no copy of the training set (a tensor whose elements are not in
+    unit stride is copied once).  With the same seeds every iteration gathers, bit for bit, the batch a fit of the same
+    values as float64 ndarrays gathers (float64 rounds to nearest on the device as the ndarray path's cast does, float16
+    / bfloat16 convert exactly), so a step's gradients are those of the ndarray route.  Whole fits agree as two ndarray
+    fits do: to the trainer's run-to-run spread (its per-dimension residual sums are float atomics).  The rows must not
+    change until fit() returns.  A CPU model raises the reference's TypeError
+    for tensors, and a CUDA model that trains with PyTorch (rnn_depth > 4) a TypeError."""
+    on_cuda = self.device.type == 'cuda'
+    if not on_cuda and isinstance(train_sequences, list) and any(isinstance(s, torch.Tensor) for s in train_sequences):
+      raise TypeError('train_sequence should be a numpy array of float type.')
+    if isinstance(train_sequences, np.ndarray) or (on_cuda and isinstance(train_sequences, torch.Tensor)):
       if self.estimate_transition_bias:
         self.logger.print(
             2, 'Warning: transition_bias cannot be correctly estimated from a concatenated sequence; '
@@ -446,6 +520,10 @@ class UISRNN:
       train_cluster_ids = [train_cluster_ids]
     elif not isinstance(train_sequences, list):
       raise TypeError('train_sequences must be a list or numpy.ndarray')
+    tensors = on_cuda and _tensor_sequences(train_sequences, self.observation_dim, self.device, 'train_sequence')
+    if tensors:
+      self._require_device_trainer(args)
+      train_cluster_ids = _fit_labels(train_cluster_ids, [s.shape[0] for s in train_sequences], self.device)
     if self._native_fit_supported(args):
       self._sync_replicas()  # before the shuffle inside concatenate_training_data
     if self.estimate_transition_bias:
@@ -460,7 +538,10 @@ class UISRNN:
         self.transition_bias_denominator = merged
     sequence, cluster_id = utils.concatenate_training_data(
         train_sequences, train_cluster_ids, args.enforce_cluster_id_uniqueness, True)
-    self.fit_concatenated(sequence, cluster_id, args)
+    if tensors:
+      self._fit_tensors(sequence, cluster_id, args)
+    else:
+      self.fit_concatenated(sequence, cluster_id, args)
 
   # ------------------------------------------------------------------ inference
   def _fingerprint(self, copy=True):

@@ -36,12 +36,47 @@ def enforce_cluster_id_uniqueness(cluster_ids):
   return unique_ids
 
 
+def host_labels(cluster_ids):
+  """`cluster_ids` with every integer torch tensor [N] replaced by the list of the strings str(v) of its values v: the
+  label rule of a fit from tensors, under which such a tensor trains exactly as that list of strings does.  All the
+  tensors are read back in one copy (8 bytes per label); other entries are returned as they are."""
+  positions = [u for u, ids in enumerate(cluster_ids) if isinstance(ids, torch.Tensor)]
+  if not positions:
+    return cluster_ids
+  for u in positions:
+    ids = cluster_ids[u]
+    if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
+      raise TypeError('utterance {}: a label tensor must have an integer dtype, got {}'.format(u, ids.dtype))
+    if ids.ndim != 1:
+      raise ValueError('a label sequence must be a 1-D sequence of labels')
+  # uint64 travels as its int64 bit pattern (a same-size view, any strides) and is unwrapped on the host
+  values = torch.cat([cluster_ids[u].detach().view(torch.int64) if cluster_ids[u].dtype == torch.uint64 else
+                      cluster_ids[u].detach().to(torch.int64) for u in positions]).cpu().tolist()
+  out, start = list(cluster_ids), 0
+  for u in positions:
+    n = cluster_ids[u].shape[0]
+    part = values[start:start + n]
+    if cluster_ids[u].dtype == torch.uint64:
+      part = [v + 2 ** 64 if v < 0 else v for v in part]
+    out[u] = [str(v) for v in part]
+    start += n
+  return out
+
+
 def concatenate_training_data(train_sequences, train_cluster_ids, enforce_uniqueness=True, shuffle=True):
-  """Validates, optionally uniquifies + shuffles, then concatenates sequences (utils.py:64-123)."""
+  """Validates, optionally uniquifies + shuffles, then concatenates sequences (utils.py:64-123).
+
+  Sequences that are torch tensors are not concatenated: the shuffled list of them is returned in place of the
+  concatenated sequence (the device trainer reads their rows where they are), and their label sequences may be integer
+  torch tensors, taken as host_labels defines them.  The `random` calls are the same either way.  With ndarray
+  sequences the label sequences follow the reference's rules: a tensor among them is a TypeError."""
   if not isinstance(train_sequences, list) or not isinstance(train_cluster_ids, list):
     raise TypeError('train_sequences and train_cluster_ids must be lists')
   if len(train_sequences) != len(train_cluster_ids):
     raise ValueError('train_sequences and train_cluster_ids must have same size')
+  tensors = any(isinstance(sequence, torch.Tensor) for sequence in train_sequences)
+  if tensors:
+    train_cluster_ids = host_labels(train_cluster_ids)
   train_cluster_ids = [ids.tolist() if isinstance(ids, np.ndarray) else ids for ids in train_cluster_ids]
   expected_dim = None
   for position, (sequence, ids) in enumerate(zip(train_sequences, train_cluster_ids)):
@@ -60,7 +95,10 @@ def concatenate_training_data(train_sequences, train_cluster_ids, enforce_unique
     paired = list(zip(train_sequences, train_cluster_ids))
     random.shuffle(paired)
     train_sequences, train_cluster_ids = zip(*paired)
-  concatenated_sequence = np.concatenate(train_sequences, axis=0)
+  if tensors:
+    concatenated_sequence = list(train_sequences)
+  else:
+    concatenated_sequence = np.concatenate(train_sequences, axis=0)
   concatenated_ids = [label for ids in train_cluster_ids for label in ids]
   return concatenated_sequence, concatenated_ids
 
