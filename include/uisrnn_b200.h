@@ -432,7 +432,10 @@ int uis_trainer_set_corpus_device(uis_trainer* t, const void* const* row_addr, i
  * (uis_trainer_comm_size() floats) into a caller-owned DEVICE buffer, all-reduces(sum) it (NCCL over
  * NVLink: one collective per iteration), and hands it back: uis_trainer_comm_apply() normalises by the
  * global row count, forms the sigma2 gradient and the three losses from the global statistics, adds the
- * regulariser, clips and takes the Adam step -- identically on every rank.
+ * regulariser, clips and takes the Adam step -- identically on every rank.  A rank that holds no column of
+ * an iteration (a mini-batch narrower than the world) runs no step and exports nothing: it contributes a
+ * zero buffer to the sum and calls uis_trainer_comm_apply() all the same, which it may do before its
+ * first uis_trainer_step().
  */
 int64_t uis_trainer_comm_size(uis_trainer* t);
 int uis_trainer_comm_export(uis_trainer* t, float* dev_buf, void* stream);

@@ -10,7 +10,8 @@ stacked GRU runs layer by layer and the output of layer l is multiplied by scale
 
 In float64 on the CPU (or on a GPU with cuDNN off) neither TF32 nor cuDNN is involved, so the result is the exact
 value of the operation up to float64 rounding: the yardstick the fp32 kernels of csrc/uis_train.cu are pinned to by
-tests/test_gpu_fit_fp64.py.  tests/test_fit_oracle_cpu.py pins this module to the repository's own torch fit() path.
+tests/test_gpu_fit_fp64.py, and in data-parallel mode (shard_dropout_scales) by tests/test_gpu_fit_dp_fp64.py.
+tests/test_fit_oracle_cpu.py pins this module to the repository's own torch fit() path.
 
 FitAdam is the tail of the iteration: clip_grad_norm_ over rnn_model.parameters(), torch.optim.Adam with its defaults
 (the param groups of UISRNN._get_optimizer) and the sigma^2 clamp, with its own float64 state, driven by gradients the
@@ -43,6 +44,27 @@ def dropout_scales(seed, iteration, depth, L, B, H, p):
   inv_keep = float(np.float32(1.0) / (np.float32(1.0) - np.float32(p)))
   return [native.dropout_keep_mask(seed, iteration, l, L * B * H, p).reshape(L, B, H) * inv_keep
           for l in range(depth - 1)]
+
+
+def shard_dropout_scales(seeds, iteration, depth, lengths, H, p, world):
+  """dropout_scales of a data-parallel iteration, laid out on the full batch: rank r (trainer seed seeds[r]) holds
+  columns shard_columns(B, r, world) and masks them as its own zero-padded shard [L_r, B_r, H], L_r the length of
+  its first column.  Column b, the j-th of rank r, carries dropout_scales(seeds[r], iteration, depth, L_r, B_r, H,
+  p)[:, j] at rows < L_r and zeros below (padding of every rank's layout).  Without dropout, the all-reduced
+  iteration is the full-batch one, so these scales make losses_and_grads on the full batch the oracle of every
+  rank's step.  Float64 arrays [L, B, H]."""
+  from uisrnn_b200.uisrnn import shard_columns
+  lengths = np.asarray(lengths)
+  L, B = int(lengths[0]), len(lengths)
+  out = [np.zeros((L, B, H)) for _ in range(depth - 1)]
+  for r in range(world):
+    mine = shard_columns(B, r, world)
+    if not len(mine):
+      continue
+    Lr = int(lengths[mine[0]])
+    for full, shard in zip(out, dropout_scales(seeds[r], iteration, depth, Lr, len(mine), H, p)):
+      full[:Lr, mine] = shard
+  return out
 
 
 def random_params(D, H, depth, seed):

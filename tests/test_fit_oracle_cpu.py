@@ -82,6 +82,41 @@ def test_dropout_path_with_unit_scales_is_the_stacked_gru(depth):
   assert not np.array_equal(dropped['gru.weight_ih_l%d' % (depth - 1)], want['gru.weight_ih_l%d' % (depth - 1)])
 
 
+def test_shard_dropout_scales_at_world_1_are_the_full_batch_scales():
+  lengths, H, depth, p = [9, 7, 7, 4, 2], 5, 3, 0.3
+  got = fit_oracle.shard_dropout_scales([0xABC], 2, depth, lengths, H, p, 1)
+  want = fit_oracle.dropout_scales(0xABC, 2, depth, 9, 5, H, p)
+  assert len(got) == depth - 1
+  for g, w in zip(got, want):
+    assert np.array_equal(g, w)
+
+
+@pytest.mark.parametrize('world', [2, 3])
+def test_shard_dropout_scales_follow_each_ranks_own_layout(world):
+  """Column b of rank r = b % world carries the keep mask of element (t, j, h) of r's shard [L_r, B_r, H] (j = b //
+  world, the column's place in that shard) under r's seed, for t < L_r; zeros below.  Seeds differ per rank, the
+  first column of rank 1 is shorter than the batch, and rank 2 of world 3 has one column fewer than rank 0."""
+  from uisrnn_b200 import native
+  lengths, H, depth, p, it = [11, 8, 8, 6, 5, 3, 2, 2], 4, 3, 0.4, 5
+  seeds = [0x1234 + 97 * r for r in range(world)]
+  got = fit_oracle.shard_dropout_scales(seeds, it, depth, lengths, H, p, world)
+  inv_keep = 1.0 / (1.0 - p)
+  B = len(lengths)
+  for l in range(depth - 1):
+    assert got[l].shape == (11, B, H)
+    for b in range(B):
+      r, j = b % world, b // world
+      Br = len(range(r, B, world))
+      Lr = lengths[r]
+      keep = native.dropout_keep_mask(seeds[r], it, l, Lr * Br * H, p).reshape(Lr, Br, H)[:, j]
+      np.testing.assert_allclose(got[l][:Lr, b], keep * inv_keep, rtol=1e-6)
+      assert np.array_equal(got[l][:Lr, b] > 0, keep)
+      assert not got[l][Lr:, b].any()
+  # the shards' masks are not one mask: rank 1's columns differ from what rank 0's seed would give them
+  keep0 = native.dropout_keep_mask(seeds[0], it, 0, 11 * B * H, p).reshape(11, B, H)
+  assert not np.array_equal(got[0][:lengths[1], 1] > 0, keep0[:lengths[1], 1])
+
+
 def test_adam_matches_torch_optimizer_on_the_model():
   """FitAdam = clip_grad_norm_ + UISRNN._get_optimizer('adam') + clamp, applied to the same gradients."""
   import torch

@@ -4,6 +4,9 @@
 * `test_shard_export_sum_apply_equals_full_step` runs on ONE GPU: two trainers stand in for two ranks and
   the all-reduce is a torch add -- it pins the C-ABI arithmetic (mode 2 + comm_export + comm_apply).
 * `test_fit_nccl_world2` is the real thing (two processes, NCCL); skipped on a box with < 2 GPUs.
+* `test_fit_gloo_world3` runs UISRNN.fit in three processes over gloo on one GPU, with a rank that never holds a
+  column.
+tests/test_gpu_fit_dp_fp64.py pins the same steps per element to float64.
 """
 import os
 import random
@@ -125,3 +128,73 @@ def test_fit_nccl_world2(tmp_path):
   assert np.allclose(np.array(model.last_training_losses), a['losses'], rtol=1e-3)
   for k, v in single.items():
     assert np.max(np.abs(v - a[k])) < 2e-4, k     # 12 Adam steps of <= 1e-3 each; fp32 re-association only
+
+
+GLOO_CONFIGS = {
+    # two columns over three ranks: rank 2 holds none in any iteration and only adds zeros and applies the sum
+    'ndarray-batch2': dict(batch=2),
+    # bfloat16 tensors read in place, two layers with inter-layer dropout (each rank masks its own columns)
+    'bf16-depth2-dropout-batch4': dict(batch=4, depth=2, dropout=0.2, tensors=True),
+}
+
+
+def _configure(m, t, config):
+  t.batch_size = config['batch']
+  m.rnn_depth = config.get('depth', 1)
+  m.rnn_dropout = config.get('dropout', 0.0)
+
+
+def _fit_outputs(model):
+  out = {k: v.detach().cpu().numpy() for k, v in model.rnn_model.state_dict().items()}
+  out['sigma2'] = model.sigma2.detach().cpu().numpy()
+  out['h0'] = model.rnn_init_hidden.detach().cpu().numpy()
+  out['losses'] = np.array(model.last_training_losses)
+  out['loss_terms'] = np.array(model.last_training_loss_terms)
+  return out
+
+
+def _gloo_worker(rank, world, port, out_dir, config):
+  sys.path.insert(0, ROOT)
+  sys.path.insert(0, os.path.join(ROOT, 'tests'))
+  import torch
+  import torch.distributed as dist
+  dist.init_process_group('gloo', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world)
+  uisrnn, _, m, t, seqs, ids = _setup(seed=21 + 100 * rank)   # ranks start from DIFFERENT weights / RNG
+  _configure(m, t, config)
+  model = uisrnn.UISRNN(m)
+  if config.get('tensors'):
+    seqs = [torch.from_numpy(s).cuda().bfloat16() for s in seqs]
+  model.fit(seqs, ids, t)
+  assert model.last_fit_backend == 'native'
+  np.savez(os.path.join(out_dir, 'rank%d.npz' % rank), **_fit_outputs(model))
+  dist.destroy_process_group()
+
+
+@pytest.mark.parametrize('name', list(GLOO_CONFIGS))
+def test_fit_gloo_world3(tmp_path, name):
+  """Data-parallel fit() in three processes on one GPU over gloo, mini-batches narrower than or not a multiple of
+  the world: every rank ends with the same model, losses and loss terms, bit for bit; without dropout the model is
+  the single-process fit from rank 0's start, within the bounds of test_fit_nccl_world2."""
+  import torch.multiprocessing as mp
+  config = GLOO_CONFIGS[name]
+  world = 3
+  with socket.socket() as s:
+    s.bind(('127.0.0.1', 0))
+    port = s.getsockname()[1]
+  mp.spawn(_gloo_worker, args=(world, port, str(tmp_path), config), nprocs=world, join=True)
+  got = [np.load(str(tmp_path / ('rank%d.npz' % r))) for r in range(world)]
+  assert len(got[0]['losses']) == 12
+  for r in range(1, world):
+    for k in got[0].files:
+      assert np.array_equal(got[0][k], got[r][k]), (r, k)
+  if config.get('dropout'):
+    return
+  uisrnn, _, m, t, seqs, ids = _setup(seed=21)
+  _configure(m, t, config)
+  model = uisrnn.UISRNN(m)
+  model.fit(seqs, ids, t)
+  single = _fit_outputs(model)
+  assert np.allclose(single['losses'], got[0]['losses'], rtol=1e-3)
+  for k in single:
+    if k not in ('losses', 'loss_terms'):
+      assert np.max(np.abs(single[k] - got[0][k])) < 2e-4, k

@@ -1018,6 +1018,9 @@ int uis_trainer_create(uis_trainer** out, int device, int D, int H, const float*
     CUT(cudaMalloc(&t->seg_off_d, sizeof(t->seg_off_h)));
     CUT(cudaMemcpy(t->seg_off_d, t->seg_off_h, sizeof(t->seg_off_h), cudaMemcpyHostToDevice));
     CUT(cudaMalloc(&t->small, (size_t)(2 * D + 128) * 4));
+    // finish_step's per-segment sum-of-squares partials: allocated here, not by the first iteration, because a
+    // data-parallel rank that holds no batch column calls uis_trainer_comm_apply before it has ever stepped
+    if (int rc = t->partial.ensure((size_t)32 * uis::kSumsqBlocks)) return rc;
     CUT(cudaMalloc(&t->tickets, 256 * sizeof(unsigned)));
     CUT(cudaMemset(t->tickets, 0, 256 * sizeof(unsigned)));
     CUT(cudaMalloc(&t->gemm_tickets, 4096 * sizeof(unsigned)));
@@ -1239,7 +1242,6 @@ int run_iteration(uis_trainer* t, const int32_t* lengths, int B, int L, int mode
   if (int rc = t->carry.ensure((size_t)B * H)) return rc;
   if (int rc = t->whh_t.ensure((size_t)3 * H * H)) return rc;
   if (int rc = t->ghbuf.ensure((size_t)32 * 3 * H)) return rc;
-  if (int rc = t->partial.ensure((size_t)32 * kSumsqBlocks)) return rc;
   if (int rc = t->skpart.ensure((size_t)((3 * H + 63) / 64) * kSplit * 32 * 64)) return rc;
   if ((3 * H + 63) / 64 > 256) return api_fail(UIS_ERR_UNSUPPORTED, "hidden size too large for the training kernels");
   if (R * 3 * H > (size_t)0x7fffffff) return api_fail(UIS_ERR_UNSUPPORTED, "batch of %d x %d rows is too large", L, B);
