@@ -113,7 +113,8 @@ typedef struct uis_stats {
                                overlapped with the copies)                                                             */
   float host_ms;            /* wall time inside uis_predict()                                                          */
   int32_t chunks;           /* staging chunks the float64 rows travelled in                                            */
-  int32_t groups;           /* > 1: the list did not fit the device at once and was decoded in this many groups        */
+  int32_t groups;           /* every predict and score entry point: groups of whole utterances the list ran in (1: at
+                               once; > 1: it did not fit the device at once); the other fields add up over the groups */
   int32_t staged;           /* 1: the inputs were pageable and went through the library's pinned staging ring (host
                                copy threads), 0: copied straight from the caller's (pinned) buffers                     */
 } uis_stats;
@@ -151,6 +152,11 @@ int uis_model_constants(uis_model* m, float* mean0, float* hidden0);
  * Host->device copies, the beam search and the device->host copy of the labels all happen
  * inside the call.  Utterances are independent; they are scheduled longest-first over
  * persistent CTAs.
+ * Lists larger than the device (every predict and score entry point): when the per-frame workspace of the whole list
+ * does not fit the free device memory, the call runs consecutive groups of whole utterances one after the other on
+ * `stream`, each planned on its own, and writes every output where the whole call would.  An utterance longer than the
+ * budget is a group of its own.  The environment variable UISRNN_B200_MAX_ROWS (frames, >= 1) sets the budget instead.
+ * Debug taps keep a call in one group.
  */
 int uis_predict(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
                 const uis_predict_opts* opts, int32_t* const* labels_out,
@@ -245,10 +251,11 @@ int uis_predict_device_nbest(uis_model* m, const float* x_dev, const int64_t* fr
  * frame_out[u] float32 [n_frames[u]]); returns when the scores have landed.  uis_score_device: device buffers in the
  * layout of uis_predict_device (x_dev fp32 [frame_offsets[U], D], labels_dev int32 [frame_offsets[U]], scores_dev [U],
  * frame_dev [frame_offsets[U]]; frame_offsets on the host).  It copies the labels back to plan the chains, which
- * synchronises `stream` once at the start of the call; the kernels are then enqueued without waiting.
+ * synchronises `stream` once at the start of the call; the kernels are then enqueued without waiting, group after group
+ * when the list runs in groups.
  * Work: one GRU + MLP column per frame that is not the first of its cluster, in the FFMA weight pass of the beam
  * kernels (every kernel shape and depth).  Workspace: the handle's cache, about (12 H + 4 D + 24) bytes per frame; a
- * list that does not fit the device fails with UIS_ERR_NOMEM (it is not split into groups).  uis_get_stats after a
+ * list that does not fit the device is scored in groups of whole utterances (see uis_predict).  uis_get_stats after a
  * score call fills utterances, frames, gru_columns, weight_passes, kernel_launches, ctas, max_k (most clusters in one
  * utterance), prepass_ms, beam_ms (the chain kernel), engine = 1 and, for uis_score, the host-path fields; the rest
  * is zero.
@@ -278,9 +285,8 @@ int uis_score_device(uis_model* m, const float* x_dev, const int64_t* frame_offs
  * (device).  The chain kernel and the first-visit kernel run once; the reduce kernel runs once per config.
  * Debug taps index jobs: trace_utt = c * U + u, final_scores [count * U][beam_size], final_k [count * U].
  * uis_get_stats after a sweep: utterances = jobs (U * count), frames = distinct input rows; the work counters cover
- * every job (a score sweep's gru_columns equal a plain score call's).  The host-buffer predict sweep decodes a list
- * that does not fit the device in groups of whole utterances, each with all its configs; a score sweep that does not
- * fit fails with UIS_ERR_NOMEM.
+ * every job (a score sweep's gru_columns equal a plain score call's).  Every sweep runs a list that does not fit the
+ * device in groups of whole utterances, each with all its configs.
  * Synchronisation: the log tables of a sweep are built on the host and cached in the handle.  A sweep whose pairs (or
  * longest tiled decode) differ from the previous sweep's rewrites them in place, and first synchronises the DEVICE
  * (cudaDeviceSynchronize: an earlier call on any stream may still read them), so uis_predict_device_sweep /
@@ -318,7 +324,10 @@ int uis_score_device_sweep(uis_model* m, const float* x_dev, const int64_t* fram
  * holds fewer than 2^31 - 1 frames, x_dev is 16-byte aligned (the rows are read with 16-byte loads) and ids_dev 8-byte
  * aligned; anything else is UIS_ERR_INVALID.  The renaming and the chain plan run on the device (sorts and scans on `stream`),
  * so the call reads nothing back: it enqueues its work on `stream` and returns, except where a sweep rewrites its log
- * tables (see above) or the handle's workspace grows (cudaMalloc / cudaFree).  The scores are those
+ * tables (see above) or the handle's workspace grows (cudaMalloc / cudaFree).  A list run in groups stays so: its
+ * groups are cut from the host frame_offsets, each is renamed and planned on the device on its own (renaming is per
+ * utterance, so its ids rename as in the whole call), and the workspace is sized for the largest group before the
+ * first is enqueued.  The scores are those
  * uis_score_device_sweep gives for the canonical labels, bit for bit.  uis_get_stats fills the fields a score call
  * fills, max_k from the device plan.
  *

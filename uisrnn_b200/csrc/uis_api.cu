@@ -186,7 +186,7 @@ struct uis_model {
   DevBuf tree_arena;  // look-ahead spill kernel: [spill CTAs][make_tree_arena(..).total]
   // score calls (uis_kernels_score.cu): chain plan, per-frame Gaussian terms, reduce scratch, host entry's outputs
   DevBuf sc_chain_off, sc_chain_rows, sc_mse, sc_blocks, sc_out;
-  DevBuf sc_counts, sc_plan;  // device-planned score calls: {chains, queued, max_k}; the plan kernels' scratch
+  DevBuf sc_counts, sc_plan;  // device-planned score calls: {chains, queued, max_k, -} per group; the plan kernels' scratch
   DevBuf dbg_win, dbg_score, dbg_off, dbg_final_scores, dbg_final_k, dbg_best_mean, dbg_best_hidden,
       dbg_best_blocks;
   // last call
@@ -203,7 +203,10 @@ struct uis_model {
   size_t last_spill_budget = 0;
   cudaStream_t last_stream = nullptr;
   bool stats_pending = false;
-  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};  // before prepass, after prepass, after beam kernel
+  // before prepass, after prepass, after beam kernel: three per group of the last call that launched kernels
+  // (last_groups of them; a call decoded or scored in groups adds up their times)
+  std::vector<cudaEvent_t> ev = std::vector<cudaEvent_t>(3, nullptr);
+  int last_groups = 1;
   // host-buffer path (uis_predict): the float64 rows travel in chunks through a small ring of staging slots on a
   // copy stream of their own, so the H2D copy of chunk c + 1 runs under the cast + input projection of chunk c and
   // the fp64 staging is O(chunk), not O(input); labels come back in ONE copy into pinned memory
@@ -740,6 +743,83 @@ size_t workspace_bytes(const uis_model* m, const Plan& pl, int U, int configs = 
   return b;
 }
 
+// ---- groups: lists larger than the device, decoded or scored in groups of whole utterances ---------------------
+//
+// Utterances are independent in every beam and score kernel (uisrnn.py:587-589), and a score chain never crosses an
+// utterance, so a list whose per-frame workspace does not fit the device runs as consecutive groups of whole
+// utterances, one after the other on the call's stream, each planned on its own.  Every entry point decides the
+// group size here.
+
+// Frames one group may hold: UISRNN_B200_MAX_ROWS when set (>= 1), else what fits in 90% of the free device memory plus
+// the `held` bytes of handle buffers that the call re-uses, after `fixed` bytes that do not grow with the frames, at
+// `per_row` bytes per frame.  At least 1.
+int row_budget(size_t per_row, size_t fixed, size_t held, size_t* max_rows) {
+  if (const char* env = std::getenv("UISRNN_B200_MAX_ROWS")) {
+    *max_rows = (size_t)std::max(1ll, std::atoll(env));
+    return 0;
+  }
+  size_t free_b = 0, total_b = 0;
+  CU(cudaMemGetInfo(&free_b, &total_b));
+  const double budget = 0.9 * (double)(free_b + held) - (double)fixed;
+  *max_rows = budget > (double)per_row ? (size_t)(budget / (double)per_row) : 1;
+  return 0;
+}
+
+// Group boundaries of U utterances (frame offsets `off`) under a budget of max_rows frames: {0, u1, ..., U}, each group
+// as many consecutive whole utterances as fit, an utterance longer than max_rows a group of its own.
+std::vector<int> cut_groups(const int64_t* off, int U, size_t max_rows) {
+  std::vector<int> cuts{0};
+  for (int u0 = 0; u0 < U;) {
+    int u1 = u0 + 1;
+    while (u1 < U && (size_t)(off[u1 + 1] - off[u0]) <= max_rows) ++u1;
+    cuts.push_back(u1);
+    u0 = u1;
+  }
+  if (U == 0) cuts.push_back(0);  // an empty list: one empty group
+  return cuts;
+}
+
+// Frame offsets of utterances [u0, u1), rebased to the group's first row.
+std::vector<int64_t> group_offsets(const int64_t* off, int u0, int u1) {
+  std::vector<int64_t> g(u1 - u0 + 1);
+  for (int q = u0; q <= u1; ++q) g[q - u0] = off[q] - off[u0];
+  return g;
+}
+
+// Where one group of a call run in groups sits in the whole call (the defaults: a call of one group).
+struct Group {
+  int index = 0;         // groups of the call that launched kernels before this one: the first resets the device
+                         // counters and uses events 0..2, the later ones add to the counters and use their own events
+  int job0 = 0;          // the group's first job in the call's per-job status
+  long long plane = 0;   // the call's rows: the row stride of its label planes and per-frame score outputs (0: the group's)
+  int stride = 0;        // the call's U: the row stride of its [configs][U] score totals (0: the group's)
+};
+
+// Bytes of the queue counters at the head of queue_stats: a later group resets only these, so that the device
+// counters behind them add up over the groups of a call.
+constexpr size_t kQueueBytes = 8 * sizeof(unsigned long long);
+
+// Adds the stats of one group to those of the groups before it.
+void add_stats(uis_stats* a, const uis_stats& b) {
+  a->utterances += b.utterances; a->frames += b.frames; a->beam_steps += b.beam_steps; a->gru_columns += b.gru_columns;
+  a->weight_passes += b.weight_passes; a->candidates += b.candidates; a->kernel_launches += b.kernel_launches;
+  a->ctas = std::max(a->ctas, b.ctas); a->max_k = std::max(a->max_k, b.max_k);
+  a->prepass_ms += b.prepass_ms; a->beam_ms += b.beam_ms; a->h2d_ms += b.h2d_ms; a->pipeline_ms += b.pipeline_ms;
+  a->lanes = std::max(a->lanes, b.lanes); a->cluster = std::max(a->cluster, b.cluster);
+  a->engine = std::max(a->engine, b.engine); a->tc_columns = std::max(a->tc_columns, b.tc_columns);
+  for (int i = 0; i < 10; ++i) a->phase_cycles[i] += b.phase_cycles[i];
+  for (int i = 0; i < 4; ++i) a->tc_cycles[i] += b.tc_cycles[i];
+  a->chunks += b.chunks; a->groups += b.groups; a->staged = std::max(a->staged, b.staged);
+}
+
+// Creates the three events of group g.
+int group_events(uis_model* m, int g) {
+  if (m->ev.size() < (size_t)3 * (g + 1)) m->ev.resize((size_t)3 * (g + 1), nullptr);
+  for (auto& e : m->ev)
+    if (!e) CU(cudaEventCreate(&e));
+  return 0;
+}
+
 // Speaker bounds of a bounded call (host arrays, either may be NULL): 0 = no bound, max >= 1, 0 <= min <= max.
 struct SpeakerBounds {
   const int32_t* max = nullptr;
@@ -880,10 +960,11 @@ uis::BeamParams model_params(const uis_model* m) {
 
 // Decodes U utterances under dp.count configs: J = U * dp.count jobs, job j = utterance j % U under config j / U.
 // Per-job outputs (status, N-best scores / speakers / counts, taps) are [J]; labels_dev holds dp.count * nb.k planes
-// of the call's rows (plane c * nb.k + j: config c, hypothesis j).
+// of the call's rows (plane c * nb.k + j: config c, hypothesis j), grp.plane rows apart when this is one group of a
+// larger call.
 int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, const Plan& pl, int32_t* labels_dev,
                const uis_debug_taps* taps, cudaStream_t st, const SpeakerBounds& sb, const NBestOut& nb,
-               const DecodeParams& dp, bool gi_ready = false) {
+               const DecodeParams& dp, bool gi_ready = false, const Group& grp = Group{}) {
   const int H = m->H, D = m->D;
   const int J = U * dp.count;
   if (sb.out_dev && U > 0) CU(cudaMemsetAsync(sb.out_dev, 0, (size_t)J * sizeof(int32_t), st));  // empty inputs: 0
@@ -902,7 +983,9 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   m->stats.ctas = pl.ctas;
   m->stats.lanes = pl.G;
   m->stats.cluster = pl.cluster;
+  m->stats.groups = 1;
   m->last_U = J;
+  m->last_groups = 1;
   m->last_score = false;
   m->last_tree_spill = pl.spill_ctas > 0;
   m->last_spill_ni = pl.spill_ni; m->last_spill_nlf = pl.spill_nlf; m->last_spill_budget = pl.spill_budget;
@@ -928,7 +1011,7 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
 
   if (int rc = m->row_off.ensure((U + 1) * sizeof(long long))) return rc;
   if (int rc = m->order.ensure((size_t)J * sizeof(int))) return rc;
-  if (int rc = m->status.ensure((size_t)J * sizeof(int))) return rc;
+  if (int rc = m->status.ensure((size_t)(grp.job0 + J) * sizeof(int))) return rc;
   if (int rc = m->queue_stats.ensure(40 * sizeof(unsigned long long))) return rc;
   if (int rc = m->gi.ensure((size_t)pl.rows * 3 * H * sizeof(float))) return rc;
   if (int rc = m->pool_mean.ensure(pool_slots(pl) * D * sizeof(float))) return rc;
@@ -950,8 +1033,8 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
 
   CU(cudaMemcpyAsync(m->row_off.p, off_ll.data(), (U + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(m->order.p, order.data(), (size_t)J * sizeof(int), cudaMemcpyHostToDevice, st));
-  CU(cudaMemsetAsync(m->queue_stats.p, 0, 40 * sizeof(unsigned long long), st));
-  CU(cudaMemsetAsync(m->status.p, 0xff, (size_t)J * sizeof(int), st));
+  CU(cudaMemsetAsync(m->queue_stats.p, 0, grp.index ? kQueueBytes : 40 * sizeof(unsigned long long), st));
+  CU(cudaMemsetAsync(m->status.as<int>() + grp.job0, 0xff, (size_t)J * sizeof(int), st));
 
   p.x = x_dev; p.gi = m->gi.as<float>();
   p.row_off = m->row_off.as<long long>(); p.order = m->order.as<int>();
@@ -961,7 +1044,7 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   p.bp = m->bp.as<unsigned>();
   p.queue = m->queue_stats.as<int>();
   p.stats = m->queue_stats.as<unsigned long long>() + 8;
-  p.labels = labels_dev; p.status = m->status.as<int>();
+  p.labels = labels_dev; p.status = m->status.as<int>() + grp.job0;
   if (sb.max || sb.min) {
     std::vector<int32_t> kb(2 * (size_t)U);
     for (int u = 0; u < U; ++u) { kb[2 * u] = sb.max ? sb.max[u] : 0; kb[2 * u + 1] = sb.min ? sb.min[u] : 0; }
@@ -970,7 +1053,7 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
     p.spk_bound = m->spk_bound.as<int>();
   }
   p.spk_out = sb.out_dev;
-  p.n_best = nb.k; p.label_plane = pl.rows;
+  p.n_best = nb.k; p.label_plane = grp.plane ? grp.plane : pl.rows;
   p.nbest_scores = nb.scores; p.nbest_speakers = nb.speakers; p.nbest_count = nb.count;
   p.trace_utt = -1;
   if (pl.kernel == uis::Kernel::Stat) {
@@ -1014,9 +1097,9 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
     }
   }
 
-  for (auto& e : m->ev)
-    if (!e) CU(cudaEventCreate(&e));
-  CU(cudaEventRecord(m->ev[0], st));
+  if (int rc = group_events(m, grp.index)) return rc;
+  cudaEvent_t* ev = m->ev.data() + 3 * grp.index;
+  CU(cudaEventRecord(ev[0], st));
   // kernel 1: input projection GEMM (the host-buffer path has already run it chunk by chunk, under the H2D copies)
   if (!gi_ready) {
     dim3 grid((3 * H + uis::PBN - 1) / uis::PBN, (unsigned)((pl.rows + uis::PBM - 1) / uis::PBM));
@@ -1024,7 +1107,7 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
                                                 (int)pl.rows, 3 * H, D);
     CU(cudaGetLastError());
   }
-  CU(cudaEventRecord(m->ev[1], st));
+  CU(cudaEventRecord(ev[1], st));
   // kernel 2: the planned persistent beam search.  Look-ahead: the spill kernel right behind it on the same stream
   // decodes the utterances it left at status -5 (every one under Kernel::TreeSpill) from a second queue; its CTAs find
   // nothing to do and exit when every tree fitted.
@@ -1040,7 +1123,7 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   }
   m->stats.engine = tc ? 2 : 1;
   m->stats.tc_columns = tc ? uis::kTcColumns : 0;
-  CU(cudaEventRecord(m->ev[2], st));
+  CU(cudaEventRecord(ev[2], st));
   m->stats.kernel_launches = 2 + (pl.kernel == uis::Kernel::Tree && pl.spill_ctas ? 1 : 0);
   m->stats_pending = true;
 
@@ -1069,22 +1152,36 @@ int run_device(uis_model* m, const float* x_dev, const int64_t* off, int U, cons
   return 0;
 }
 
+// prepass_ms and beam_ms of the last call: the sums over its groups' events.
+int event_times(uis_model* m) {
+  m->stats.prepass_ms = m->stats.beam_ms = 0.f;
+  for (int g = 0; g < m->last_groups; ++g) {
+    const cudaEvent_t* ev = m->ev.data() + 3 * g;
+    float a = 0.f, b = 0.f;
+    CU(cudaEventElapsedTime(&a, ev[0], ev[1]));
+    CU(cudaEventElapsedTime(&b, ev[1], ev[2]));
+    m->stats.prepass_ms += a;
+    m->stats.beam_ms += b;
+  }
+  return 0;
+}
+
 // Pull the device-side counters and per-utterance status of the last call (synchronises).
 int collect(uis_model* m) {
   if (!m->stats_pending) return 0;
   CU(cudaStreamSynchronize(m->last_stream));
   unsigned long long s[24];
   CU(cudaMemcpy(s, m->queue_stats.as<unsigned long long>() + 8, sizeof s, cudaMemcpyDeviceToHost));
-  if (m->last_score) {  // the chain kernel's columns and passes; max_k came from the labels (or the device plan)
+  if (m->last_score) {  // the chain kernel's columns and passes; max_k came from the labels (or the device plans)
     m->stats.gru_columns = (int64_t)s[0];
     m->stats.weight_passes = (int64_t)s[1];
-    if (m->last_score_counts) {
-      int counts[3];
-      CU(cudaMemcpy(counts, m->sc_counts.p, sizeof counts, cudaMemcpyDeviceToHost));
-      m->stats.max_k = counts[2];
+    if (m->last_score_counts) {  // {chains, queued, max_k, -} of every group
+      std::vector<int> counts((size_t)4 * m->last_groups);
+      CU(cudaMemcpy(counts.data(), m->sc_counts.p, counts.size() * sizeof(int), cudaMemcpyDeviceToHost));
+      m->stats.max_k = 0;
+      for (int g = 0; g < m->last_groups; ++g) m->stats.max_k = std::max(m->stats.max_k, counts[(size_t)4 * g + 2]);
     }
-    CU(cudaEventElapsedTime(&m->stats.prepass_ms, m->ev[0], m->ev[1]));
-    CU(cudaEventElapsedTime(&m->stats.beam_ms, m->ev[1], m->ev[2]));
+    if (int rc = event_times(m)) return rc;
     m->stats_pending = false;
     return 0;
   }
@@ -1095,8 +1192,7 @@ int collect(uis_model* m) {
   m->stats.candidates = (int64_t)s[2];
   m->stats.beam_steps = (int64_t)s[3];
   m->stats.max_k = (int32_t)s[4];
-  CU(cudaEventElapsedTime(&m->stats.prepass_ms, m->ev[0], m->ev[1]));
-  CU(cudaEventElapsedTime(&m->stats.beam_ms, m->ev[1], m->ev[2]));
+  if (int rc = event_times(m)) return rc;
   m->stats_pending = false;
   std::vector<int> status(m->last_U);
   CU(cudaMemcpy(status.data(), m->status.p, (size_t)m->last_U * sizeof(int), cudaMemcpyDeviceToHost));
@@ -1163,6 +1259,65 @@ class CallOrder {
   cudaStream_t st_;
 };
 
+// A device-buffer decode in the groups `cuts` (cut_groups), one after the other on `st`, nothing read back.  Group
+// [u0, u1) reads its rows from x_dev + off[u0] rows, padded to the kernel's D in the handle's x32 when the model is
+// padded, so that its float4 loads start on a 16-byte boundary either way (an unpadded row is a multiple of 64
+// floats).  Its label planes start at row off[u0] of the call's [C][k][rows] planes (rows = plane apart); its
+// per-job outputs land in the handle's buffers and one 2-D copy per output puts their [C][u1 - u0] blocks at column
+// u0 of the caller's [C][U][k] / [C][U] arrays.  Its jobs' status sits at [u0 * C, u1 * C) of the handle's, which
+// collect() reads for the whole call.
+int predict_device_groups(uis_model* m, const float* x_dev, const int64_t* off, int U, long long plane,
+                          const uis_predict_opts* opts, int32_t* labels_dev, cudaStream_t st, const SpeakerBounds& sb,
+                          const NBestOut& nb, const DecodeParams& dp, const std::vector<int>& cuts) {
+  const int C = dp.count, K = nb.k, G = (int)cuts.size() - 1;
+  size_t max_jobs = 0;
+  for (int g = 0; g < G; ++g) max_jobs = std::max(max_jobs, (size_t)(cuts[g + 1] - cuts[g]) * C);
+  NBestOut gnb{K};
+  if (nb.scores) {
+    if (int rc = m->nb_scores.ensure(max_jobs * K * 4)) return rc;
+    gnb.scores = m->nb_scores.as<float>();
+  }
+  if (nb.speakers) {
+    if (int rc = m->nb_speakers.ensure(max_jobs * K * 4)) return rc;
+    gnb.speakers = m->nb_speakers.as<int32_t>();
+  }
+  if (nb.count) {
+    if (int rc = m->nb_count.ensure(max_jobs * 4)) return rc;
+    gnb.count = m->nb_count.as<int32_t>();
+  }
+  if (int rc = m->status.ensure((size_t)U * C * sizeof(int))) return rc;
+  CU(cudaMemsetAsync(m->status.p, 0, (size_t)U * C * sizeof(int), st));  // a group of empty utterances launches nothing
+  uis_stats total{};
+  int ran = 0;
+  for (int g = 0; g < G; ++g) {
+    const int u0 = cuts[g], u1 = cuts[g + 1], Ug = u1 - u0;
+    const std::vector<int64_t> goff = group_offsets(off, u0, u1);
+    Plan gp;
+    if (int rc = make_plan(m, goff.data(), Ug, opts, &gp, C)) return rc;
+    const float* gx = x_dev + (size_t)off[u0] * m->D_user;
+    if (int rc = pad_to_kernel_d(m, &gx, (size_t)gp.rows, st)) return rc;
+    if (int rc = run_device(m, gx, goff.data(), Ug, gp, labels_dev + off[u0], nullptr, st, sb.at(u0), gnb, dp, false,
+                            Group{ran, u0 * C, plane, 0}))
+      return rc;
+    ran += gp.rows > 0 ? 1 : 0;
+    const size_t w = (size_t)Ug * K * 4;  // one config's block of the group: [Ug][k]
+    if (nb.scores)
+      CU(cudaMemcpy2DAsync(nb.scores + (size_t)u0 * K, (size_t)U * K * 4, gnb.scores, w, w, C, cudaMemcpyDeviceToDevice, st));
+    if (nb.speakers)
+      CU(cudaMemcpy2DAsync(nb.speakers + (size_t)u0 * K, (size_t)U * K * 4, gnb.speakers, w, w, C,
+                           cudaMemcpyDeviceToDevice, st));
+    if (nb.count)
+      CU(cudaMemcpy2DAsync(nb.count + u0, (size_t)U * 4, gnb.count, (size_t)Ug * 4, (size_t)Ug * 4, C,
+                           cudaMemcpyDeviceToDevice, st));
+    add_stats(&total, m->stats);
+  }
+  m->stats = total;
+  m->last_U = U * C;
+  m->last_groups = ran;
+  m->stats_pending = ran > 0;
+  return 0;
+}
+
 int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U,
                         const uis_predict_opts* opts, int32_t* labels_dev, const uis_debug_taps* taps, void* stream,
                         const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_dev,
@@ -1178,9 +1333,19 @@ int predict_device_impl(uis_model* m, const float* x_dev, const int64_t* frame_o
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CallOrder order(m, st);
   CU(order.status);
+  // Memory: the rows and the label planes are the caller's; per frame the call holds gi (12H B) and, for a model
+  // padded to its kernel shape, the padded fp32 rows (4D B).
+  const bool padded = m->D != m->D_user;
+  const size_t per_row = (size_t)3 * m->H * 4 + (padded ? (size_t)m->D * 4 : 0);
+  const size_t fixed = workspace_bytes(m, pl, U, dp.count) - (size_t)pl.rows * 3 * m->H * 4;
+  size_t max_rows = 0;
+  if (int rc = row_budget(per_row, fixed, m->gi.cap + (padded ? m->x32.cap : 0), &max_rows)) return rc;
+  const SpeakerBounds sb{max_speakers, min_speakers, speakers_dev};
+  if ((size_t)pl.rows > max_rows && !taps && U > 1)
+    return predict_device_groups(m, x_dev, frame_offsets, U, pl.rows, opts, labels_dev, st, sb, nb, dp,
+                                 cut_groups(frame_offsets, U, max_rows));
   if (int rc = pad_to_kernel_d(m, &x_dev, (size_t)pl.rows, st)) return rc;
-  return run_device(m, x_dev, frame_offsets, U, pl, labels_dev, taps, st,
-                    SpeakerBounds{max_speakers, min_speakers, speakers_dev}, nb, dp);
+  return run_device(m, x_dev, frame_offsets, U, pl, labels_dev, taps, st, sb, nb, dp);
 }
 
 // ---- host input pipeline -----------------------------------------------------------------------------------------
@@ -1398,18 +1563,6 @@ int predict_host_group(uis_model* m, const double* const* seqs, const int64_t* n
   return rc;
 }
 
-void add_stats(uis_stats* a, const uis_stats& b) {
-  a->utterances += b.utterances; a->frames += b.frames; a->beam_steps += b.beam_steps; a->gru_columns += b.gru_columns;
-  a->weight_passes += b.weight_passes; a->candidates += b.candidates; a->kernel_launches += b.kernel_launches;
-  a->ctas = std::max(a->ctas, b.ctas); a->max_k = std::max(a->max_k, b.max_k);
-  a->prepass_ms += b.prepass_ms; a->beam_ms += b.beam_ms; a->h2d_ms += b.h2d_ms; a->pipeline_ms += b.pipeline_ms;
-  a->lanes = std::max(a->lanes, b.lanes); a->cluster = std::max(a->cluster, b.cluster);
-  a->engine = std::max(a->engine, b.engine); a->tc_columns = std::max(a->tc_columns, b.tc_columns);
-  for (int i = 0; i < 10; ++i) a->phase_cycles[i] += b.phase_cycles[i];
-  for (int i = 0; i < 4; ++i) a->tc_cycles[i] += b.tc_cycles[i];
-  a->chunks += b.chunks; a->groups += b.groups; a->staged = std::max(a->staged, b.staged);
-}
-
 int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
                       const uis_predict_opts* opts, int32_t* const* labels_out, const uis_debug_taps* taps, void* stream,
                       const int32_t* max_speakers, const int32_t* min_speakers, int32_t* speakers_out,
@@ -1441,20 +1594,13 @@ int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_
   CallOrder order(m, st);
   CU(order.status);
   // Memory: the per-frame workspace (gi 12H B + fp32 rows 4D B + labels) is the part that grows with the input.
-  // A list that does not fit the device at once is decoded in groups of whole utterances, one after the other
-  // (utterances are independent, uisrnn.py:587-589); UISRNN_B200_MAX_ROWS forces a limit (tests).
+  // A list that does not fit the device at once is decoded in groups of whole utterances (row_budget, cut_groups).
   const size_t per_row = (size_t)3 * m->H * 4 + (size_t)m->D * 4 + (size_t)4 * nb.k * dp.count;  // (+ one label per plane)
+  const size_t held = m->gi.cap + m->x32.cap + m->labels.cap + m->x64.cap;  // re-used by this call
+  const size_t fixed = workspace_bytes(m, pl, U, dp.count) - (size_t)pl.rows * 3 * m->H * 4 +
+                       (size_t)uis_model::kSlots * staging_chunk_rows(m->D_user) * m->D_user * 8 + J * (2 * nb.k + 1) * 4;
   size_t max_rows = 0;
-  if (const char* env = std::getenv("UISRNN_B200_MAX_ROWS")) max_rows = (size_t)std::max(1ll, std::atoll(env));
-  if (!max_rows) {
-    size_t free_b = 0, total_b = 0;
-    CU(cudaMemGetInfo(&free_b, &total_b));
-    const size_t held = m->gi.cap + m->x32.cap + m->labels.cap + m->x64.cap;  // re-used by this call
-    const size_t fixed = workspace_bytes(m, pl, U, dp.count) - (size_t)pl.rows * 3 * m->H * 4 +
-                         (size_t)uis_model::kSlots * staging_chunk_rows(m->D_user) * m->D_user * 8 + J * (2 * nb.k + 1) * 4;
-    const double budget = 0.9 * (double)(free_b + held) - (double)fixed;
-    max_rows = budget > (double)per_row ? (size_t)(budget / (double)per_row) : 1;
-  }
+  if (int rc = row_budget(per_row, fixed, held, &max_rows)) return rc;
   if ((size_t)pl.rows <= max_rows || taps || U <= 1) {
     if (int rc = predict_host_group(m, seqs, n_frames, U, off.data(), pl, labels_out, taps, st,
                                     SpeakerBounds{max_speakers, min_speakers}, speakers_out, nb, 0, U, dp))
@@ -1462,12 +1608,10 @@ int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_
     m->stats.groups = 1;
   } else {
     uis_stats total{};
-    int u0 = 0;
-    while (u0 < U) {
-      int u1 = u0 + 1;
-      while (u1 < U && (size_t)(off[u1 + 1] - off[u0]) <= max_rows) ++u1;
-      std::vector<int64_t> goff(u1 - u0 + 1);
-      for (int q = u0; q <= u1; ++q) goff[q - u0] = off[q] - off[u0];
+    const std::vector<int> cuts = cut_groups(off.data(), U, max_rows);
+    for (size_t g = 0; g + 1 < cuts.size(); ++g) {
+      const int u0 = cuts[g], u1 = cuts[g + 1];
+      const std::vector<int64_t> goff = group_offsets(off.data(), u0, u1);
       Plan gp;
       if (int rc = make_plan(m, goff.data(), u1 - u0, opts, &gp, dp.count)) return rc;
       if (int rc = predict_host_group(m, seqs + u0, n_frames + u0, u1 - u0, goff.data(), gp, labels_out + u0, nullptr, st,
@@ -1476,7 +1620,6 @@ int predict_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_
         return rc;
       m->stats.groups = 1;
       add_stats(&total, m->stats);
-      u0 = u1;
     }
     m->stats = total;
   }
@@ -1493,7 +1636,7 @@ struct ChainPlan {
   int chains = 0, queued = 0, max_k = 0;  // queued: chains of length >= 2 (a prefix, longest first)
 };
 
-int plan_chains(const int32_t* labels, const int64_t* off, int U, ChainPlan* cp) {
+int plan_chains(const int32_t* labels, const int64_t* off, int U, ChainPlan* cp, int u_base = 0) {
   std::vector<long long> base(U + 1, 0);  // first chain id of every utterance
   for (int u = 0; u < U; ++u) {
     int K = 0;
@@ -1501,7 +1644,7 @@ int plan_chains(const int32_t* labels, const int64_t* off, int U, ChainPlan* cp)
       const int c = labels[r];
       if (c < 0 || c > K)
         return fail(UIS_ERR_INVALID, "utterance %d frame %lld: label %d is not canonical (labels are 0, 1, 2, ... in "
-                    "order of first appearance, so at most %d here)", u, r - off[u], c, K);
+                    "order of first appearance, so at most %d here)", u_base + u, r - off[u], c, K);
       K += (c == K) ? 1 : 0;
     }
     base[u + 1] = base[u] + K;
@@ -1531,11 +1674,13 @@ int plan_chains(const int32_t* labels, const int64_t* off, int U, ChainPlan* cp)
 }
 
 // Enqueues a score call on `st`: input projection (unless gi_ready), chain kernel, first visits, then one reduce per
-// config of `dp` (scores_dev [configs][U], frame_dev [configs][rows]).  x_dev: the fp32 rows at the kernel shape (m->D);
-// labels_dev: the canonical labels the plan was made from.  cp: a host plan, uploaded here; nullptr: the device plan
-// that score_plan wrote to sc_chain_off / sc_chain_rows / sc_counts earlier on `st` (row_off is on the device too).
+// config of `dp` (scores_dev [configs][U], frame_dev [configs][rows]; a group of a larger call: rows grp.stride and
+// grp.plane apart).  x_dev: the fp32 rows at the kernel shape (m->D); labels_dev: the canonical labels the plan was
+// made from.  cp: a host plan, uploaded here; nullptr: the device plan that score_plan wrote to sc_chain_off /
+// sc_chain_rows / the group's sc_counts earlier on `st` (row_off is on the device too).
 int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const ChainPlan* cp, const int32_t* labels_dev,
-              float* scores_dev, float* frame_dev, cudaStream_t st, bool gi_ready, const DecodeParams& dp) {
+              float* scores_dev, float* frame_dev, cudaStream_t st, bool gi_ready, const DecodeParams& dp,
+              const Group& grp = Group{}) {
   const int H = m->H, D = m->D;
   const long long rows = off[U];
   long long maxN = 0;
@@ -1565,7 +1710,7 @@ int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const
     CU(cudaMemcpyAsync(m->sc_chain_rows.p, cp->rows.data(), cp->rows.size() * sizeof(long long), cudaMemcpyHostToDevice,
                        st));
   }
-  CU(cudaMemsetAsync(m->queue_stats.p, 0, 40 * sizeof(unsigned long long), st));
+  CU(cudaMemsetAsync(m->queue_stats.p, 0, grp.index ? kQueueBytes : 40 * sizeof(unsigned long long), st));
 
   sp.b.x = x_dev; sp.b.gi = m->gi.as<float>();
   sp.b.row_off = m->row_off.as<long long>();
@@ -1575,27 +1720,29 @@ int run_score(uis_model* m, const float* x_dev, const int64_t* off, int U, const
   sp.b.stats = m->queue_stats.as<unsigned long long>() + 8;
   sp.chain_off = m->sc_chain_off.as<long long>(); sp.chain_rows = m->sc_chain_rows.as<long long>();
   sp.chains = cp ? cp->chains : (int)rows; sp.queued = (int)queued;
-  sp.counts = cp ? nullptr : m->sc_counts.as<int>();
+  sp.counts = cp ? nullptr : m->sc_counts.as<int>() + 4 * grp.index;
   sp.mse = m->sc_mse.as<float>(); sp.labels = labels_dev; sp.scores = scores_dev; sp.frame_out = frame_dev;
+  sp.score_stride = grp.stride ? grp.stride : U;
+  sp.frame_stride = grp.plane ? grp.plane : rows;
   sp.blocks = m->sc_blocks.as<int>();
 
-  for (auto& e : m->ev)
-    if (!e) CU(cudaEventCreate(&e));
-  CU(cudaEventRecord(m->ev[0], st));
+  if (int rc = group_events(m, grp.index)) return rc;
+  cudaEvent_t* ev = m->ev.data() + 3 * grp.index;
+  CU(cudaEventRecord(ev[0], st));
   if (!gi_ready) {
     dim3 grid((3 * H + uis::PBN - 1) / uis::PBN, (unsigned)((rows + uis::PBM - 1) / uis::PBM));
     uis::input_proj_kernel<<<grid, 256, 0, st>>>(x_dev, m->wih_t.as<float>(), m->bih.as<float>(), m->gi.as<float>(),
                                                 (int)rows, 3 * H, D);
     CU(cudaGetLastError());
   }
-  CU(cudaEventRecord(m->ev[1], st));
+  CU(cudaEventRecord(ev[1], st));
   cudaError_t e = cudaSuccess;
   if (queued > 0) {
     if (!uis::launch_score_chains(H, D, sp, ctas, st, &e))
       return fail(UIS_ERR_UNSUPPORTED, "no score kernel for hidden=%d dim=%d", H, D);
     if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score chain kernel launch failed: %s", cudaGetErrorString(e));
   }
-  CU(cudaEventRecord(m->ev[2], st));
+  CU(cudaEventRecord(ev[2], st));
   if (!uis::launch_score_first(H, D, sp, st, &e)) return fail(UIS_ERR_UNSUPPORTED, "no score kernel for dim=%d", D);
   if (e != cudaSuccess) return fail(UIS_ERR_CUDA, "score first-visit kernel launch failed: %s", cudaGetErrorString(e));
   for (int c = 0; c < dp.count; ++c) {  // the Gaussian terms in sc_mse serve every config
@@ -1615,12 +1762,92 @@ void begin_score_stats(uis_model* m, int jobs, long long rows, const ChainPlan& 
   m->stats.frames = rows;
   m->stats.max_k = cp.max_k;
   m->stats.engine = 1;
+  m->stats.groups = 1;
   m->last_U = jobs;
+  m->last_groups = 1;
   m->last_score = true;
   m->last_score_counts = false;
   m->last_tree_spill = false;
   m->last_stream = st;
   m->stats_pending = false;
+}
+
+// Per-frame bytes of a score call's device workspace: gi (12H), the Gaussian term and block count of every frame,
+// the chain plan (an offset and a row), and the fp32 rows at the kernel shape when the call holds them (staged host
+// rows, or a padded model's device rows).  *held: what the handle's buffers of those already hold.
+size_t score_row_bytes(const uis_model* m, bool x32, size_t* held) {
+  *held = m->gi.cap + m->sc_mse.cap + m->sc_blocks.cap + m->sc_chain_off.cap + m->sc_chain_rows.cap + (x32 ? m->x32.cap : 0);
+  return (size_t)3 * m->H * 4 + 4 + 4 + 8 + 8 + (x32 ? (size_t)m->D * 4 : 0);
+}
+
+// Bytes of a score call over U utterances and C configs that do not grow with the frames: the chain kernel's slot
+// pools at its largest grid, the offsets and the totals.
+size_t score_fixed_bytes(const uis_model* m, int U, int C) {
+  int CP = 0;
+  uis::with_shape(uis::AllShapes{}, m->H, m->D, [&](auto s) { CP = uis::beam_cp<decltype(s)::H>(); });
+  return (size_t)m->num_sms * CP * 2 * (m->D + (size_t)m->depth * m->H) * 4 + (size_t)(U + 1) * 8 + (size_t)U * C * 4;
+}
+
+// Chain plans of the groups `cuts` of a host-planned score call (offsets `off`, canonical labels `lab` of every row),
+// each over its group's own rows.  Made before any group runs, so that a bad label fails the call before it enqueues.
+int plan_groups(const int32_t* lab, const int64_t* off, const std::vector<int>& cuts, std::vector<ChainPlan>* plans) {
+  plans->resize(cuts.size() - 1);
+  for (size_t g = 0; g + 1 < cuts.size(); ++g) {
+    const std::vector<int64_t> goff = group_offsets(off, cuts[g], cuts[g + 1]);
+    if (int rc = plan_chains(lab + off[cuts[g]], goff.data(), cuts[g + 1] - cuts[g], &(*plans)[g], cuts[g])) return rc;
+  }
+  return 0;
+}
+
+// The stats of a device score call run in groups: `total` of its groups, whose `ran` groups that launched kernels
+// left their counters, events and device plans' counts for collect().
+void finish_groups(uis_model* m, const uis_stats& total, int jobs, int ran) {
+  m->stats = total;
+  m->last_U = jobs;
+  m->last_groups = ran;
+  m->stats_pending = ran > 0;
+}
+
+// Utterances [u0, u0 + U) of a host score call of U_all utterances: offsets `off` and labels `lab` rebased to the
+// group, chains `cp`.  Staged, scored and copied back on their own: totals to scores_out[c][u0 + u] (scores_out points
+// at column u0 of the call's [C][U_all]), increments to frame_out[u][c][..].  Leaves the group's stats in m->stats.
+int score_host_group(uis_model* m, const double* const* seqs, int U, const int64_t* off, const int32_t* lab,
+                     const ChainPlan& cp, float* scores_out, float* const* frame_out, int U_all, cudaStream_t st,
+                     const DecodeParams& dp) {
+  const int C = dp.count;
+  const long long rows = off[U];
+  begin_score_stats(m, U * C, rows, cp, st);
+  if (rows == 0) return 0;  // (the totals are 0 already)
+  int n_chunks = 0;
+  bool staged = false;
+  if (int rc = stage_host_rows(m, seqs, U, off, (size_t)rows, st, &n_chunks, &staged)) return rc;
+  if (int rc = m->labels.ensure((size_t)rows * 4)) return rc;
+  CU(cudaMemcpyAsync(m->labels.p, lab, (size_t)rows * 4, cudaMemcpyHostToDevice, st));
+  if (int rc = m->sc_out.ensure(((size_t)U + (frame_out ? (size_t)rows : 0)) * C * 4)) return rc;
+  float* dev_frames = frame_out ? m->sc_out.as<float>() + (size_t)U * C : nullptr;
+  if (int rc = run_score(m, m->x32.as<float>(), off, U, &cp, m->labels.as<int32_t>(), m->sc_out.as<float>(),
+                         dev_frames, st, /*gi_ready=*/true, dp))
+    return rc;
+  m->stats.kernel_launches += 2 * (int64_t)n_chunks;
+  m->stats.chunks = n_chunks;
+  m->stats.staged = staged ? 1 : 0;
+  CU(cudaMemcpy2DAsync(scores_out, (size_t)U_all * 4, m->sc_out.p, (size_t)U * 4, (size_t)U * 4, C,
+                       cudaMemcpyDeviceToHost, st));
+  if (frame_out) {
+    std::vector<float> inc((size_t)rows * C);
+    CU(cudaMemcpyAsync(inc.data(), dev_frames, (size_t)rows * C * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    for (int c = 0; c < C; ++c)  // config c's increments -> row c of the caller's [C][n] buffers
+      for (int u = 0; u < U; ++u)
+        if (off[u + 1] > off[u])
+          std::memcpy(frame_out[u] + (size_t)c * (off[u + 1] - off[u]), inc.data() + (size_t)c * rows + off[u],
+                      (size_t)(off[u + 1] - off[u]) * 4);
+  }
+  CU(cudaStreamSynchronize(st));
+  if (int rc = collect(m)) return rc;
+  CU(cudaEventElapsedTime(&m->stats.h2d_ms, m->ev_h2d[0], m->ev_h2d[1]));
+  CU(cudaEventElapsedTime(&m->stats.pipeline_ms, m->ev_pipe, m->ev[1]));
+  return 0;
 }
 
 int score_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_frames, int U,
@@ -1639,40 +1866,31 @@ int score_host_impl(uis_model* m, const double* const* seqs, const int64_t* n_fr
   std::vector<int32_t> lab((size_t)rows);
   for (int u = 0; u < U; ++u)
     if (n_frames[u] > 0) std::memcpy(lab.data() + off[u], labels[u], (size_t)n_frames[u] * 4);
-  ChainPlan cp;
-  if (int rc = plan_chains(lab.data(), off.data(), U, &cp)) return rc;
-  begin_score_stats(m, U * C, rows, cp, st);
+  // Memory: per frame the score workspace, the staged fp32 rows, the labels and the per-frame outputs when asked
+  size_t held = 0;
+  const size_t per_row = score_row_bytes(m, true, &held) + 4 + (frame_out ? (size_t)4 * C : 0);
+  held += m->labels.cap + m->sc_out.cap + m->x64.cap;
+  const size_t fixed = score_fixed_bytes(m, U, C) +
+                       (size_t)uis_model::kSlots * staging_chunk_rows(m->D_user) * m->D_user * 8;
+  size_t max_rows = 0;
+  if (rows > 0)
+    if (int rc = row_budget(per_row, fixed, held, &max_rows)) return rc;
+  const std::vector<int> cuts = rows > 0 ? cut_groups(off.data(), U, max_rows) : std::vector<int>{0, U};
+  std::vector<ChainPlan> plans;
+  if (int rc = plan_groups(lab.data(), off.data(), cuts, &plans)) return rc;
   std::fill(scores_out, scores_out + (size_t)U * C, 0.f);  // empty utterances score 0
-  if (rows == 0) return 0;
-  int n_chunks = 0;
-  bool staged = false;
-  if (int rc = stage_host_rows(m, seqs, U, off.data(), (size_t)rows, st, &n_chunks, &staged)) return rc;
-  if (int rc = m->labels.ensure((size_t)rows * 4)) return rc;
-  CU(cudaMemcpyAsync(m->labels.p, lab.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, st));
-  if (int rc = m->sc_out.ensure(((size_t)U + (frame_out ? (size_t)rows : 0)) * C * 4)) return rc;
-  float* dev_frames = frame_out ? m->sc_out.as<float>() + (size_t)U * C : nullptr;
-  if (int rc = run_score(m, m->x32.as<float>(), off.data(), U, &cp, m->labels.as<int32_t>(), m->sc_out.as<float>(),
-                         dev_frames, st, /*gi_ready=*/true, dp))
-    return rc;
-  m->stats.kernel_launches += 2 * (int64_t)n_chunks;
-  m->stats.chunks = n_chunks;
-  m->stats.staged = staged ? 1 : 0;
-  CU(cudaMemcpyAsync(scores_out, m->sc_out.p, (size_t)U * C * 4, cudaMemcpyDeviceToHost, st));
-  if (frame_out) {
-    lab.resize((size_t)rows * C);  // (lab: spent)
-    CU(cudaMemcpyAsync(lab.data(), dev_frames, (size_t)rows * C * 4, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    for (int c = 0; c < C; ++c)  // config c's increments -> row c of the caller's [C][n_frames[u]] buffers
-      for (int u = 0; u < U; ++u)
-        if (n_frames[u] > 0)
-          std::memcpy(frame_out[u] + (size_t)c * n_frames[u], lab.data() + (size_t)c * rows + off[u], (size_t)n_frames[u] * 4);
+  const int G = (int)plans.size();
+  uis_stats total{};
+  for (int g = 0; g < G; ++g) {
+    const int u0 = cuts[g], u1 = cuts[g + 1];
+    const std::vector<int64_t> goff = group_offsets(off.data(), u0, u1);
+    if (int rc = score_host_group(m, seqs + u0, u1 - u0, goff.data(), lab.data() + off[u0], plans[g], scores_out + u0,
+                                  frame_out ? frame_out + u0 : nullptr, U, st, dp))
+      return rc;
+    add_stats(&total, m->stats);
   }
-  CU(cudaStreamSynchronize(st));
-  if (int rc = collect(m)) return rc;
-  CU(cudaEventElapsedTime(&m->stats.h2d_ms, m->ev_h2d[0], m->ev_h2d[1]));
-  CU(cudaEventElapsedTime(&m->stats.pipeline_ms, m->ev_pipe, m->ev[1]));
-  m->stats.groups = 1;
-  m->stats.host_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+  if (G > 1) m->stats = total;
+  if (rows > 0) m->stats.host_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
   return 0;
 }
 
@@ -1687,6 +1905,86 @@ int score_host(uis_model* m, const double* const* seqs, const int64_t* n_frames,
   const int rc = score_host_impl(m, seqs, n_frames, U, labels, scores_out, frame_out, st, dp);
   if (rc != 0 && rc != UIS_ERR_INVALID) drain_after_failure(m, st);
   return rc;
+}
+
+// A device-buffer score call in the groups `cuts` (cut_groups), one after the other on `st`.  Group [u0, u1) reads
+// rows off[u0].. of x_dev (padded into the handle's x32 for a padded model: 16-byte aligned either way, as in
+// predict_device_groups), labels_dev and ids_dev, and its reduce kernels write columns u0.. of the caller's [C][U]
+// totals and [C][rows] increments in place (ScoreParams' row strides).  ids_dev: the chains are planned on the device,
+// group by group, with nothing read back (each group's counts in its own slot of sc_counts); else `lab` holds the
+// canonical labels of every row, read back by the caller, and the chains are planned here.
+int score_device_groups(uis_model* m, const float* x_dev, const int64_t* off, int U, const std::vector<int32_t>& lab,
+                        const int32_t* labels_dev, float* scores_dev, float* frame_dev, cudaStream_t st,
+                        const DecodeParams& dp, const std::vector<int>& cuts, const int64_t* ids_dev = nullptr,
+                        int32_t* labels_out = nullptr) {
+  const int C = dp.count, G = (int)cuts.size() - 1;
+  const long long rows = off[U];
+  std::vector<ChainPlan> plans;
+  if (!ids_dev)
+    if (int rc = plan_groups(lab.data(), off, cuts, &plans)) return rc;
+  // the handle's buffers, sized for the largest group before the first is enqueued: growing one later would free it
+  // under the groups still in flight, which waits for them
+  long long max_rows = 0;
+  int max_u = 0;
+  size_t plan_bytes = 0;
+  for (int g = 0; g < G; ++g) {
+    const long long r = off[cuts[g + 1]] - off[cuts[g]];
+    max_rows = std::max(max_rows, r);
+    max_u = std::max(max_u, cuts[g + 1] - cuts[g]);
+    if (ids_dev && r > 0) plan_bytes = std::max(plan_bytes, uis::score_plan_bytes(r, cuts[g + 1] - cuts[g]));
+  }
+  const size_t R = (size_t)max_rows;
+  if (int rc = m->gi.ensure(R * 3 * m->H * sizeof(float))) return rc;
+  if (int rc = m->sc_mse.ensure(R * sizeof(float))) return rc;
+  if (int rc = m->sc_blocks.ensure(R * sizeof(int))) return rc;
+  if (int rc = m->row_off.ensure((size_t)(max_u + 1) * sizeof(long long))) return rc;
+  if (m->D != m->D_user)
+    if (int rc = m->x32.ensure(R * m->D * 4)) return rc;
+  if (ids_dev) {
+    if (int rc = m->labels.ensure(R * 4)) return rc;
+    if (int rc = m->sc_chain_off.ensure((R + 1) * sizeof(long long))) return rc;
+    if (int rc = m->sc_chain_rows.ensure(R * sizeof(long long))) return rc;
+    if (int rc = m->sc_counts.ensure((size_t)4 * G * sizeof(int))) return rc;
+    if (int rc = m->sc_plan.ensure(plan_bytes)) return rc;
+  }
+  uis_stats total{};
+  int ran = 0;
+  for (int g = 0; g < G; ++g) {
+    const int u0 = cuts[g], u1 = cuts[g + 1], Ug = u1 - u0;
+    const std::vector<int64_t> goff = group_offsets(off, u0, u1);
+    const long long rg = goff[Ug];
+    begin_score_stats(m, Ug * C, rg, ids_dev ? ChainPlan{} : plans[g], st);
+    if (rg == 0) {  // empty utterances score 0
+      CU(cudaMemset2DAsync(scores_dev + u0, (size_t)U * 4, 0, (size_t)Ug * 4, C, st));
+      add_stats(&total, m->stats);
+      continue;
+    }
+    const float* gx = x_dev + (size_t)off[u0] * m->D_user;
+    if (int rc = pad_to_kernel_d(m, &gx, (size_t)rg, st)) return rc;
+    float* gframe = frame_dev ? frame_dev + off[u0] : nullptr;
+    const Group grp{ran, 0, rows, U};
+    if (ids_dev) {
+      std::vector<long long> off_ll(goff.begin(), goff.end());
+      CU(cudaMemcpyAsync(m->row_off.p, off_ll.data(), (Ug + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+      CU(uis::score_plan(reinterpret_cast<const long long*>(ids_dev + off[u0]), m->row_off.as<long long>(), Ug, rg,
+                         m->sc_plan.p, m->sc_plan.cap, m->labels.as<int>(), labels_out ? labels_out + off[u0] : nullptr,
+                         m->sc_chain_off.as<long long>(), m->sc_chain_rows.as<long long>(),
+                         m->sc_counts.as<int>() + 4 * ran, m->num_sms, st));
+      m->last_score_counts = true;
+      if (int rc = run_score(m, gx, goff.data(), Ug, nullptr, m->labels.as<int32_t>(), scores_dev + u0, gframe, st,
+                             /*gi_ready=*/false, dp, grp))
+        return rc;
+      m->stats.kernel_launches += uis::kScorePlanLaunches;
+    } else if (int rc = run_score(m, gx, goff.data(), Ug, &plans[g], labels_dev + off[u0], scores_dev + u0, gframe, st,
+                                  /*gi_ready=*/false, dp, grp)) {
+      return rc;
+    }
+    ++ran;
+    add_stats(&total, m->stats);
+  }
+  finish_groups(m, total, U * C, ran);
+  m->last_score_counts = ids_dev != nullptr;  // (an empty group's begin_score_stats cleared it)
+  return 0;
 }
 
 int score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets, int U, const int32_t* labels_dev,
@@ -1707,6 +2005,12 @@ int score_device(uis_model* m, const float* x_dev, const int64_t* frame_offsets,
     CU(cudaMemcpyAsync(lab.data(), labels_dev, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
   }
+  size_t held = 0, max_rows = 0;
+  const size_t per_row = score_row_bytes(m, m->D != m->D_user, &held);
+  if (rows > 0)
+    if (int rc = row_budget(per_row, score_fixed_bytes(m, U, dp.count), held, &max_rows)) return rc;
+  const std::vector<int> cuts = rows > 0 ? cut_groups(frame_offsets, U, max_rows) : std::vector<int>{0, U};
+  if (cuts.size() > 2) return score_device_groups(m, x_dev, frame_offsets, U, lab, labels_dev, scores_dev, frame_dev, st, dp, cuts);
   ChainPlan cp;
   if (int rc = plan_chains(lab.data(), frame_offsets, U, &cp)) return rc;
   begin_score_stats(m, U * dp.count, rows, cp, st);
@@ -1743,6 +2047,16 @@ int score_device_ids(uis_model* m, const float* x_dev, const int64_t* frame_offs
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CallOrder order(m, st);
   CU(order.status);
+  if (rows > 0) {  // per frame: the score workspace, the canonical labels and the device plan's scratch
+    size_t held = 0, max_rows = 0;
+    const size_t per_row = score_row_bytes(m, m->D != m->D_user, &held) + 4 + uis::score_plan_bytes(rows, U) / (size_t)rows + 1;
+    held += m->labels.cap + m->sc_plan.cap;
+    if (int rc = row_budget(per_row, score_fixed_bytes(m, U, dp.count), held, &max_rows)) return rc;
+    const std::vector<int> cuts = cut_groups(frame_offsets, U, max_rows);
+    if (cuts.size() > 2)
+      return score_device_groups(m, x_dev, frame_offsets, U, {}, nullptr, scores_dev, frame_dev, st, dp, cuts, ids_dev,
+                                 labels_dev);
+  }
   begin_score_stats(m, U * dp.count, rows, ChainPlan{}, st);
   if (U == 0) return 0;
   if (rows == 0) {

@@ -209,14 +209,14 @@ __global__ void __launch_bounds__(256) score_first_kernel(const __grid_constant_
 }
 
 // One thread per utterance: loss_t = fl32(f64(mse_t) - pen_t) and S = fl32(S + loss_t) in frame order, with pen_t the
-// beam kernel's transition / ddCRP term (phase P1a) of the trace so far under config `cfg`, whose totals go to
-// scores[cfg][U] and increments to frame_out[cfg][rows].
+// beam kernel's transition / ddCRP term (phase P1a) of the trace so far under config `cfg`, whose totals go to row
+// cfg of scores and increments to row cfg of frame_out.
 __global__ void __launch_bounds__(128) score_reduce_kernel(const __grid_constant__ ScoreParams sp, int cfg) {
   const BeamParams& p = sp.b;
   const int u = blockIdx.x * blockDim.x + threadIdx.x;
   if (u >= p.U) return;
   const JobLogs lg = job_logs(p, cfg);
-  float* frame_out = sp.frame_out ? sp.frame_out + (size_t)cfg * p.row_off[p.U] : nullptr;
+  float* frame_out = sp.frame_out ? sp.frame_out + (size_t)cfg * sp.frame_stride : nullptr;
   const long long r0 = p.row_off[u], r1 = p.row_off[u + 1];
   int* blk = sp.blocks + r0;  // block counts of the utterance's clusters (K <= frames)
   int K = 0, last = -1, tot = 0;
@@ -236,7 +236,7 @@ __global__ void __launch_bounds__(128) score_reduce_kernel(const __grid_constant
     tot += moved ? 1 : 0;
     last = c;
   }
-  sp.scores[(size_t)cfg * p.U + u] = S;
+  sp.scores[(size_t)cfg * sp.score_stride + u] = S;
 }
 
 unsigned score_smem(int H, int D) {

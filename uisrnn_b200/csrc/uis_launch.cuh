@@ -70,8 +70,12 @@ struct ScoreParams {
   int queued;                   // the first `queued` chains (length >= 2) run through the chain kernel
   float* mse;                   // [rows] Gaussian term of a frame against its cluster's mean before that frame
   const int* labels;            // [rows] canonical labels
-  float* scores;                // [configs][U]    neg_likelihood
-  float* frame_out;             // [configs][rows] per-frame increments (may be null)
+  float* scores;                // [configs][score_stride]  neg_likelihood of utterance u at [config][u]
+  float* frame_out;             // [configs][frame_stride]  per-frame increments of row r at [config][r] (may be null)
+  // Row strides of the two outputs: U and rows for a whole call; a group of a call scored in groups of utterances
+  // writes its columns of the call's arrays, whose rows are the whole call's U and rows
+  int score_stride;
+  long long frame_stride;
   int* blocks;                  // [rows] reduce kernel scratch: block counts of utterance u's clusters at row_off[u]
   // A plan made on the device (score_plan): {chains, queued, max_k} in device memory, written by the plan kernels
   // earlier on the stream.  The kernels read `chains` / `queued` from here; the two fields above then only bound the

@@ -632,7 +632,10 @@ class UISRNN:
 
   def predict(self, test_sequences, args, *, max_speakers=None, min_speakers=None, n_best=None, decode_params=None):
     """Labels for one sequence (ndarray -> list of ints) or many (list -> list of lists)
-    (uisrnn.py:564-590).  On CUDA a list is decoded by a single native call.
+    (uisrnn.py:564-590).  On CUDA a list is decoded by a single native call; a list whose workspace does not fit
+    the free device memory is decoded inside that call in groups of whole utterances, one after the other, with the
+    results of one group (UISRNN_B200_MAX_ROWS sets the frames per group).  This holds for tensors, n_best, bounds and
+    decode_params too.
 
     Speaker bounds (not in the reference): `max_speakers` / `min_speakers` is an int for every utterance or one
     value per utterance, 0 or None = no bound.  A hypothesis never holds more than max_speakers clusters, so every
@@ -679,7 +682,8 @@ class UISRNN:
     renaming: they are mapped to 0, 1, 2, ... in order of first appearance.  test_iteration is not applied: the
     sequence is scored once, as given (tile both the sequence and its labels to score a tiled decode).  An empty
     sequence scores 0.  With per_frame=True every utterance gives a `FrameScores(total, increments)` instead.  On a
-    CUDA device a list is scored by one native call.
+    CUDA device a list is scored by one native call, in groups of whole utterances when it does not fit the device at
+    once (as `predict`; the scores are those of one group, bit for bit).
 
     With `decode_params` (a non-empty sequence of (crp_alpha, transition_bias) pairs, validated as in `predict`) the
     result is a list with one entry per pair, each being what this call returns for a model with that pair.  On a CUDA
